@@ -66,7 +66,7 @@ class A3DError(RuntimeError):
 
 
 def load(require_gpu: bool = True) -> C.CDLL:
-    """dlopen liba3d.so; with require_gpu also run a3d_init() (sm_100 + TMA entry points)."""
+    """dlopen liba3d.so; with require_gpu also run a3d_init() (sm_90 + TMA entry points)."""
     global _lib, _inited
     if _lib is None:
         if not os.path.exists(LIB_PATH):
@@ -80,7 +80,7 @@ def load(require_gpu: bool = True) -> C.CDLL:
         _lib = lib
     if require_gpu and not _inited:
         if not torch.cuda.is_available():
-            raise A3DError("animate3d_b200 needs a CUDA device (sm_100a); none is visible and there is no fallback")
+            raise A3DError("animate3d_b200 needs a CUDA device (sm_90a); none is visible and there is no fallback")
         check(_lib.a3d_init())
         _inited = True
     return _lib

@@ -1,6 +1,6 @@
-"""Build liba3d.so (sm_100a only) in-tree with nvcc.  `python -m animate3d_b200.build [--force]`.
+"""Build liba3d.so (sm_90a only) in-tree with nvcc.  `python -m animate3d_b200.build [--force]`.
 
-The .so is git-ignored but travels to the GPU box with the gpurun snapshot."""
+The .so and the object files are build products (git-ignored); the package loads the library from next to this file."""
 from __future__ import annotations
 
 import hashlib
@@ -17,7 +17,8 @@ SOURCES = ["a3d_api.cu", "a3d_gemm.cu", "a3d_attn.cu", "a3d_ops.cu", "a3d_raster
 # index-defining rasterizer arithmetic must not be contracted into FMAs (bit parity with oracle/raster_oracle.py)
 EXTRA = {"a3d_raster_pre.cu": ["--fmad=false"]}
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC",
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
+FLAGS = [*ARCH, "-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC",
          "--expt-relaxed-constexpr"]
 
 
@@ -55,7 +56,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
 
     with ThreadPoolExecutor(max_workers=len(SOURCES)) as ex:
         objs = list(ex.map(compile_one, SOURCES))
-    r = subprocess.run([NVCC, "-shared", "-o", OUT, *objs, "-gencode", "arch=compute_100a,code=sm_100a"],
+    r = subprocess.run([NVCC, "-shared", "-o", OUT, *objs, *ARCH],
                        capture_output=True, text=True)
     if r.returncode != 0:
         raise RuntimeError(f"link failed:\n{r.stdout}\n{r.stderr}")

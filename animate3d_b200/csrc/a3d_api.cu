@@ -79,7 +79,7 @@ int a3d_init(void) {
   int major = 0, minor = 0;
   cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev);
   cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, dev);
-  if (major != 10) return a3d::fail(A3D_ENOTSUP, "liba3d needs an sm_100 device, found sm_%d%d", major, minor);
+  if (major != 9 || minor != 0) return a3d::fail(A3D_ENOTSUP, "liba3d needs an sm_90 device, found sm_%d%d", major, minor);
   if (!a3d::get_encode_fn()) return a3d::fail(A3D_ECUDA, "cuTensorMapEncodeTiled entry point unavailable");
   a3d::sm_count();
   return A3D_OK;

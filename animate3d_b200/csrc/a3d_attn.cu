@@ -1,13 +1,14 @@
-// a3d_attention: O = softmax(scale * Q K^T) V, flash-style, on tcgen05 tensor cores with TMEM accumulators.
+// a3d_attention: O = softmax(scale * Q K^T) V, flash-style, on Hopper tensor cores (wgmma).
 //
-//   one CTA = one 128-row query tile of one (batch, head); 6 warps:
-//     warp 0      TMA producer (Q once, K/V tiles through a ring of smem stages; 128B-swizzled boxes read straight out
-//                 of the projection GEMM's output through rank-5 strided views -> the reference's
+//   one CTA = one 128-row query tile of one (batch, head); 9 warps:
+//     warp 8      TMA producer (Q once, K/V tiles of 64 keys through a ring of smem stages; 128B-swizzled boxes read straight
+//                 out of the projection GEMM's output through rank-5 strided views -> the reference's
 //                 "(b n f) l c -> (b f) (n l) c" regroupings and frame-0 K/V broadcasts never materialise)
-//     warp 1      tcgen05.mma issuer:  S = Q K^T  (K-major A and B),  O += P V  (P K-major from smem, V MN-major)
-//     warps 2..5  softmax: one thread per query row reads S from TMEM, keeps the running max in the log2 domain, writes
-//                 fp16 P into swizzled smem, rescales O in TMEM only when the max moved by more than kRescaleLog2
-//   The row sum is not computed by the softmax warps: V carries a column of ones at index d (placed there by the
+//     warps 0..7  two consumer warpgroups of 64 query rows each:  S = Q K^T (wgmma, both operands K-major in smem, fp32 in
+//                 registers), online softmax in registers, O += P V (wgmma with P as the register A operand, V MN-major)
+//   Single-pass ("stale stabiliser") softmax: the running row maximum of the previous key steps stays the exponent offset
+//   and O is rescaled only when a later step raises it by more than kRescaleLog2 (P then stays below 2^kRescaleLog2, far
+//   inside fp16).  The row sum is not computed separately: V carries a column of ones at index d (placed there by the
 //   projection epilogue), so O[:, d] accumulates sum(P) in fp32 alongside the PV product.
 //
 // Replaces xformers.ops.memory_efficient_attention at animatediff/models/attention_processor.py:103,233,268,405,416,656,691.
@@ -15,12 +16,13 @@
 
 #include "a3d_common.cuh"
 #include "a3d_host.cuh"
+#include "a3d_wgmma.cuh"
 
 namespace a3d {
 
 struct AttnDev {
   int q_tiles, kv_tiles;
-  int rows_q, rows_k;            // valid rows per q tile / kv tile (<= 128)
+  int rows_q, rows_k;            // valid rows per q tile (<= 128) / in the LAST kv tile (<= 64)
   int heads;
   int q_t1, q_box1, q_box2, q_e3;
   int k_t1, k_box1, k_box2, k_e3, kv_div, kv_i3_zero;
@@ -30,1099 +32,220 @@ struct AttnDev {
   int64_t os1, os2, os3, os4;
   int accumulate;
   float out_scale;
-  int early_test;            // head-dim-40 kernel: non-blocking barrier tests one step ahead (see the step loop)
-  int late_pfree;            // head-dim-40 kernel, TS: no explicit "P buffer consumed" wait (implied by s_full, see the step loop)
-  unsigned long long* dbg;   // debug (null in production): dbg[0] counts (warp, step) pairs that took the lazy-rescale branch;
-                             // dbg[8 + (w*32 + j)*8 + k]: clock64 timeline of 4 softmax warps of CTA (0,0,0) (head-dim-40 kernel)
+  unsigned long long* dbg;   // debug (null in production): dbg[0] counts (warp, step) pairs that took the lazy-rescale branch
 };
 
 constexpr float kRescaleLog2 = 8.0f;
+constexpr int kAttnThreads = 288;
 
 template <int D>
 struct AttnCfg {
   static constexpr int kDqk = (D + 15) / 16 * 16;        // 48 / 80 / 160
   static constexpr int kDv = (D + 1 + 15) / 16 * 16;     // 48 / 96 / 176
-  static constexpr int kQBoxes = (kDqk + 63) / 64;       // 1 / 2 / 3
-  static constexpr int kVBoxes = (kDv + 63) / 64;        // 1 / 2 / 3
-  static constexpr int kStages = (D == 160) ? 1 : 2;
-  static constexpr int kBox = 128 * 128;                 // bytes of one 128-row x 64-col fp16 box
-  static constexpr int kSmemQ = kQBoxes * kBox;
-  static constexpr int kSmemK = kStages * kQBoxes * kBox;
-  static constexpr int kSmemV = kStages * kVBoxes * kBox;
-  static constexpr int kSmemP = 2 * kBox;
-  static constexpr int kSmemBytes = kSmemQ + kSmemK + kSmemV + kSmemP + 1024 + 256;
-  static constexpr int kTmemCols = (128 + kDv <= 256) ? 256 : 512;
+  static constexpr int kQB = (kDqk + 63) / 64;           // 64-column boxes per Q / K row: 1 / 2 / 3
+  static constexpr int kVB = (kDv + 63) / 64;            // 1 / 2 / 3
+  static constexpr int kStages = (D == 160) ? 3 : 4;
+  static constexpr int kQBox = 128 * 128;                // 128 rows x 64 cols fp16
+  static constexpr int kKVBox = 64 * 128;                // 64 keys x 64 cols fp16
+  static constexpr int kSmemQ = kQB * kQBox;
+  static constexpr int kSmemK = kStages * kQB * kKVBox;
+  static constexpr int kSmemV = kStages * kVB * kKVBox;
+  static constexpr int kSmemBytes = kSmemQ + kSmemK + kSmemV + 1024 + 256;
   static constexpr int kMinBlocks = (kSmemBytes <= 113 * 1024) ? 2 : 1;
+  static_assert(kSmemBytes <= 227 * 1024, "shared memory budget");
 };
 
+template <int N>
+__device__ __forceinline__ void wgmma_pv(float (&o)[N / 2], const uint32_t (&a)[4], uint64_t bdesc, uint32_t acc) {
+  if constexpr (N == 48) wgmma_rs_n48<1>(o, a, bdesc, acc);
+  else if constexpr (N == 96) wgmma_rs_n96<1>(o, a, bdesc, acc);
+  else wgmma_rs_n176<1>(o, a, bdesc, acc);
+}
+
 template <int D>
-__global__ void __launch_bounds__(192, AttnCfg<D>::kMinBlocks)
+__global__ void __launch_bounds__(kAttnThreads, AttnCfg<D>::kMinBlocks)
 attn_tc_kernel(const AttnDev p, const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapK,
                const __grid_constant__ CUtensorMap mapV) {
   using Cfg = AttnCfg<D>;
+  constexpr int S = Cfg::kStages;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sQ = smem;
   uint8_t* sK = sQ + Cfg::kSmemQ;
   uint8_t* sV = sK + Cfg::kSmemK;
-  uint8_t* sP = sV + Cfg::kSmemV;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sP + Cfg::kSmemP);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sV + Cfg::kSmemV);
   uint64_t* q_full = bars;
-  uint64_t* k_full = bars + 1;                     // [kStages]
-  uint64_t* v_full = k_full + Cfg::kStages;        // [kStages]
-  uint64_t* kv_empty = v_full + Cfg::kStages;      // [kStages]
-  uint64_t* s_full = kv_empty + Cfg::kStages;
-  uint64_t* p_full = s_full + 1;
-  uint64_t* o_full = p_full + 1;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(o_full + 1);
+  uint64_t* k_full = bars + 1;          // [S]
+  uint64_t* v_full = k_full + S;        // [S]
+  uint64_t* kv_empty = v_full + S;      // [S]
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-
   const int qt = blockIdx.x;
   const int head = blockIdx.y;
   const int qb = blockIdx.z;
+  const int n = p.kv_tiles;
+  const int rows_tile = p.k_box1 * p.k_box2;
 
-  if (p.rows_q < 128 || p.rows_k < 128) {
+  if (p.rows_q < 128 || rows_tile < 64) {
     // partially filled tiles: rows TMA never writes must read as zeros (0 * garbage could be NaN in P V)
     uint4* z = reinterpret_cast<uint4*>(sQ);
     const int n16 = (Cfg::kSmemQ + Cfg::kSmemK + Cfg::kSmemV) / 16;
     for (int i = threadIdx.x; i < n16; i += blockDim.x) z[i] = make_uint4(0, 0, 0, 0);
     fence_proxy_async_smem();
   }
-  if (warp == 0 && lane == 0) {
+  if (warp == 8 && lane == 0) {
     tma_prefetch_desc(&mapQ);
     tma_prefetch_desc(&mapK);
     tma_prefetch_desc(&mapV);
     mbar_init(q_full, 1);
-    for (int i = 0; i < Cfg::kStages; ++i) {
+    for (int i = 0; i < S; ++i) {
       mbar_init(&k_full[i], 1);
       mbar_init(&v_full[i], 1);
-      mbar_init(&kv_empty[i], 1);
+      mbar_init(&kv_empty[i], 8);   // one arrive per consumer warp
     }
-    mbar_init(s_full, 1);
-    mbar_init(p_full, 4);
-    mbar_init(o_full, 1);
     mbar_fence_init();
   }
-  if (warp == 1) tmem_alloc<Cfg::kTmemCols>(tmem_slot);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t tmem_S = tmem_base;
-  const uint32_t tmem_O = tmem_base + 128;
 
-  // query / key coordinates
   const int q_i1 = (qt % p.q_t1) * p.q_box1;
   const int q_i2 = (qt / p.q_t1) * p.q_box2;
   const int q_i3 = qb % p.q_e3;
   const int q_i4 = qb / p.q_e3;
 
-  if (warp == 0) {
+  if (warp == 8) {
+    // ------------------------------------------------------------------ TMA producer (one thread)
     if (lane == 0) {
       const int kb = qb / p.kv_div;
       const int k_i3 = p.kv_i3_zero ? 0 : (kb % p.k_e3);
       const int k_i4 = kb / p.k_e3;
-      mbar_expect_tx(q_full, p.q_box_bytes * Cfg::kQBoxes);
+      mbar_expect_tx(q_full, p.q_box_bytes * Cfg::kQB);
 #pragma unroll
-      for (int b = 0; b < Cfg::kQBoxes; ++b)
-        tma_load_5d(sQ + b * Cfg::kBox, &mapQ, q_full, head * Cfg::kDqk + b * 64, q_i1, q_i2, q_i3, q_i4);
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int j = 0; j < p.kv_tiles; ++j) {
-        const int k_i1 = (j % p.k_t1) * p.k_box1;
-        const int k_i2 = (j / p.k_t1) * p.k_box2;
-        mbar_wait(&kv_empty[stage], phase ^ 1);
-        mbar_expect_tx(&k_full[stage], p.k_box_bytes * Cfg::kQBoxes);
+      for (int b = 0; b < Cfg::kQB; ++b)
+        tma_load_5d(sQ + b * Cfg::kQBox, &mapQ, q_full, head * Cfg::kDqk + b * 64, q_i1, q_i2, q_i3, q_i4);
+      for (int j = 0; j < n; ++j) {
+        const int st = j % S;
+        const int k_i1 = (j % p.k_t1) * p.k_box1, k_i2 = (j / p.k_t1) * p.k_box2;
+        mbar_wait(&kv_empty[st], ((j / S) & 1) ^ 1);
+        mbar_expect_tx(&k_full[st], p.k_box_bytes * Cfg::kQB);
 #pragma unroll
-        for (int b = 0; b < Cfg::kQBoxes; ++b)
-          tma_load_5d(sK + (stage * Cfg::kQBoxes + b) * Cfg::kBox, &mapK, &k_full[stage], head * Cfg::kDqk + b * 64, k_i1,
-                      k_i2, k_i3, k_i4);
-        mbar_expect_tx(&v_full[stage], p.k_box_bytes * Cfg::kVBoxes);
+        for (int b = 0; b < Cfg::kQB; ++b)
+          tma_load_5d(sK + (st * Cfg::kQB + b) * Cfg::kKVBox, &mapK, &k_full[st], head * Cfg::kDqk + b * 64, k_i1, k_i2, k_i3,
+                      k_i4);
+        mbar_expect_tx(&v_full[st], p.k_box_bytes * Cfg::kVB);
 #pragma unroll
-        for (int b = 0; b < Cfg::kVBoxes; ++b)
-          tma_load_5d(sV + (stage * Cfg::kVBoxes + b) * Cfg::kBox, &mapV, &v_full[stage], head * Cfg::kDv + b * 64, k_i1,
-                      k_i2, k_i3, k_i4);
-        if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
+        for (int b = 0; b < Cfg::kVB; ++b)
+          tma_load_5d(sV + (st * Cfg::kVB + b) * Cfg::kKVBox, &mapV, &v_full[st], head * Cfg::kDv + b * 64, k_i1, k_i2, k_i3,
+                      k_i4);
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      constexpr uint32_t idesc_qk = make_idesc_f16(128, 128, false, false);
-      constexpr uint32_t idesc_pv = make_idesc_f16(128, Cfg::kDv, false, true);
-      mbar_wait(q_full, 0);
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int j = 0; j < p.kv_tiles; ++j) {
-        // ---- S = Q K^T
-        mbar_wait(&k_full[stage], phase);
-        tc_fence_after();
+    return;
+  }
+
+  // -------------------------------------------------------------------- consumers: warpgroup wg owns query rows [64 wg, 64 wg + 64)
+  // thread (warp w, lane 4 g + t) holds rows r_lo = 16 (w % 4) + g and r_hi = r_lo + 8 of its warpgroup; score / output
+  // columns 8 jj + 2 t, +1 (the wgmma accumulator layout)
+  const int wg = warp >> 2;
+  const int g = lane >> 2, t = lane & 3;
+  float s[32];
+  float o[Cfg::kDv / 2];
 #pragma unroll
-        for (int kk = 0; kk < Cfg::kDqk / 16; ++kk) {
-          const uint64_t adesc = make_smem_desc_sw128(smem_u32(sQ + (kk / 4) * Cfg::kBox) + (kk % 4) * 32, 16, 1024);
-          const uint64_t bdesc = make_smem_desc_sw128(
-              smem_u32(sK + (stage * Cfg::kQBoxes + kk / 4) * Cfg::kBox) + (kk % 4) * 32, 16, 1024);
-          umma_f16(tmem_S, adesc, bdesc, idesc_qk, kk ? 1u : 0u);
-        }
-        umma_commit(s_full);
-        // ---- O += P V
-        mbar_wait(p_full, j & 1);
-        mbar_wait(&v_full[stage], phase);
-        tc_fence_after();
+  for (int i = 0; i < Cfg::kDv / 2; ++i) o[i] = 0.f;
+  float m_lo = -INFINITY, m_hi = -INFINITY;
+  const uint32_t q0 = smem_u32(sQ + wg * (64 * 128));
+  mbar_wait(q_full, 0);
+  for (int j = 0; j < n; ++j) {
+    const int st = j % S;
+    const uint32_t ph = (j / S) & 1;
+    // ---- S = Q K^T
+    mbar_wait(&k_full[st], ph);
+    wgmma_fence();
 #pragma unroll
-        for (int kk = 0; kk < 8; ++kk) {
-          const uint64_t adesc = make_smem_desc_sw128(smem_u32(sP + (kk / 4) * Cfg::kBox) + (kk % 4) * 32, 16, 1024);
-          // V is MN-major: 16 keys = two 8-row swizzle atoms (SBO = 1024 B); the next 64 value columns live one TMA
-          // box further (LBO = kBox)
-          const uint64_t bdesc = make_smem_desc_sw128(smem_u32(sV + stage * Cfg::kVBoxes * Cfg::kBox) + kk * 2048,
-                                                      Cfg::kBox, 1024);
-          umma_f16(tmem_O, adesc, bdesc, idesc_pv, (j | kk) ? 1u : 0u);
-        }
-        umma_commit(&kv_empty[stage]);
-        if (j == p.kv_tiles - 1) umma_commit(o_full);
-        if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
+    for (int kk = 0; kk < Cfg::kDqk / 16; ++kk) {
+      const uint64_t qd = make_smem_desc_sw128(q0 + (kk / 4) * Cfg::kQBox + (kk % 4) * 32, 16, 1024);
+      const uint64_t kd = make_smem_desc_sw128(smem_u32(sK + (st * Cfg::kQB + kk / 4) * Cfg::kKVBox) + (kk % 4) * 32, 16, 1024);
+      wgmma_ss_n64<0>(s, qd, kd, kk ? 1u : 0u);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence(s);
+    // ---- row maxima over the valid keys (a quad of lanes shares a row)
+    const int valid = (j == n - 1) ? p.rows_k : rows_tile;
+    float mx_lo = -INFINITY, mx_hi = -INFINITY;
+#pragma unroll
+    for (int jj = 0; jj < 8; ++jj) {
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        if (8 * jj + 2 * t + e >= valid) { s[4 * jj + e] = -INFINITY; s[4 * jj + 2 + e] = -INFINITY; }
+        mx_lo = fmaxf(mx_lo, s[4 * jj + e]);
+        mx_hi = fmaxf(mx_hi, s[4 * jj + 2 + e]);
       }
     }
-  } else {
-    const int quad = warp & 3;
-    const int r = quad * 32 + lane;                    // query row inside the tile == TMEM lane
-    const uint32_t lane_addr = (uint32_t)(quad * 32) << 16;
-    float m_run = -INFINITY;
-    for (int j = 0; j < p.kv_tiles; ++j) {
-      mbar_wait(s_full, j & 1);
-      tc_fence_after();
-      // ---- pass 1: row max over the valid keys
-      float mx = -INFINITY;
-#pragma unroll 1
-      for (int ch = 0; ch < 4; ++ch) {
-        uint32_t s[32];
-        tmem_ld32(tmem_S + lane_addr + ch * 32, s);
-        tmem_wait_ld();
-        if (p.rows_k == 128) {
-          float mx1 = -INFINITY;
 #pragma unroll
-          for (int i = 0; i < 32; i += 4) {
-            mx = fmax3(mx, __uint_as_float(s[i]), __uint_as_float(s[i + 1]));
-            mx1 = fmax3(mx1, __uint_as_float(s[i + 2]), __uint_as_float(s[i + 3]));
-          }
-          mx = fmaxf(mx, mx1);
-        } else {
-#pragma unroll
-          for (int i = 0; i < 32; ++i) if (ch * 32 + i < p.rows_k) mx = fmaxf(mx, __uint_as_float(s[i]));
-        }
-      }
-      const float m_new = fmaxf(m_run, mx * p.scale_log2);
-      if (j == 0) {
-        m_run = m_new;
-      } else if (__any_sync(0xffffffffu, m_new - m_run > kRescaleLog2)) {
-        if (p.dbg && lane == 0) atomicAdd(p.dbg, 1ull);
-        const float alpha = ex2_approx(m_run - m_new);
-#pragma unroll 1
-        for (int c = 0; c < Cfg::kDv / 16; ++c) {
-          uint32_t o[16];
-          tmem_ld16(tmem_O + lane_addr + c * 16, o);
-          tmem_wait_ld();
-#pragma unroll
-          for (int i = 0; i < 16; ++i) o[i] = __float_as_uint(__uint_as_float(o[i]) * alpha);
-          tmem_st16(tmem_O + lane_addr + c * 16, o);
-        }
-        tmem_wait_st();
-        m_run = m_new;
-      }
-      // ---- pass 2: P = exp2(s * scale_log2 - m_run) -> fp16 -> swizzled smem (K-major A operand of the PV product)
-#pragma unroll 1
-      for (int ch = 0; ch < 4; ++ch) {
-        uint32_t s[32];
-        tmem_ld32(tmem_S + lane_addr + ch * 32, s);
-        tmem_wait_ld();
-        uint8_t* pbox = sP + (ch >> 1) * Cfg::kBox;
-#pragma unroll
-        for (int g = 0; g < 4; ++g) {
-          uint4 q;
-          __half2* h = reinterpret_cast<__half2*>(&q);
-#pragma unroll
-          for (int t = 0; t < 4; ++t) {
-            const int i = g * 8 + 2 * t;
-            float p0 = ex2_approx(fmaf(__uint_as_float(s[i]), p.scale_log2, -m_run));
-            float p1 = ex2_approx(fmaf(__uint_as_float(s[i + 1]), p.scale_log2, -m_run));
-            if (p.rows_k != 128) {
-              if (ch * 32 + i >= p.rows_k) p0 = 0.f;
-              if (ch * 32 + i + 1 >= p.rows_k) p1 = 0.f;
-            }
-            h[t] = __floats2half2_rn(p0, p1);
-          }
-          *reinterpret_cast<uint4*>(pbox + sw128_offset(r, (ch & 1) * 4 + g)) = q;
-        }
-      }
-      fence_proxy_async_smem();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(p_full);
+    for (int x = 1; x <= 2; x <<= 1) {
+      mx_lo = fmaxf(mx_lo, __shfl_xor_sync(0xffffffffu, mx_lo, x));
+      mx_hi = fmaxf(mx_hi, __shfl_xor_sync(0xffffffffu, mx_hi, x));
     }
-    // ---- epilogue: O / O[:, D] -> fp16 -> global (through the query view geometry)
-    mbar_wait(o_full, 0);
-    tc_fence_after();
-    float inv;
-    {
-      uint32_t o[16];
-      tmem_ld16(tmem_O + lane_addr + (D / 16) * 16, o);
-      tmem_wait_ld();
-      inv = p.out_scale / __uint_as_float(o[D % 16]);
+    const float mn_lo = fmaxf(m_lo, mx_lo * p.scale_log2), mn_hi = fmaxf(m_hi, mx_hi * p.scale_log2);
+    if (j == 0) {
+      m_lo = mn_lo; m_hi = mn_hi;
+    } else if (__any_sync(0xffffffffu, mn_lo - m_lo > kRescaleLog2 || mn_hi - m_hi > kRescaleLog2)) {
+      if (p.dbg && lane == 0) atomicAdd(p.dbg, 1ull);
+      const float a_lo = ex2_approx(m_lo - mn_lo), a_hi = ex2_approx(m_hi - mn_hi);
+#pragma unroll
+      for (int c = 0; c < Cfg::kDv / 8; ++c) {
+        o[4 * c] *= a_lo; o[4 * c + 1] *= a_lo; o[4 * c + 2] *= a_hi; o[4 * c + 3] *= a_hi;
+      }
+      m_lo = mn_lo; m_hi = mn_hi;
     }
-    const bool row_ok = r < p.rows_q;
+    // ---- P = exp2(s * scale_log2 - m) -> fp16 A fragments of the four 16-key k-steps
+    uint32_t pa[4][4];
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const float* sb = s + 4 * (2 * kk + h);
+        pa[kk][2 * h] = pack_f16x2(ex2_approx(fmaf(sb[0], p.scale_log2, -m_lo)), ex2_approx(fmaf(sb[1], p.scale_log2, -m_lo)));
+        pa[kk][2 * h + 1] = pack_f16x2(ex2_approx(fmaf(sb[2], p.scale_log2, -m_hi)), ex2_approx(fmaf(sb[3], p.scale_log2, -m_hi)));
+      }
+    }
+    // ---- O += P V
+    mbar_wait(&v_full[st], ph);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) {
+      // V is MN-major: 16 keys = two 8-row swizzle atoms (SBO = 1024 B); the next 64 value columns live one TMA box further
+      const uint64_t vd = make_smem_desc_sw128(smem_u32(sV + st * Cfg::kVB * Cfg::kKVBox) + kk * 2048, Cfg::kKVBox, 1024);
+      wgmma_pv<Cfg::kDv>(o, pa[kk], vd, 1u);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence(o);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&kv_empty[st]);
+  }
+  // ---- epilogue: O / O[:, D] -> fp16 -> global (through the query view geometry); column D sits in lane t = 0 of the quad
+  const float l_lo = __shfl_sync(0xffffffffu, o[4 * (D / 8)], lane & ~3);
+  const float l_hi = __shfl_sync(0xffffffffu, o[4 * (D / 8) + 2], lane & ~3);
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int r = wg * 64 + (warp & 3) * 16 + g + 8 * h;
+    if (r >= p.rows_q) continue;
+    const float inv = p.out_scale / (h ? l_hi : l_lo);
     const int i1 = q_i1 + r % p.q_box1;
     const int i2 = q_i2 + r / p.q_box1;
     __half* orow = p.out + (int64_t)i1 * p.os1 + (int64_t)i2 * p.os2 + (int64_t)q_i3 * p.os3 + (int64_t)q_i4 * p.os4 +
-                   head * D;
-#pragma unroll 1
-    for (int c = 0; c < (D + 15) / 16; ++c) {
-      uint32_t o[16];
-      tmem_ld16(tmem_O + lane_addr + c * 16, o);
-      tmem_wait_ld();
-      if (row_ok) {
+                   head * D + 2 * t;
 #pragma unroll
-        for (int g = 0; g < 2; ++g) {
-          if (c * 16 + g * 8 < D) {
-            uint4 q;
-            __half2* h = reinterpret_cast<__half2*>(&q);
-            float v[8];
-#pragma unroll
-            for (int t = 0; t < 8; ++t) v[t] = __uint_as_float(o[g * 8 + t]) * inv;
-            if (p.accumulate) {
-              const uint4 old = *reinterpret_cast<const uint4*>(orow + c * 16 + g * 8);
-              const __half2* ho = reinterpret_cast<const __half2*>(&old);
-#pragma unroll
-              for (int t = 0; t < 4; ++t) {
-                const float2 f = __half22float2(ho[t]);
-                v[2 * t] += f.x;
-                v[2 * t + 1] += f.y;
-              }
-            }
-#pragma unroll
-            for (int t = 0; t < 4; ++t) h[t] = __floats2half2_rn(v[2 * t], v[2 * t + 1]);
-            *reinterpret_cast<uint4*>(orow + c * 16 + g * 8) = q;
-          }
-        }
+    for (int c = 0; c < D / 8; ++c) {
+      float v0 = o[4 * c + 2 * h] * inv, v1 = o[4 * c + 2 * h + 1] * inv;
+      if (p.accumulate) {
+        const float2 f = __half22float2(*reinterpret_cast<const __half2*>(orow + 8 * c));
+        v0 += f.x; v1 += f.y;
       }
+      *reinterpret_cast<uint32_t*>(orow + 8 * c) = pack_f16x2(v0, v1);
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc<Cfg::kTmemCols>(tmem_base);
-}
-
-// ---------------------------------------------------------------------------------------------------------------
-// v4 (head_dim 40 and 80): v3's pipeline with SIXTEEN softmax warps.  Every 128-row query tile is served by 8 warps: the
-//   two warps that own a 32-row TMEM lane quadrant split the 64 keys of a step (32 columns each).  Four softmax warps
-//   per SM sub-partition instead of two: while one sits in its barrier / TMEM-load / arrive bookkeeping the other three
-//   keep the MUFU pipe (the bound at head_dim 40: 8 cycles per warp-wide ex2 + 4 per F2FP, profiles/r01_pipes_ubench.txt)
-//   busy, and 32 score registers per thread instead of 64 leave room for the compiler to software-pipeline the
-//   exponentials.  The two halves of a row keep ONE stabiliser m_run: they exchange their step maxima through shared
-//   memory + a 64-thread named barrier and reach the same rescale decision (both see the same 32 rows).
-//   TMEM: S[g][b] at column (2g+b)*64, O[g] at 256 + g*kOStride.
-//   Warps: 0-15 softmax (tile g = w>>3, half h = (w>>2)&1, quadrant w&3), 16/17 MMA issue for tile 0/1, 18 TMA, 19 TMEM.
-// ---------------------------------------------------------------------------------------------------------------
-template <int D>
-struct Attn4Cfg {
-  static constexpr int kDqk = (D + 15) / 16 * 16;
-  static constexpr int kDv = (D + 1 + 15) / 16 * 16;
-  static constexpr int kQB = (kDqk + 63) / 64;       // 64-column boxes per Q / K row
-  static constexpr int kVB = (kDv + 63) / 64;
-  static constexpr int kStages = (kQB == 1) ? 4 : 2;
-  static constexpr int kQBox = 128 * 128;            // 128 rows x 64 cols fp16
-  static constexpr int kKVBox = 64 * 128;            // 64 keys x 64 cols fp16
-  static constexpr int kSmemQ = 2 * kQB * kQBox;
-  static constexpr int kSmemK = kStages * kQB * kKVBox;
-  static constexpr int kSmemV = kStages * kVB * kKVBox;
-  static constexpr int kPBox = 128 * 128;            // 128 rows x 64 keys fp16
-  static constexpr int kSmemP = 2 * 2 * kPBox;       // [2 tiles][2 buffers]
-  static constexpr int kSmemMx = 3 * 2 * 2 * 128 * 4;   // [step parity | step-0 slot][tile][half][row] fp32 step maxima
-  static constexpr int kSmemBytes = kSmemQ + kSmemK + kSmemV + kSmemP + kSmemMx + 1024 + 512;
-  static constexpr int kOStride = (kDv <= 64) ? 64 : 128;
-  static_assert(256 + 2 * kOStride <= 512, "TMEM budget");
-  static_assert(kSmemBytes <= 227 * 1024, "shared memory budget");
-  static constexpr int kOChunks = kDv / 16;                  // 16-column chunks of an O row
-  static constexpr int kOChunks0 = (kOChunks + 1) / 2;       // chunks half 0 owns (rescale + epilogue); half 1: the rest
-};
-
-// POLY: how many of the 4 fp16x2 pairs of every 8-key chunk take exp2 on the FMA pipe (exp2_fma) instead of MUFU.
-template <int D, int POLY>
-__global__ void __launch_bounds__(640, 1)
-attn4_tc_kernel(const AttnDev p, const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapK,
-                const __grid_constant__ CUtensorMap mapV) {
-  using Cfg = Attn4Cfg<D>;
-  constexpr int S = Cfg::kStages;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* sQ = smem;
-  uint8_t* sK = sQ + Cfg::kSmemQ;
-  uint8_t* sV = sK + Cfg::kSmemK;
-  uint8_t* sP = sV + Cfg::kSmemV;              // [2 tiles][2 buffers] 128 x 64 fp16, K-major, 128B-swizzled
-  float* sMx = reinterpret_cast<float*>(sP + Cfg::kSmemP);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sP + Cfg::kSmemP + Cfg::kSmemMx);
-  uint64_t* q_full = bars;
-  uint64_t* k_full = bars + 1;                 // [S]
-  uint64_t* v_full = k_full + S;               // [S]
-  uint64_t* k_empty = v_full + S;              // [S]
-  uint64_t* v_empty = k_empty + S;             // [S]
-  uint64_t* s_full = v_empty + S;              // [2 tiles][2 buffers]
-  uint64_t* s_free = s_full + 4;               // [2][2]  S(j) sits in the softmax warps' registers
-  uint64_t* p_full = s_free + 4;               // [2][2]
-  uint64_t* pv_done = p_full + 4;              // [2][2]
-  uint64_t* o_full = pv_done + 4;              // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(o_full + 2);
-
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const int qt0 = blockIdx.x * 2;
-  const bool has1 = qt0 + 1 < p.q_tiles;
-  const int head = blockIdx.y;
-  const int qb = blockIdx.z;
-  const int n = p.kv_tiles;
-
-  if (p.rows_q < 128 || p.k_box1 * p.k_box2 < 64 || !has1) {
-    // partially filled tiles: rows TMA never writes must read as zeros (0 * garbage could be NaN in P V)
-    uint4* z = reinterpret_cast<uint4*>(sQ);
-    const int n16 = (Cfg::kSmemQ + Cfg::kSmemK + Cfg::kSmemV) / 16;
-    for (int i = threadIdx.x; i < n16; i += blockDim.x) z[i] = make_uint4(0, 0, 0, 0);
-    fence_proxy_async_smem();
-  }
-  if (warp == 18 && lane == 0) {
-    tma_prefetch_desc(&mapQ);
-    tma_prefetch_desc(&mapK);
-    tma_prefetch_desc(&mapV);
-    mbar_init(q_full, 1);
-    const int tiles = has1 ? 2 : 1;
-    for (int i = 0; i < S; ++i) {
-      mbar_init(&k_full[i], 1);
-      mbar_init(&v_full[i], 1);
-      mbar_init(&k_empty[i], tiles);          // one commit per MMA-issuing warp
-      mbar_init(&v_empty[i], tiles);
-    }
-    for (int i = 0; i < 4; ++i) {
-      mbar_init(&s_full[i], 1);
-      mbar_init(&s_free[i], 8);
-      mbar_init(&p_full[i], 8);
-      mbar_init(&pv_done[i], 1);
-    }
-    mbar_init(&o_full[0], 1);
-    mbar_init(&o_full[1], 1);
-    mbar_fence_init();
-  }
-  if (warp == 19) tmem_alloc<512>(tmem_slot);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const int q_i3 = qb % p.q_e3;
-  const int q_i4 = qb / p.q_e3;
-
-  if (warp == 18) {
-    if (lane == 0) {
-      const int kb = qb / p.kv_div;
-      const int k_i3 = p.kv_i3_zero ? 0 : (kb % p.k_e3);
-      const int k_i4 = kb / p.k_e3;
-      const int tiles = has1 ? 2 : 1;
-      mbar_expect_tx(q_full, p.q_box_bytes * (uint32_t)(tiles * Cfg::kQB));
-      for (int t = 0; t < tiles; ++t) {
-        const int qt = qt0 + t;
-#pragma unroll
-        for (int b = 0; b < Cfg::kQB; ++b)
-          tma_load_5d(sQ + (t * Cfg::kQB + b) * Cfg::kQBox, &mapQ, q_full, head * Cfg::kDqk + b * 64, (qt % p.q_t1) * p.q_box1,
-                      (qt / p.q_t1) * p.q_box2, q_i3, q_i4);
-      }
-      // K runs two steps ahead of V (QK^T(j+2) is issued during step j): interleave the issue order accordingly
-      auto load_k = [&](int j) {
-        const int st = j % S;
-        mbar_wait(&k_empty[st], ((j / S) & 1) ^ 1);
-        mbar_expect_tx(&k_full[st], p.k_box_bytes * Cfg::kQB);
-#pragma unroll
-        for (int b = 0; b < Cfg::kQB; ++b)
-          tma_load_5d(sK + (st * Cfg::kQB + b) * Cfg::kKVBox, &mapK, &k_full[st], head * Cfg::kDqk + b * 64,
-                      (j % p.k_t1) * p.k_box1, (j / p.k_t1) * p.k_box2, k_i3, k_i4);
-      };
-      auto load_v = [&](int j) {
-        const int st = j % S;
-        mbar_wait(&v_empty[st], ((j / S) & 1) ^ 1);
-        mbar_expect_tx(&v_full[st], p.k_box_bytes * Cfg::kVB);
-#pragma unroll
-        for (int b = 0; b < Cfg::kVB; ++b)
-          tma_load_5d(sV + (st * Cfg::kVB + b) * Cfg::kKVBox, &mapV, &v_full[st], head * Cfg::kDv + b * 64,
-                      (j % p.k_t1) * p.k_box1, (j / p.k_t1) * p.k_box2, k_i3, k_i4);
-      };
-      if (n > 0) load_k(0);
-      if (n > 1) load_k(1);
-      for (int j = 0; j < n; ++j) {
-        if (j + 2 < n) load_k(j + 2);
-        load_v(j);
-      }
-    }
-  } else if (warp == 16 || warp == 17) {
-    const int g = warp - 16;
-    if (lane == 0 && (g == 0 || has1)) {
-      constexpr uint32_t idesc_qk = make_idesc_f16(128, 64, false, false);
-      constexpr uint32_t idesc_pv = make_idesc_f16(128, Cfg::kDv, false, true);
-      // descriptors differ only in the 14-bit (address >> 4) field: build the bases once, add offsets in the loop
-      const uint64_t dq = make_smem_desc_sw128(smem_u32(sQ + g * Cfg::kQB * Cfg::kQBox), 16, 1024);
-      const uint64_t dk = make_smem_desc_sw128(smem_u32(sK), 16, 1024);
-      const uint64_t dv = make_smem_desc_sw128(smem_u32(sV), Cfg::kKVBox, 1024);   // MN-major: next 64 columns one box on
-      const uint64_t dp = make_smem_desc_sw128(smem_u32(sP + 2 * g * Cfg::kPBox), 16, 1024);
-      const uint32_t tS = tmem_base + 2 * g * 64, tO = tmem_base + 256 + g * Cfg::kOStride;
-      auto issue_qk = [&](int j) {      // S[g][j&1] = Q_g K_j^T; the K stage is released as soon as these MMAs retire
-        const uint64_t kb_ = dk + (uint64_t)((j % S) * ((Cfg::kQB * Cfg::kKVBox) >> 4));
-#pragma unroll
-        for (int kk = 0; kk < Cfg::kDqk / 16; ++kk)
-          umma_f16(tS + (j & 1) * 64, dq + (uint64_t)((kk / 4) * (Cfg::kQBox >> 4) + 2 * (kk % 4)),
-                   kb_ + (uint64_t)((kk / 4) * (Cfg::kKVBox >> 4) + 2 * (kk % 4)), idesc_qk, kk ? 1u : 0u);
-        umma_commit(&s_full[2 * g + (j & 1)]);
-        umma_commit(&k_empty[j % S]);
-      };
-      auto issue_pv = [&](int j) {      // O_g += P_g(j) V_j
-        const uint64_t pb_ = dp + (uint64_t)((j & 1) * (Cfg::kPBox >> 4));
-        const uint64_t vb_ = dv + (uint64_t)((j % S) * ((Cfg::kVB * Cfg::kKVBox) >> 4));
-#pragma unroll
-        for (int kk = 0; kk < 4; ++kk)
-          umma_f16(tO, pb_ + (uint64_t)(2 * kk), vb_ + (uint64_t)(128 * kk), idesc_pv, (j | kk) ? 1u : 0u);
-        umma_commit(&pv_done[2 * g + (j & 1)]);
-        umma_commit(&v_empty[j % S]);
-      };
-      mbar_wait(q_full, 0);
-      for (int j0 = 0; j0 < 2 && j0 < n; ++j0) {
-        mbar_wait(&k_full[j0 % S], (j0 / S) & 1);
-        tc_fence_after();
-        issue_qk(j0);
-      }
-      for (int j = 0; j < n; ++j) {
-        if (j + 2 < n) {
-          mbar_wait(&s_free[2 * g + (j & 1)], (j >> 1) & 1);
-          mbar_wait(&k_full[(j + 2) % S], ((j + 2) / S) & 1);
-          tc_fence_after();
-          issue_qk(j + 2);
-        }
-        mbar_wait(&p_full[2 * g + (j & 1)], (j >> 1) & 1);
-        mbar_wait(&v_full[j % S], (j / S) & 1);
-        tc_fence_after();
-        issue_pv(j);
-      }
-      umma_commit(&o_full[g]);
-    } else if (lane == 0 && n > 0) {
-      // tile 1 absent: nothing to issue, and k_empty / v_empty were initialised for a single committer
-    }
-  } else if (warp < 16) {
-    const int g = warp >> 3;
-    if (g == 0 || has1) {
-      const int h = (warp >> 2) & 1;
-      const int quad = warp & 3;
-      const int r = quad * 32 + lane;
-      const uint32_t lane_addr = (uint32_t)(quad * 32) << 16;
-      const uint32_t tmem_O = tmem_base + 256 + g * Cfg::kOStride;
-      const int pair_bar = 1 + g * 4 + quad;       // named barrier shared with the warp that owns the other 32 keys
-      float m_run = -INFINITY;
-      const int rows_tile = p.k_box1 * p.k_box2;   // keys a full tile holds (<= 64)
-      // 16-column chunks of O this half rescales / writes out
-      const int oc0 = h ? Cfg::kOChunks0 : 0, oc1 = h ? Cfg::kOChunks : Cfg::kOChunks0;
-      for (int j = 0; j < n; ++j) {
-        const int valid = ((j == n - 1) ? p.rows_k : rows_tile) - 32 * h;   // valid keys among this half's 32 columns
-        const int b = 2 * g + (j & 1);
-        mbar_wait(&s_full[b], (j >> 1) & 1);
-        tc_fence_after();
-        uint32_t s[32];
-        tmem_ld32(tmem_base + lane_addr + b * 64 + 32 * h, s);
-        tmem_wait_ld();
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&s_free[b]);   // S buffer may be overwritten by QK^T(j+2)
-        if (valid < 32) {
-#pragma unroll
-          for (int i = 0; i < 32; ++i)
-            if (i >= valid) s[i] = 0xff800000u;    // absent key: score -inf -> P = 0
-        }
-        float* mx_mine = sMx + (((j & 1) * 2 + g) * 2 + h) * 128 + r;
-        float* mx_other = sMx + (((j & 1) * 2 + g) * 2 + (h ^ 1)) * 128 + r;
-        auto pair_sync = [&]() { asm volatile("bar.sync %0, 64;" ::"r"(pair_bar) : "memory"); };
-        if (j == 0) {   // no stabiliser yet: the real row maximum first
-          float mx0 = -INFINITY, mx1 = -INFINITY;
-#pragma unroll
-          for (int i = 0; i < 32; i += 4) {
-            mx0 = fmax3(mx0, __uint_as_float(s[i]), __uint_as_float(s[i + 1]));
-            mx1 = fmax3(mx1, __uint_as_float(s[i + 2]), __uint_as_float(s[i + 3]));
-          }
-          const float mloc = fmaxf(mx0, mx1);
-          sMx[((4 + g) * 2 + h) * 128 + r] = mloc;           // slot 2: written once, so no reuse hazard
-          pair_sync();
-          m_run = fmaxf(mloc, sMx[((4 + g) * 2 + (h ^ 1)) * 128 + r]) * p.scale_log2;
-        }
-        uint8_t* sPg = sP + b * Cfg::kPBox;
-        if (j >= 2) mbar_wait(&pv_done[b], ((j - 2) >> 1) & 1);   // P buffer of step j-2 consumed (long ago)
-#pragma unroll 1
-        for (int pass = 0;; ++pass) {
-          // Single pass with a STALE stabiliser (the running max of the previous steps); this step's max is accumulated in
-          // the same loop.  Only when a row's new max exceeds the stabiliser by more than kRescaleLog2 (P could overflow
-          // fp16) is the step redone with the updated stabiliser -- after the first few steps that never happens.
-          float mx0 = -INFINITY, mx1 = -INFINITY;
-          const float neg_m = -m_run;
-#pragma unroll
-          for (int c16 = 0; c16 < 4; ++c16) {
-            uint4 q;
-            uint32_t* qw = reinterpret_cast<uint32_t*>(&q);
-#pragma unroll
-            for (int t = 0; t < 4; ++t) {
-              const int i = c16 * 8 + 2 * t;
-              const float s0 = __uint_as_float(s[i]), s1 = __uint_as_float(s[i + 1]);
-              if (t & 1) mx1 = fmax3(mx1, s0, s1); else mx0 = fmax3(mx0, s0, s1);
-              const bool poly = POLY == 1 ? (t == 1) : POLY == 2 ? (t & 1) : false;
-              const float y0 = fmaf(s0, p.scale_log2, neg_m), y1 = fmaf(s1, p.scale_log2, neg_m);
-              qw[t] = poly ? pack_f16x2(exp2_fma(y0), exp2_fma(y1)) : pack_f16x2(ex2_approx(y0), ex2_approx(y1));
-            }
-            *reinterpret_cast<uint4*>(sPg + sw128_offset(r, 4 * h + c16)) = q;
-          }
-          if (pass > 0 || j == 0) break;
-          *mx_mine = fmaxf(mx0, mx1);
-          pair_sync();
-          const float m_new = fmaxf(fmaxf(mx0, mx1), *mx_other) * p.scale_log2;   // identical in both halves of the row
-          if (!__any_sync(0xffffffffu, m_new - m_run > kRescaleLog2)) break;
-          if (p.dbg && lane == 0) atomicAdd(p.dbg, 1ull);
-          // rare: O_g must be stable -> PV of the previous step has to be complete; each half rescales its O chunks
-          const float m_up = fmaxf(m_run, m_new);
-          mbar_wait(&pv_done[2 * g + ((j - 1) & 1)], ((j - 1) >> 1) & 1);
-          tc_fence_after();
-          const float alpha = ex2_approx(m_run - m_up);
-#pragma unroll 1
-          for (int c = oc0; c < oc1; ++c) {
-            uint32_t o[16];
-            tmem_ld16(tmem_O + lane_addr + c * 16, o);
-            tmem_wait_ld();
-#pragma unroll
-            for (int i = 0; i < 16; ++i) o[i] = __float_as_uint(__uint_as_float(o[i]) * alpha);
-            tmem_st16(tmem_O + lane_addr + c * 16, o);
-          }
-          tmem_wait_st();
-          m_run = m_up;
-        }
-        fence_proxy_async_smem();
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&p_full[b]);
-      }
-      // ---- epilogue: this half writes its chunks of the normalised rows
-      mbar_wait(&o_full[g], 0);
-      tc_fence_after();
-      float inv;
-      {
-        uint32_t o[16];
-        tmem_ld16(tmem_O + lane_addr + (D / 16) * 16, o);
-        tmem_wait_ld();
-        inv = p.out_scale / __uint_as_float(o[D % 16]);
-      }
-      const int qt = qt0 + g;
-      const int q_i1 = (qt % p.q_t1) * p.q_box1, q_i2 = (qt / p.q_t1) * p.q_box2;
-      const bool row_ok = r < p.rows_q;
-      const int i1 = q_i1 + r % p.q_box1;
-      const int i2 = q_i2 + r / p.q_box1;
-      __half* orow = p.out + (int64_t)i1 * p.os1 + (int64_t)i2 * p.os2 + (int64_t)q_i3 * p.os3 + (int64_t)q_i4 * p.os4 + head * D;
-#pragma unroll 1
-      for (int c = oc0; c < oc1; ++c) {
-        if (c * 16 >= D) break;
-        uint32_t o[16];
-        tmem_ld16(tmem_O + lane_addr + c * 16, o);
-        tmem_wait_ld();
-        if (row_ok) {
-#pragma unroll
-          for (int gq = 0; gq < 2; ++gq) {
-            if (c * 16 + gq * 8 < D) {
-              uint4 q;
-              __half2* hh = reinterpret_cast<__half2*>(&q);
-              float v[8];
-#pragma unroll
-              for (int t = 0; t < 8; ++t) v[t] = __uint_as_float(o[gq * 8 + t]) * inv;
-              if (p.accumulate) {
-                const uint4 old = *reinterpret_cast<const uint4*>(orow + c * 16 + gq * 8);
-                const __half2* ho = reinterpret_cast<const __half2*>(&old);
-#pragma unroll
-                for (int t = 0; t < 4; ++t) {
-                  const float2 f = __half22float2(ho[t]);
-                  v[2 * t] += f.x;
-                  v[2 * t + 1] += f.y;
-                }
-              }
-#pragma unroll
-              for (int t = 0; t < 4; ++t) hh[t] = __floats2half2_rn(v[2 * t], v[2 * t + 1]);
-              *reinterpret_cast<uint4*>(orow + c * 16 + gq * 8) = q;
-            }
-          }
-        }
-      }
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 19) tmem_dealloc<512>(tmem_base);
-}
-
-// ---------------------------------------------------------------------------------------------------------------
-// softmax arithmetic of the v5 kernel
-//   * the exponent offset carries a fixed bias: P' = 2^(y + kPBias) with y = s*scale*log2e - stabiliser.  The bias cancels in
-//     O / rowsum (the row sum is the ones column of V, accumulated from the same P'); it moves the fp16 flush-to-zero point of
-//     cvt.rn.f16x2 from 2^-14 to 2^-24 of the stabiliser.  Head-room: y <= kRescale5 (stale stabiliser), P' <= 2^14 < 65504.
-//   * y for a score pair comes from one packed fma.rn.f32x2; ex2.approx per score, cvt.rn.f16x2 per pair: 20 XU-pipe cycles per
-//     pair (MUFU.EX2 8 cycles per warp instruction, F2FP 4, same pipe: profiles/r01_pipes_ubench.txt) -- the kernel's floor.
-//   Measured and NOT kept (profiles/r02_attn_experiments.txt, code in git history at the commit named there): a half2
-//   Cody-Waite polynomial 2^y on the FMA pipe for 1-3 of every 4 pairs (correct to 3.6e-4 rel-l2, but the softmax warps are
-//   issue-bound once the XU pipe is relieved: 1.85 -> 1.91 / 1.98 / 2.08 ms); XU turn-taking tickets between the warps of an
-//   SM sub-partition (a single warp reaches only ~45 % of the pipe: 1.97 -> 3.37 / 2.22 / 2.14 ms for 1 / 2 / 3 warps at a
-//   time); a software-pipelined step loop with split TMEM loads (2.13 -> 2.23 ms).
-// ---------------------------------------------------------------------------------------------------------------
-constexpr float kPBias = 10.0f;
-constexpr float kRescale5 = 4.0f;
-
-__device__ __forceinline__ uint64_t pack2(float lo, float hi) {
-  uint64_t r;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
-  return r;
-}
-__device__ __forceinline__ uint64_t pack2u(uint32_t lo, uint32_t hi) {
-  uint64_t r;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "r"(lo), "r"(hi));
-  return r;
-}
-__device__ __forceinline__ void unpack2(uint64_t v, float& lo, float& hi) { asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v)); }
-__device__ __forceinline__ uint64_t ffma2(uint64_t a, uint64_t b, uint64_t c) {
-  uint64_t d;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c));
-  return d;
-}
-__device__ __forceinline__ void st_shared_v4(uint32_t addr, const uint4& v) {
-  asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
-}
-
-// ---------------------------------------------------------------------------------------------------------------
-// v5 (head_dim 40): v4 with the two key halves of a step made INDEPENDENT.  In v4 the two warps that share a 32-row
-//   quadrant keep one stabiliser and meet at a named barrier every step; both sit on the same SM sub-partition, so they
-//   behave like one 64-key warp and the MUFU pipe still idles ~37% of the time (profiles/r01_ncu_attn4.txt).  Here each half
-//   owns a full online-softmax state: its own stabiliser, its own O accumulator in TMEM (4 x 64 columns fit next to the
-//   4 x 64 score columns only at head_dim 40) and its own P-ready barrier; PV is issued per half (K = 32 keys).  The two
-//   partial results of a row are merged once, in the epilogue: O = (w0 O0 + w1 O1) / (w0 l0 + w1 l1), w_h = 2^(m_h - m).
-//   TMEM: S[g][b] at column (2g+b)*64, O[g][h] at 256 + (2g+h)*64.
-// ---------------------------------------------------------------------------------------------------------------
-template <int D, int G>
-struct Attn5Cfg {
-  static constexpr int kDqk = (D + 15) / 16 * 16;
-  static constexpr int kDv = (D + 1 + 15) / 16 * 16;
-  static constexpr int kQB = (kDqk + 63) / 64;       // 64-column boxes per Q / K row
-  static constexpr int kVB = (kDv + 63) / 64;
-  static constexpr int kStages = (G == 2) ? 4 : 3;       // G = 1: two CTAs share an SM's shared memory
-  static constexpr int kQBox = 128 * 128;            // 128 rows x 64 cols fp16
-  static constexpr int kKVBox = 64 * 128;            // 64 keys x 64 cols fp16
-  static constexpr int kSmemQ = G * kQB * kQBox;
-  static constexpr int kSmemK = kStages * kQB * kKVBox;
-  static constexpr int kSmemV = kStages * kVB * kKVBox;
-  static constexpr int kPBox = 128 * 128;            // 128 rows x 64 keys fp16
-  static constexpr int kSmemP = G * 2 * kPBox;       // [G tiles][2 buffers]
-  static constexpr int kSmemMx = G * 2 * 128 * 4;       // [tile][half][row] final stabilisers (epilogue merge)
-  static constexpr int kSmemBytes = kSmemQ + kSmemK + kSmemV + kSmemP + kSmemMx + 1024 + 512;
-  static_assert(kDv <= 64 && kQB == 1 && kVB == 1, "v5 keeps four O accumulators in TMEM: head_dim <= 47 only");
-  static_assert(kSmemBytes <= (G == 2 ? 227 : 113) * 1024, "shared memory budget");
-  static constexpr int kThreads = G == 2 ? 640 : 320;
-  static constexpr int kSoft = 8 * G;                        // softmax warps [0, 8G); MMA issuers kSoft .. kSoft+G-1
-  static constexpr int kTmaWarp = kSoft + G;                 // TMA producer (also initialises the barriers)
-  static constexpr int kAllocWarp = G == 2 ? 19 : kTmaWarp;  // TMEM allocation / release
-  static constexpr int kTmemCols = G == 2 ? 512 : 256;
-  static constexpr int kColP = G == 2 ? 128 : 64;            // TS: P[g][b] at kColP + (2g+b)*32
-  static constexpr int kColO = G == 2 ? 256 : 128;           // O[g][h] at kColO + (2g+h)*64
-  static constexpr int kOChunks = kDv / 16;                  // 16-column chunks of an O row
-  static constexpr int kOChunks0 = (kOChunks + 1) / 2;       // chunks half 0 owns (rescale + epilogue); half 1: the rest
-};
-
-// POLY: how many of the 4 fp16x2 pairs of every 8-key chunk take exp2 on the FMA pipe (exp2_fma) instead of MUFU.
-// TS: the probabilities of a step go to TENSOR MEMORY (tcgen05.st) and the P V product reads its A operand from there
-//   (tcgen05.mma [d], [a_tmem], b_desc): no swizzled shared-memory stores, no fence.proxy.async / MEMBAR per step.  TMEM then holds
-//   S[g] single-buffered at column g*64 (S(j) sits in registers right after the step starts, so QK^T(j+1) has a whole step to
-//   land), P[g][b] (64 keys = 32 packed columns) at 128 + (2g+b)*32, O[g][h] at 256 + (2g+h)*64.
-template <int D, bool TS, int G>
-__global__ void __launch_bounds__(G == 2 ? 640 : 320, G == 2 ? 1 : 2)
-attn5_tc_kernel(const AttnDev p, const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapK,
-                const __grid_constant__ CUtensorMap mapV) {
-  using Cfg = Attn5Cfg<D, G>;
-  constexpr int S = Cfg::kStages;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* sQ = smem;
-  uint8_t* sK = sQ + Cfg::kSmemQ;
-  uint8_t* sV = sK + Cfg::kSmemK;
-  uint8_t* sP = sV + Cfg::kSmemV;              // [2 tiles][2 buffers] 128 x 64 fp16, K-major, 128B-swizzled
-  float* sMx = reinterpret_cast<float*>(sP + Cfg::kSmemP);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sP + Cfg::kSmemP + Cfg::kSmemMx);
-  uint64_t* q_full = bars;
-  uint64_t* k_full = bars + 1;                 // [S]
-  uint64_t* v_full = k_full + S;               // [S]
-  uint64_t* k_empty = v_full + S;              // [S]
-  uint64_t* v_empty = k_empty + S;             // [S]
-  uint64_t* s_full = v_empty + S;              // [2 tiles][2 buffers]
-  uint64_t* s_free = s_full + 4;               // [2][2]  S(j) sits in the softmax warps' registers
-  uint64_t* p_full = s_free + 4;               // [2 tiles][2 halves][2 buffers]
-  uint64_t* pv_done = p_full + 8;              // [2][2][2]
-  uint64_t* o_full = pv_done + 8;              // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(o_full + 2);
-
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const int qt0 = blockIdx.x * G;
-  const bool has1 = G == 2 && qt0 + 1 < p.q_tiles;
-  const int head = blockIdx.y;
-  const int qb = blockIdx.z;
-  const int n = p.kv_tiles;
-  // debug: life cycle of four CTAs (linear ids 0, 1/4, 1/2, 3/4 of the grid): clock64 at entry / set-up done / first scores in
-  // registers / step loop done / accumulators complete / rows stored / exit, and the SM id (tools/attn_timeline.py)
-  unsigned long long* ctr = nullptr;
-  if (p.dbg) {
-    const unsigned lin = blockIdx.x + gridDim.x * (blockIdx.y + gridDim.y * blockIdx.z), tot = gridDim.x * gridDim.y * gridDim.z;
-    for (unsigned k = 0; k < 4; ++k)
-      if (lin == (tot / 4) * k) ctr = p.dbg + 8 + 4 * 32 * 8 + k * 8;
-  }
-  if (ctr && threadIdx.x == 0) {
-    unsigned smid;
-    asm volatile("mov.u32 %0, %%smid;" : "=r"(smid));
-    ctr[0] = clock64();
-    ctr[7] = smid;
-  }
-
-  if (p.rows_q < 128 || p.k_box1 * p.k_box2 < 64 || (G == 2 && !has1)) {
-    // partially filled tiles: rows TMA never writes must read as zeros (0 * garbage could be NaN in P V)
-    uint4* z = reinterpret_cast<uint4*>(sQ);
-    const int n16 = (Cfg::kSmemQ + Cfg::kSmemK + Cfg::kSmemV) / 16;
-    for (int i = threadIdx.x; i < n16; i += blockDim.x) z[i] = make_uint4(0, 0, 0, 0);
-    fence_proxy_async_smem();
-  }
-  if (warp == Cfg::kTmaWarp && lane == 0) {
-    tma_prefetch_desc(&mapQ);
-    tma_prefetch_desc(&mapK);
-    tma_prefetch_desc(&mapV);
-    mbar_init(q_full, 1);
-    const int tiles = has1 ? 2 : 1;
-    for (int i = 0; i < S; ++i) {
-      mbar_init(&k_full[i], 1);
-      mbar_init(&v_full[i], 1);
-      mbar_init(&k_empty[i], tiles);          // one commit per MMA-issuing warp
-      mbar_init(&v_empty[i], tiles);
-    }
-    for (int i = 0; i < 4; ++i) {
-      mbar_init(&s_full[i], 1);
-      mbar_init(&s_free[i], 8);
-    }
-    for (int i = 0; i < 8; ++i) {
-      mbar_init(&p_full[i], 4);
-      mbar_init(&pv_done[i], 1);
-    }
-    mbar_init(&o_full[0], 1);
-    mbar_init(&o_full[1], 1);
-    mbar_fence_init();
-  }
-  if (warp == Cfg::kAllocWarp) tmem_alloc<Cfg::kTmemCols>(tmem_slot);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  if (ctr && threadIdx.x == 0) ctr[1] = clock64();
-  const int q_i3 = qb % p.q_e3;
-  const int q_i4 = qb / p.q_e3;
-
-  if (warp == Cfg::kTmaWarp) {
-    if (lane == 0) {
-      const int kb = qb / p.kv_div;
-      const int k_i3 = p.kv_i3_zero ? 0 : (kb % p.k_e3);
-      const int k_i4 = kb / p.k_e3;
-      const int tiles = has1 ? 2 : 1;
-      mbar_expect_tx(q_full, p.q_box_bytes * (uint32_t)(tiles * Cfg::kQB));
-      for (int t = 0; t < tiles; ++t) {
-        const int qt = qt0 + t;
-#pragma unroll
-        for (int b = 0; b < Cfg::kQB; ++b)
-          tma_load_5d(sQ + (t * Cfg::kQB + b) * Cfg::kQBox, &mapQ, q_full, head * Cfg::kDqk + b * 64, (qt % p.q_t1) * p.q_box1,
-                      (qt / p.q_t1) * p.q_box2, q_i3, q_i4);
-      }
-      // K runs two steps ahead of V (QK^T(j+2) is issued during step j): interleave the issue order accordingly
-      auto load_k = [&](int j) {
-        const int st = j % S;
-        mbar_wait(&k_empty[st], ((j / S) & 1) ^ 1);
-        mbar_expect_tx(&k_full[st], p.k_box_bytes * Cfg::kQB);
-#pragma unroll
-        for (int b = 0; b < Cfg::kQB; ++b)
-          tma_load_5d(sK + (st * Cfg::kQB + b) * Cfg::kKVBox, &mapK, &k_full[st], head * Cfg::kDqk + b * 64,
-                      (j % p.k_t1) * p.k_box1, (j / p.k_t1) * p.k_box2, k_i3, k_i4);
-      };
-      auto load_v = [&](int j) {
-        const int st = j % S;
-        mbar_wait(&v_empty[st], ((j / S) & 1) ^ 1);
-        mbar_expect_tx(&v_full[st], p.k_box_bytes * Cfg::kVB);
-#pragma unroll
-        for (int b = 0; b < Cfg::kVB; ++b)
-          tma_load_5d(sV + (st * Cfg::kVB + b) * Cfg::kKVBox, &mapV, &v_full[st], head * Cfg::kDv + b * 64,
-                      (j % p.k_t1) * p.k_box1, (j / p.k_t1) * p.k_box2, k_i3, k_i4);
-      };
-      if (n > 0) load_k(0);
-      if (n > 1) load_k(1);
-      for (int j = 0; j < n; ++j) {
-        if (j + 2 < n) load_k(j + 2);
-        load_v(j);
-      }
-    }
-  } else if (warp >= Cfg::kSoft && warp < Cfg::kSoft + G) {
-    const int g = warp - Cfg::kSoft;
-    if (lane == 0 && (g == 0 || has1)) {
-      constexpr uint32_t idesc_qk = make_idesc_f16(128, 64, false, false);
-      constexpr uint32_t idesc_pv = make_idesc_f16(128, Cfg::kDv, false, true);
-      // descriptors differ only in the 14-bit (address >> 4) field: build the bases once, add offsets in the loop
-      const uint64_t dq = make_smem_desc_sw128(smem_u32(sQ + g * Cfg::kQB * Cfg::kQBox), 16, 1024);
-      const uint64_t dk = make_smem_desc_sw128(smem_u32(sK), 16, 1024);
-      const uint64_t dv = make_smem_desc_sw128(smem_u32(sV), Cfg::kKVBox, 1024);   // MN-major: next 64 columns one box on
-      const uint64_t dp = make_smem_desc_sw128(smem_u32(sP + 2 * g * Cfg::kPBox), 16, 1024);
-      const uint32_t tS = tmem_base + (TS ? g * 64 : 2 * g * 64), tO = tmem_base + Cfg::kColO + 2 * g * 64;
-      const uint32_t tP = tmem_base + Cfg::kColP + 2 * g * 32;     // TS only
-      auto issue_qk = [&](int j) {      // S[g][j&1] (TS: S[g]) = Q_g K_j^T; the K stage is released as soon as these MMAs retire
-        const uint64_t kb_ = dk + (uint64_t)((j % S) * ((Cfg::kQB * Cfg::kKVBox) >> 4));
-#pragma unroll
-        for (int kk = 0; kk < Cfg::kDqk / 16; ++kk)
-          umma_f16(tS + (TS ? 0 : (j & 1) * 64), dq + (uint64_t)((kk / 4) * (Cfg::kQBox >> 4) + 2 * (kk % 4)),
-                   kb_ + (uint64_t)((kk / 4) * (Cfg::kKVBox >> 4) + 2 * (kk % 4)), idesc_qk, kk ? 1u : 0u);
-        umma_commit(&s_full[2 * g + (TS ? 0 : (j & 1))]);
-        umma_commit(&k_empty[j % S]);
-      };
-      auto issue_pv = [&](int j, int hh) {      // O_g,hh += P_g(j)[:, 32 hh .. 32 hh + 31] V_j[32 hh .. 32 hh + 31, :]
-        const uint64_t pb_ = dp + (uint64_t)((j & 1) * (Cfg::kPBox >> 4));
-        const uint64_t vb_ = dv + (uint64_t)((j % S) * ((Cfg::kVB * Cfg::kKVBox) >> 4));
-#pragma unroll
-        for (int kk = 0; kk < 2; ++kk) {
-          if (TS)   // A = P[g][j&1] in TMEM: 16 keys = 8 packed columns per MMA
-            umma_f16_ts(tO + hh * 64, tP + (j & 1) * 32 + (2 * hh + kk) * 8, vb_ + (uint64_t)(128 * (2 * hh + kk)), idesc_pv,
-                        (j | kk) ? 1u : 0u);
-          else
-            umma_f16(tO + hh * 64, pb_ + (uint64_t)(2 * (2 * hh + kk)), vb_ + (uint64_t)(128 * (2 * hh + kk)), idesc_pv,
-                     (j | kk) ? 1u : 0u);
-        }
-        umma_commit(&pv_done[(2 * g + hh) * 2 + (j & 1)]);
-      };
-      mbar_wait(q_full, 0);
-      constexpr int kAhead = TS ? 1 : 2;       // QK^T runs this many steps ahead of the softmax
-      for (int j0 = 0; j0 < kAhead && j0 < n; ++j0) {
-        mbar_wait(&k_full[j0 % S], (j0 / S) & 1);
-        tc_fence_after();
-        issue_qk(j0);
-      }
-      for (int j = 0; j < n; ++j) {
-        if (j + kAhead < n) {
-          if (TS) mbar_wait(&s_free[2 * g], j & 1);                   // S(j) is in the softmax warps' registers
-          else mbar_wait(&s_free[2 * g + (j & 1)], (j >> 1) & 1);
-          mbar_wait(&k_full[(j + kAhead) % S], ((j + kAhead) / S) & 1);
-          tc_fence_after();
-          issue_qk(j + kAhead);
-        }
-        mbar_wait(&v_full[j % S], (j / S) & 1);
-#pragma unroll
-        for (int hh = 0; hh < 2; ++hh) {
-          mbar_wait(&p_full[(2 * g + hh) * 2 + (j & 1)], (j >> 1) & 1);
-          tc_fence_after();
-          issue_pv(j, hh);
-        }
-        umma_commit(&v_empty[j % S]);
-      }
-      umma_commit(&o_full[g]);
-    } else if (lane == 0 && n > 0) {
-      // tile 1 absent: nothing to issue, and k_empty / v_empty were initialised for a single committer
-    }
-  } else if (warp < Cfg::kSoft) {
-    const int g = warp >> 3;
-    if (g == 0 || has1) {
-      const int h = (warp >> 2) & 1;
-      const int quad = warp & 3;
-      const int r = quad * 32 + lane;
-      const uint32_t lane_addr = (uint32_t)(quad * 32) << 16;
-      const uint32_t tmem_O = tmem_base + Cfg::kColO + (2 * g + h) * 64;     // this half's accumulator
-      const int pair_bar = 1 + g * 4 + quad;       // named barrier shared with the warp that owns the other 32 keys
-      float m_run = -INFINITY;
-      uint64_t* my_p_full = p_full + (2 * g + h) * 2;
-      uint64_t* my_pv_done = pv_done + (2 * g + h) * 2;
-      const int rows_tile = p.k_box1 * p.k_box2;   // keys a full tile holds (<= 64)
-      // 16-column chunks of O this half rescales / writes out
-      const uint32_t sP_u32 = smem_u32(sP);
-      uint32_t p_off[4];      // this thread's four 16-byte P chunks of a step (128B-swizzled row r, chunks 4h .. 4h+3)
-#pragma unroll
-      for (int c16 = 0; c16 < 4; ++c16) p_off[c16] = sw128_offset(r, 4 * h + c16);
-      const uint64_t sc2 = pack2(p.scale_log2, p.scale_log2);
-      const int oc0 = h ? Cfg::kOChunks0 : 0, oc1 = h ? Cfg::kOChunks : Cfg::kOChunks0;
-      // "is S(j+1) there" / "are the P columns of step j+1 free" are TESTED (non-blocking) while step j's exponentials run and
-      // only waited for when the test failed: an mbarrier try_wait costs ~100-190 cycles even on a completed phase, and the
-      // four warps of a sub-partition pay it in lockstep while the XU pipe idles (profiles/r02_attn_timeline.txt)
-      bool s_ok = false, p_ok = true;
-      for (int j = 0; j < n; ++j) {
-        const int valid = ((j == n - 1) ? p.rows_k : rows_tile) - 32 * h;   // valid keys among this half's 32 columns
-        const int b = 2 * g + (j & 1);                                 // P buffer (and, without TS, S buffer) of this step
-        const int sb_ = TS ? 2 * g : b;                                // S barrier / buffer index
-        const uint32_t s_par = TS ? (uint32_t)(j & 1) : (uint32_t)((j >> 1) & 1);
-        // debug timeline (tools/attn_timeline.py): the four softmax warps of SM sub-partition 0 of CTA (0,0,0), 32 steps
-        const bool tr = p.dbg && j < 32 && quad == 0 && lane == 0 && blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0;
-        unsigned long long* trow = p.dbg + 8 + ((warp >> 2) * 32 + j) * 8;
-        if (tr) trow[0] = clock64();
-        if (!(p.early_test && s_ok)) mbar_wait(&s_full[sb_], s_par);
-        tc_fence_after();
-        uint32_t s[32];
-        tmem_ld32(tmem_base + lane_addr + (TS ? g * 64 : b * 64) + 32 * h, s);
-        tmem_wait_ld();
-        if (tr) trow[1] = clock64();
-        if (ctr && j == 0 && threadIdx.x == 0) ctr[2] = clock64();
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&s_free[sb_]);   // S buffer may be overwritten by the next QK^T into it
-        if (valid < 32) {
-#pragma unroll
-          for (int i = 0; i < 32; ++i)
-            if (i >= valid) s[i] = 0xff800000u;    // absent key: score -inf -> P = 0
-        }
-        if (j == 0) {   // no stabiliser yet: this half's real row maximum first (a fully masked half gets a huge negative one)
-          float mx0 = -INFINITY, mx1 = -INFINITY;
-#pragma unroll
-          for (int i = 0; i < 32; i += 4) {
-            mx0 = fmax3(mx0, __uint_as_float(s[i]), __uint_as_float(s[i + 1]));
-            mx1 = fmax3(mx1, __uint_as_float(s[i + 2]), __uint_as_float(s[i + 3]));
-          }
-          m_run = fmaxf(fmaxf(mx0, mx1) * p.scale_log2, -1.0e30f);
-        }
-        const uint32_t sPg = sP_u32 + b * Cfg::kPBox;
-        // P buffer of step j-2 consumed?  Shared-memory P: needed before the first store of the loop below.  TS: the probabilities
-        // stay in registers until the single tcgen05.st after the loop, so the check moves there (by then P V(j-2) has long retired
-        // and a non-blocking test suffices -- in front of the loop it cost every step ~200-400 cycles of barrier latency)
-        const bool late = TS && p.late_pfree;
-        if (!late && j >= 2 && !(p.early_test && p_ok)) mbar_wait(&my_pv_done[j & 1], ((j - 2) >> 1) & 1);
-        if (p.early_test) {   // tests for step j+1, consumed at its top
-          s_ok = j + 1 < n && (TS ? mbar_test(&s_full[2 * g], (j + 1) & 1) : mbar_test(&s_full[2 * g + ((j + 1) & 1)], ((j + 1) >> 1) & 1));
-          if (!late) p_ok = j + 1 < 2 || mbar_test(&my_pv_done[(j + 1) & 1], ((j - 1) >> 1) & 1);
-        }
-        if (tr) trow[2] = clock64();
-#pragma unroll 1
-        for (int pass = 0;; ++pass) {
-          // Single pass with a STALE stabiliser (the running max of the previous steps); this step's max is accumulated in
-          // the same loop.  Only when a row's new max exceeds the stabiliser by more than kRescale5 (P could overflow
-          // fp16) is the step redone with the updated stabiliser -- after the first few steps that never happens.
-          float mx0 = -INFINITY, mx1 = -INFINITY;
-          const uint64_t nm2 = pack2(kPBias - m_run, kPBias - m_run);
-          uint32_t pk[16];           // TS: the 32 probabilities of this thread's row, key pairs packed (even key in the low half)
-#pragma unroll
-          for (int c16 = 0; c16 < 4; ++c16) {
-            uint4 q;
-            uint32_t* qw = reinterpret_cast<uint32_t*>(&q);
-#pragma unroll
-            for (int t = 0; t < 4; ++t) {
-              const int i = c16 * 8 + 2 * t;
-              const float s0 = __uint_as_float(s[i]), s1 = __uint_as_float(s[i + 1]);
-              if (t & 1) mx1 = fmax3(mx1, s0, s1); else mx0 = fmax3(mx0, s0, s1);
-              float y0, y1;
-              unpack2(ffma2(pack2u(s[i], s[i + 1]), sc2, nm2), y0, y1);
-              qw[t] = pack_f16x2(ex2_approx(y0), ex2_approx(y1));
-              if (TS) pk[c16 * 4 + t] = qw[t];
-            }
-            if (!TS) st_shared_v4(sPg + p_off[c16], q);
-          }
-          if (TS) {
-            // "P buffer of step j-2 consumed" needs no barrier of its own here: the MMA warp issued P V(j-2) BEFORE Q K^T(j), tcgen05
-            // operations of one thread complete in order and tcgen05.commit tracks all of its earlier ones, so having seen
-            // s_full(j) at the top of this step already implies P V(j-2) has retired (late_pfree = 0 keeps the explicit wait)
-            tmem_st16(tmem_base + lane_addr + Cfg::kColP + (uint32_t)(b * 32 + h * 16), pk);
-          }
-          if (pass > 0 || j == 0) break;
-          const float m_new = fmaxf(mx0, mx1) * p.scale_log2;
-          if (!__any_sync(0xffffffffu, m_new - m_run > kRescale5)) break;
-          if (p.dbg && lane == 0) atomicAdd(p.dbg, 1ull);
-          // rare: O_g,h must be stable -> this half's PV of the previous step has to be complete
-          const float m_up = fmaxf(m_run, m_new);
-          mbar_wait(&my_pv_done[(j - 1) & 1], ((j - 1) >> 1) & 1);
-          tc_fence_after();
-          const float alpha = ex2_approx(m_run - m_up);
-#pragma unroll 1
-          for (int c = 0; c < Cfg::kOChunks; ++c) {
-            uint32_t o[16];
-            tmem_ld16(tmem_O + lane_addr + c * 16, o);
-            tmem_wait_ld();
-#pragma unroll
-            for (int i = 0; i < 16; ++i) o[i] = __float_as_uint(__uint_as_float(o[i]) * alpha);
-            tmem_st16(tmem_O + lane_addr + c * 16, o);
-          }
-          tmem_wait_st();
-          m_run = m_up;
-        }
-        if (tr) trow[3] = clock64();
-        if (TS) tmem_wait_st(); else fence_proxy_async_smem();
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&my_p_full[j & 1]);
-        if (tr) trow[4] = clock64();
-      }
-      // ---- epilogue: merge the two halves' partial softmax states; this half writes its chunks of the rows
-      if (ctr && threadIdx.x == 0) ctr[3] = clock64();
-      mbar_wait(&o_full[g], 0);
-      tc_fence_after();
-      if (ctr && threadIdx.x == 0) ctr[4] = clock64();
-      sMx[(g * 2 + h) * 128 + r] = m_run;
-      asm volatile("bar.sync %0, 64;" ::"r"(pair_bar) : "memory");
-      const float m_oth = sMx[(g * 2 + (h ^ 1)) * 128 + r];
-      const float m_all = fmaxf(m_run, m_oth);
-      const float w_mine = ex2_approx(m_run - m_all), w_oth = ex2_approx(m_oth - m_all);
-      const float w0 = h ? w_oth : w_mine, w1 = h ? w_mine : w_oth;
-      const uint32_t tO0 = tmem_base + Cfg::kColO + 2 * g * 64 + lane_addr, tO1 = tO0 + 64;
-      float inv;
-      {
-        uint32_t o0[16], o1[16];
-        tmem_ld16(tO0 + (D / 16) * 16, o0);
-        tmem_ld16(tO1 + (D / 16) * 16, o1);
-        tmem_wait_ld();
-        inv = p.out_scale / (w0 * __uint_as_float(o0[D % 16]) + w1 * __uint_as_float(o1[D % 16]));
-      }
-      const float a0 = w0 * inv, a1 = w1 * inv;
-      const int qt = qt0 + g;
-      const int q_i1 = (qt % p.q_t1) * p.q_box1, q_i2 = (qt / p.q_t1) * p.q_box2;
-      const bool row_ok = r < p.rows_q;
-      const int i1 = q_i1 + r % p.q_box1;
-      const int i2 = q_i2 + r / p.q_box1;
-      __half* orow = p.out + (int64_t)i1 * p.os1 + (int64_t)i2 * p.os2 + (int64_t)q_i3 * p.os3 + (int64_t)q_i4 * p.os4 + head * D;
-#pragma unroll 1
-      for (int c = oc0; c < oc1; ++c) {
-        if (c * 16 >= D) break;
-        uint32_t o[16], o1[16];
-        tmem_ld16(tO0 + c * 16, o);
-        tmem_ld16(tO1 + c * 16, o1);
-        tmem_wait_ld();
-        if (row_ok) {
-#pragma unroll
-          for (int gq = 0; gq < 2; ++gq) {
-            if (c * 16 + gq * 8 < D) {
-              uint4 q;
-              __half2* hh = reinterpret_cast<__half2*>(&q);
-              float v[8];
-#pragma unroll
-              for (int t = 0; t < 8; ++t) v[t] = a0 * __uint_as_float(o[gq * 8 + t]) + a1 * __uint_as_float(o1[gq * 8 + t]);
-              if (p.accumulate) {
-                const uint4 old = *reinterpret_cast<const uint4*>(orow + c * 16 + gq * 8);
-                const __half2* ho = reinterpret_cast<const __half2*>(&old);
-#pragma unroll
-                for (int t = 0; t < 4; ++t) {
-                  const float2 f = __half22float2(ho[t]);
-                  v[2 * t] += f.x;
-                  v[2 * t + 1] += f.y;
-                }
-              }
-#pragma unroll
-              for (int t = 0; t < 4; ++t) hh[t] = __floats2half2_rn(v[2 * t], v[2 * t + 1]);
-              *reinterpret_cast<uint4*>(orow + c * 16 + gq * 8) = q;
-            }
-          }
-        }
-      }
-    }
-  }
-  if (ctr && threadIdx.x == 0) ctr[5] = clock64();
-  tc_fence_before();
-  __syncthreads();
-  if (ctr && threadIdx.x == 0) ctr[6] = clock64();
-  if (warp == Cfg::kAllocWarp) tmem_dealloc<Cfg::kTmemCols>(tmem_base);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -1179,7 +302,7 @@ __global__ void attn_simt_kernel(ViewDev q, ViewDev k, ViewDev v, __half* out, i
 
 // ---------------------------------------------------------------------------------------------------------------
 // Few-keys attention (IP-adapter image tokens: 4 keys per image group).  The tensor path would spend a whole CTA
-// life-cycle (TMEM allocation, barrier set-up, TMA round trips) on one 64-key step that is 94% padding; the work itself
+// life-cycle (barrier set-up, TMA round trips) on one 64-key step that is 94% padding; the work itself
 // is a read of Q and a read-modify-write of the output.  One thread per (query row, head): fp32 math, 16-byte loads,
 // K/V of the image group stay in L1.  HBM-bound: ~(|Q| + 2|out|) bytes.
 // ---------------------------------------------------------------------------------------------------------------
@@ -1283,8 +406,8 @@ attn_fewkeys_kernel(ViewDev q, ViewDev k, ViewDev v, __half* out, int64_t os1, i
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// Short-key attention (text cross-attention: 77 keys shared by the F frames of an image group).  A tcgen05 CTA would live for
-// two 64-key steps, so its set-up (TMEM allocation, barrier init, TMA round trips) dominated: 4096 CTAs x ~7 us.  Here the
+// Short-key attention (text cross-attention: 77 keys shared by the F frames of an image group).  A tensor-path CTA would live
+// for two 64-key steps, so its set-up (barrier init, TMA round trips) would dominate.  Here the
 // 77 keys/values of a (key batch, head) are staged once per block in shared memory (zero-padded to 80 rows) and each warp
 // walks 16-row query tiles with mma.sync.m16n8k16: S (16 x 80) and P stay in registers, V^T fragments come from
 // ldmatrix.trans.  HBM-bound (Q in, O out).
@@ -1435,7 +558,8 @@ static int launch_shortkeys(const a3d_attn_args* a, int dqk, int dv, int kv_div,
   }
   const int Lq = a->q.e1 * a->q.e2;
   int rows_per_block = 256;                       // 4 x 64-row rounds per block amortise the K/V staging
-  while (rows_per_block > 64 && (int64_t)((Lq + rows_per_block - 1) / rows_per_block) * a->heads * batches < 1184) rows_per_block /= 2;
+  while (rows_per_block > 64 && (int64_t)((Lq + rows_per_block - 1) / rows_per_block) * a->heads * batches < 8 * sm_count())
+    rows_per_block /= 2;
   dim3 grid((unsigned)((Lq + rows_per_block - 1) / rows_per_block), (unsigned)a->heads, (unsigned)batches);
   attn_shortkeys_kernel<D><<<grid, 128, Cfg::kSmem, st>>>(q, k, v, reinterpret_cast<__half*>(a->out), a->os1, a->os2, a->os3, a->os4,
                                                           dqk, dv, a->scale * 1.4426950408889634f, kv_div, a->kv_i3_zero,
@@ -1465,21 +589,7 @@ static int view_map(const a3d_view5& v, int box1, int box2, const CUtensorMap** 
   return get_tensor_map(k, out);
 }
 
-template <int D>
-static int launch_attn(const AttnDev& dev, const CUtensorMap* mq, const CUtensorMap* mk, const CUtensorMap* mv, dim3 grid,
-                       cudaStream_t st) {
-  using Cfg = AttnCfg<D>;
-  static bool attr_set = false;
-  if (!attr_set) {
-    A3D_CUDA_CHECK(cudaFuncSetAttribute(attn_tc_kernel<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
-    attr_set = true;
-  }
-  attn_tc_kernel<D><<<grid, 192, Cfg::kSmemBytes, st>>>(dev, *mq, *mk, *mv);
-  A3D_LAUNCH_CHECK();
-  return A3D_OK;
-}
-
-// key tiles of 64 rows (v4 / v5 kernels)
+// key tiles of 64 rows
 static int tile_geom_k64(const a3d_view5& v, int* box1, int* box2, int* t1, int* tiles, int* rows_last) {
   if (v.e1 >= 64) {
     *box1 = 64; *box2 = 1; *t1 = (v.e1 + 63) / 64; *tiles = *t1 * v.e2;
@@ -1494,12 +604,9 @@ static int tile_geom_k64(const a3d_view5& v, int* box1, int* box2, int* t1, int*
   return 0;
 }
 
-static int g_attn_g1 = 1;      // head-dim-40 kernel: one 128-query tile per CTA, two CTAs per SM (prologue / epilogue of one overlaps the other)
-static int g_attn_late_pfree = 1;
-
-template <int D, bool TS, int G>
-static int launch_attn5(AttnDev dev, const a3d_attn_args* a, const CUtensorMap* mq, dim3 grid, cudaStream_t st) {
-  using Cfg = Attn5Cfg<D, G>;
+template <int D>
+static int launch_attn(AttnDev dev, const a3d_attn_args* a, const CUtensorMap* mq, dim3 grid, cudaStream_t st) {
+  using Cfg = AttnCfg<D>;
   int kb1, kb2, kt1, ktiles, klast;
   if (int r = tile_geom_k64(a->k, &kb1, &kb2, &kt1, &ktiles, &klast)) return r;
   dev.kv_tiles = ktiles; dev.rows_k = klast; dev.k_t1 = kt1; dev.k_box1 = kb1; dev.k_box2 = kb2;
@@ -1509,39 +616,15 @@ static int launch_attn5(AttnDev dev, const a3d_attn_args* a, const CUtensorMap* 
   if (int r = view_map(a->v, kb1, kb2, &mv)) return r;
   static bool attr_set = false;
   if (!attr_set) {
-    A3D_CUDA_CHECK(cudaFuncSetAttribute(attn5_tc_kernel<D, TS, G>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
+    A3D_CUDA_CHECK(cudaFuncSetAttribute(attn_tc_kernel<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
     attr_set = true;
   }
-  if (G == 2) grid.x = (grid.x + 1) / 2;
-  attn5_tc_kernel<D, TS, G><<<grid, Cfg::kThreads, Cfg::kSmemBytes, st>>>(dev, *mq, *mk, *mv);
-  A3D_LAUNCH_CHECK();
-  return A3D_OK;
-}
-
-template <int D, int POLY>
-static int launch_attn4(AttnDev dev, const a3d_attn_args* a, const CUtensorMap* mq, dim3 grid, cudaStream_t st) {
-  using Cfg = Attn4Cfg<D>;
-  int kb1, kb2, kt1, ktiles, klast;
-  if (int r = tile_geom_k64(a->k, &kb1, &kb2, &kt1, &ktiles, &klast)) return r;
-  dev.kv_tiles = ktiles; dev.rows_k = klast; dev.k_t1 = kt1; dev.k_box1 = kb1; dev.k_box2 = kb2;
-  dev.k_box_bytes = 128u * (uint32_t)(kb1 * kb2);
-  const CUtensorMap *mk, *mv;
-  if (int r = view_map(a->k, kb1, kb2, &mk)) return r;
-  if (int r = view_map(a->v, kb1, kb2, &mv)) return r;
-  static bool attr_set = false;
-  if (!attr_set) {
-    A3D_CUDA_CHECK(cudaFuncSetAttribute(attn4_tc_kernel<D, POLY>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
-    attr_set = true;
-  }
-  grid.x = (grid.x + 1) / 2;
-  attn4_tc_kernel<D, POLY><<<grid, 640, Cfg::kSmemBytes, st>>>(dev, *mq, *mk, *mv);
+  attn_tc_kernel<D><<<grid, kAttnThreads, Cfg::kSmemBytes, st>>>(dev, *mq, *mk, *mv);
   A3D_LAUNCH_CHECK();
   return A3D_OK;
 }
 
 static unsigned long long* g_attn_dbg = nullptr;
-static int g_attn_early = 1;
-static int g_attn_ts = 1;      // head-dim-40 kernel: probabilities through tensor memory (TS-mode P V product)
 
 }  // namespace a3d
 
@@ -1575,8 +658,8 @@ extern "C" int a3d_attention(const a3d_attn_args* a, void* stream) {
 
   if ((a->os1 | a->os2 | a->os3 | a->os4) % 8 || (reinterpret_cast<uintptr_t>(a->out) & 15))
     return fail(A3D_EINVAL, "a3d_attention: output rows must be 16-byte aligned");
-  // impl == AUTO picks the kernel by key count; an explicit A3D_GEMM_TCGEN05 forces the tcgen05 kernels (tests use it to keep
-  // their ragged-key paths covered)
+  // impl == AUTO picks the kernel by key count; an explicit A3D_GEMM_TCGEN05 forces the tensor-core kernel (tests use it to
+  // keep its ragged-key paths covered)
   const bool auto_impl = a->impl == A3D_GEMM_AUTO;
   if (auto_impl && a->k.e1 * a->k.e2 <= kFewKeysMax) {
     // a handful of keys (IP-adapter image tokens): HBM-bound thread-per-(row, head) kernel, see attn_fewkeys_kernel
@@ -1617,60 +700,34 @@ extern "C" int a3d_attention(const a3d_attn_args* a, void* stream) {
 
   AttnDev dev;
   memset(&dev, 0, sizeof(dev));
-  int qb1, qb2, qt1, qtiles, qrows, kb1, kb2, kt1, ktiles, krows;
+  int qb1, qb2, qt1, qtiles, qrows;
   if (int r = tile_geom(a->q, &qb1, &qb2, &qt1, &qtiles, &qrows)) return r;
-  if (d == 160) {   // 128-key steps (v1 kernel); head_dim 40 / 80 use 64-key steps and set their own key geometry (ragged ok)
-    if (int r = tile_geom(a->k, &kb1, &kb2, &kt1, &ktiles, &krows)) return r;
-  } else {
-    kb1 = kb2 = kt1 = ktiles = krows = 0;
-  }
-  dev.q_tiles = qtiles; dev.kv_tiles = ktiles; dev.rows_q = qrows; dev.rows_k = krows;
+  dev.q_tiles = qtiles; dev.rows_q = qrows;
   dev.heads = a->heads;
   dev.q_t1 = qt1; dev.q_box1 = qb1; dev.q_box2 = qb2; dev.q_e3 = a->q.e3;
-  dev.k_t1 = kt1; dev.k_box1 = kb1; dev.k_box2 = kb2; dev.k_e3 = a->k.e3;
+  dev.k_e3 = a->k.e3;
   dev.kv_div = kv_div; dev.kv_i3_zero = a->kv_i3_zero;
-  dev.q_box_bytes = 128u * qrows; dev.k_box_bytes = 128u * krows;
+  dev.q_box_bytes = 128u * qrows;
   dev.scale_log2 = a->scale * 1.4426950408889634f;
   dev.out = reinterpret_cast<__half*>(a->out);
   dev.os1 = a->os1; dev.os2 = a->os2; dev.os3 = a->os3; dev.os4 = a->os4;
   dev.accumulate = a->accumulate;
   dev.out_scale = a->out_scale == 0.f ? 1.f : a->out_scale;
   dev.dbg = g_attn_dbg;
-  dev.early_test = g_attn_early;
-  dev.late_pfree = g_attn_late_pfree;
-  if ((a->os1 | a->os2 | a->os3 | a->os4) % 8 || (reinterpret_cast<uintptr_t>(a->out) & 15))
-    return fail(A3D_EINVAL, "a3d_attention: output rows must be 16-byte aligned");
-  const CUtensorMap *mq, *mk, *mv;
+  const CUtensorMap* mq;
   if (int r = view_map(a->q, qb1, qb2, &mq)) return r;
-  mk = mv = nullptr;
-  if (d == 160) {
-    if (int r = view_map(a->k, kb1, kb2, &mk)) return r;
-    if (int r = view_map(a->v, kb1, kb2, &mv)) return r;
-  }
   dim3 grid(qtiles, a->heads, batches);
   if (batches > 65535 || a->heads > 65535) return fail(A3D_EINVAL, "a3d_attention: grid too large");
   switch (d) {
-    case 40:
-      if (g_attn_g1) return g_attn_ts ? launch_attn5<40, true, 1>(dev, a, mq, grid, st) : launch_attn5<40, false, 1>(dev, a, mq, grid, st);
-      return g_attn_ts ? launch_attn5<40, true, 2>(dev, a, mq, grid, st) : launch_attn5<40, false, 2>(dev, a, mq, grid, st);
-    case 80:
-      return launch_attn4<80, 0>(dev, a, mq, grid, st);
-    default: return launch_attn<160>(dev, mq, mk, mv, grid, st);
+    case 40: return launch_attn<40>(dev, a, mq, grid, st);
+    case 80: return launch_attn<80>(dev, a, mq, grid, st);
+    default: return launch_attn<160>(dev, a, mq, grid, st);
   }
 }
 
-// debug hook (not part of the product path): device counter the softmax warps of the tcgen05 kernels bump whenever they
-// take the lazy-rescale branch (tests assert that adversarial inputs really exercise it); null switches it off
-extern "C" int a3d_debug_set_attn_trace(void* device_counter_u64) {   // buffer of >= 8 + 4*32*8 uint64
+// debug hook (not part of the product path): device counter the softmax of the tensor-core kernel bumps whenever a warp takes
+// the lazy-rescale branch (tests assert that adversarial inputs really exercise it); null switches it off
+extern "C" int a3d_debug_set_attn_trace(void* device_counter_u64) {
   a3d::g_attn_dbg = reinterpret_cast<unsigned long long*>(device_counter_u64);
-  return A3D_OK;
-}
-
-// tuning hook (tools/attn_timeline.py): 0 switches the one-step-ahead non-blocking barrier tests of the head-dim-40 kernel off
-extern "C" int a3d_debug_set_attn_poly(int flags) {   // bit 0: early barrier tests, bit 1: P through tensor memory (TS-mode P V)
-  a3d::g_attn_early = flags & 1;
-  a3d::g_attn_ts = (flags >> 1) & 1;
-  a3d::g_attn_g1 = (flags >> 2) & 1;
-  a3d::g_attn_late_pfree = (flags >> 3) & 1;
   return A3D_OK;
 }

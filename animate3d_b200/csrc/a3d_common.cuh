@@ -1,5 +1,5 @@
-// animate3d_b200 -- sm_100a device helpers: mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (MMA / TMEM), descriptors.
-// Everything here is inline PTX for sm_100a; there is no other backend.
+// animate3d_b200 -- sm_90a device helpers: mbarrier, TMA (cp.async.bulk.tensor), wgmma fences and descriptors.
+// Everything here is inline PTX for sm_90a; there is no other backend.
 #pragma once
 #include <cuda.h>
 #include <cuda_fp16.h>
@@ -13,18 +13,6 @@ namespace a3d {
 // small utilities
 // ---------------------------------------------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
-__device__ __forceinline__ uint32_t lane_id() { return threadIdx.x & 31; }
-
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred = 0;
-  asm volatile(
-      "{\n\t.reg .pred P;\n\t"
-      "elect.sync _|P, 0xffffffff;\n\t"
-      "selp.b32 %0, 1, 0, P;\n\t}\n"
-      : "=r"(pred));
-  return pred != 0;
-}
 
 // ---------------------------------------------------------------------------------------------------------------
 // mbarrier
@@ -52,29 +40,13 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
   return ok != 0;
 }
 // Spin on the barrier phase.  A pipeline bug would otherwise hang the GPU forever; after ~4 s of waiting the kernel
-// traps so that the host sees a launch failure instead (the check costs nothing on the fast path).
-// non-blocking phase test: the result can be consumed long after the instruction issues (used to hide the barrier latency
-// behind independent work); follow up with mbar_wait when it returns false
-__device__ __forceinline__ bool mbar_test(uint64_t* bar, uint32_t parity) {
-  uint32_t ok;
-  asm volatile(
-      "{\n\t.reg .pred P;\n\t"
-      "mbarrier.test_wait.parity.shared::cta.b64 P, [%1], %2;\n\t"
-      "selp.b32 %0, 1, 0, P;\n\t}\n"
-      : "=r"(ok)
-      : "r"(smem_u32(bar)), "r"(parity)
-      : "memory");
-  return ok != 0;
-}
+// traps so that the host sees a launch failure instead (the check costs nothing on the fast path).  No printf here: a call
+// inside the wgmma main loops would make ptxas serialise the asynchronous MMAs.
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   if (mbar_try_wait(bar, parity)) return;
   const long long t0 = clock64();
   while (!mbar_try_wait(bar, parity)) {
-    if (clock64() - t0 > 8000000000ll) {
-      printf("a3d: mbarrier wait timed out (block %d,%d,%d thread %d bar@%u parity %u)\n", blockIdx.x, blockIdx.y,
-             blockIdx.z, threadIdx.x, smem_u32(bar), parity);
-      __trap();
-    }
+    if (clock64() - t0 > 8000000000ll) __trap();
   }
 }
 
@@ -94,235 +66,64 @@ __device__ __forceinline__ void tma_load_5d(void* smem_dst, const CUtensorMap* m
         "r"(c3), "r"(c4)
       : "memory");
 }
-// TMA store: shared -> global, bulk-group completion (the issuing thread commits / waits)
-__device__ __forceinline__ void tma_store_5d(const CUtensorMap* map, const void* smem_src, int c0, int c1, int c2, int c3, int c4) {
-  asm volatile("cp.async.bulk.tensor.5d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5, %6}], [%1];"
-               :
-               : "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(smem_src)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4)
-               : "memory");
-}
-__device__ __forceinline__ void tma_store_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-__device__ __forceinline__ void tma_store_wait_read() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
-__device__ __forceinline__ void tma_store_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
-// generic-proxy writes to smem (st.shared) -> visible to the async proxy (UMMA / TMA reads)
-__device__ __forceinline__ uint32_t ld_volatile_shared(uint32_t addr) {
-  uint32_t v;
-  asm volatile("ld.volatile.shared.u32 %0, [%1];" : "=r"(v) : "r"(addr) : "memory");
-  return v;
-}
-__device__ __forceinline__ void red_add_shared(uint32_t addr, uint32_t v) {
-  asm volatile("red.shared.add.u32 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
-}
+// generic-proxy writes to smem (st.shared) -> visible to the async proxy (wgmma / TMA reads)
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
-// ---------------------------------------------------------------------------------------------------------------
-// tcgen05: TMEM allocation, MMA, commit, ld/st, fences
-// ---------------------------------------------------------------------------------------------------------------
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst) {  // one full warp
-  static_assert(kCols == 32 || kCols == 64 || kCols == 128 || kCols == 256 || kCols == 512, "pow2 >= 32");
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)), "n"(kCols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {  // same warp that allocated
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(kCols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// D[tmem] (+)= A[smem desc] * B[smem desc]; issued by ONE thread.
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}\n"
-      :
-      : "r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// D[tmem] (+)= A[tmem] * B[smem desc]: the A operand (M = 128 rows = TMEM lanes, K packed two fp16 per 32-bit column) is read
-// from tensor memory -- e.g. softmax probabilities written there with tcgen05.st, no shared-memory round trip.
-__device__ __forceinline__ void umma_f16_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}\n"
-      :
-      : "r"(tmem_d), "r"(tmem_a), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// arrives on `bar` when every tcgen05.mma previously issued by this thread has completed
-// (implicitly performs tcgen05.fence::before_thread_sync)
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-
-// TMEM -> registers: warp w may touch lanes [32*(w%4), 32*(w%4)+32); thread = lane (row), N consecutive 32-bit columns.
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-// pointer flavours (the caller guarantees r[0..N) are registers, i.e. only static indexing)
-__device__ __forceinline__ void tmem_ld32p(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld16p(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld64(uint32_t taddr, uint32_t (&r)[64]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x64.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
-      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
-      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, [%64];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31]), "=r"(r[32]),
-        "=r"(r[33]), "=r"(r[34]), "=r"(r[35]), "=r"(r[36]), "=r"(r[37]), "=r"(r[38]), "=r"(r[39]), "=r"(r[40]),
-        "=r"(r[41]), "=r"(r[42]), "=r"(r[43]), "=r"(r[44]), "=r"(r[45]), "=r"(r[46]), "=r"(r[47]), "=r"(r[48]),
-        "=r"(r[49]), "=r"(r[50]), "=r"(r[51]), "=r"(r[52]), "=r"(r[53]), "=r"(r[54]), "=r"(r[55]), "=r"(r[56]),
-        "=r"(r[57]), "=r"(r[58]), "=r"(r[59]), "=r"(r[60]), "=r"(r[61]), "=r"(r[62]), "=r"(r[63])
-      : "r"(taddr)
-      : "memory");
-}
-// 256-bit global accesses (sm_100: LDG/STG.E.ENL2.256): one full 32-byte sector per lane per instruction
+// 32-byte global accesses as two 16-byte vector instructions (sm_90 has no 256-bit LDG / STG): the pair still covers one
+// whole 32-byte sector per lane
 __device__ __forceinline__ void st_global_256(void* ptr, const uint32_t* r) {
-  asm volatile("st.global.v8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"l"(ptr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]),
-               "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7])
+  asm volatile("st.global.v4.b32 [%0], {%1, %2, %3, %4};" ::"l"(ptr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]) : "memory");
+  asm volatile("st.global.v4.b32 [%0], {%1, %2, %3, %4};" ::"l"(reinterpret_cast<uint8_t*>(ptr) + 16), "r"(r[4]), "r"(r[5]),
+               "r"(r[6]), "r"(r[7])
                : "memory");
-}
-__device__ __forceinline__ void ld_global_256(const void* ptr, uint32_t* r) {
-  asm volatile("ld.global.v8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-               : "l"(ptr)
-               : "memory");
-}
-// single-instruction math used by the softmax warps
-// 2^y on the FMA/ALU pipes only (no MUFU): y <= 127, flushes to ~1e-38 below -126.  Round-to-nearest split y = n + f with
-// the 1.5*2^23 magic constant (n lands in the low mantissa bits of t), degree-3 minimax polynomial for 2^f on [-0.5, 0.5]
-// (max relative error 7.5e-5), exponent added with one integer add.
-__device__ __forceinline__ float exp2_fma(float y) {
-  y = fmaxf(y, -126.0f);
-  const float t = y + 12582912.0f;
-  const float f = y - (t - 12582912.0f);
-  float r = fmaf(0.0551716685295105f, f, 0.2426111251115799f);
-  r = fmaf(r, f, 0.6932609677314758f);
-  r = fmaf(r, f, 0.9999280571937561f);
-  return __uint_as_float(__float_as_uint(r) + (__float_as_uint(t) << 23));
 }
 
+// single-instruction math used by the softmax code
 __device__ __forceinline__ float ex2_approx(float x) {
   float y;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
 }
-__device__ __forceinline__ float fmax3(float a, float b, float c) {
-  float r;
-  asm("max.f32 %0, %1, %2, %3;" : "=f"(r) : "f"(a), "f"(b), "f"(c));
-  return r;
-}
-// Pack two probabilities into an fp16 pair WITHOUT the XU-pipe F2FP conversion.  The caller evaluates
-// e = ex2(x - 112) = P * 2^-112 (flushed to 0 below 2^-126, i.e. P < 2^-14 = fp16 min normal); for such e the fp32 bit
-// pattern shifted right by 13 IS the fp16 bit pattern of P (exponent field E-112+... lines up, mantissa truncated), so
-// rounding is an integer add and the pack is shift/mask on the ALU + FMA pipes.  Valid for 0 <= P < 65536.
-__device__ __forceinline__ uint32_t pack_f16x2_scaled(float e_lo, float e_hi) {
-  const uint32_t lo = (__float_as_uint(e_lo) + 0x1000u) >> 13;
-  const uint32_t hi = (__float_as_uint(e_hi) * 8u + 0x8000u) & 0xFFFF0000u;
-  return hi | lo;
-}
-constexpr float kPackBias = 112.0f;
 __device__ __forceinline__ uint32_t pack_f16x2(float lo, float hi) {
   uint32_t d;
   asm("cvt.rn.f16x2.f32 %0, %1, %2;" : "=r"(d) : "f"(hi), "f"(lo));
   return d;
 }
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};"
-      :
-      : "r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]),
-        "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
 // ---------------------------------------------------------------------------------------------------------------
-// UMMA descriptors (bit layouts: cute/arch/mma_sm100_desc.hpp in CUTLASS 4.x; restated, not included)
+// wgmma (sm_90a warpgroup MMA): fences, commit / wait, shared-memory matrix descriptors
 // ---------------------------------------------------------------------------------------------------------------
-// Shared-memory matrix descriptor, SWIZZLE_128B, version 1 (Blackwell).  Addresses/offsets are encoded >> 4.
+// Accumulator registers touched by ordinary code must be fenced before the next wgmma reads them.
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accumulator reads / writes across an asynchronous wgmma (register operands only)
+template <int R>
+__device__ __forceinline__ void reg_fence(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+// Shared-memory matrix descriptor, SWIZZLE_128B (bit layout: PTX ISA, "Matrix Descriptor Format" of wgmma).  Addresses and
+// offsets are encoded >> 4; tiles are 1024-byte aligned, so the base-offset field stays 0.
 //   K-major operand  : tile = R rows x 64 halves (128 B/row), 8-row groups 1024 B apart  -> SBO = 1024, LBO unused (1)
 //   MN-major operand : atom = 64 (MN, contiguous) x 8 (K) halves = 1024 B; next 8 K-rows at SBO = 1024;
 //                      next 64 MN elements at LBO = bytes of one TMA box (rows * 128 B)
+// Stepping 16 halves along K inside a K-major atom adds 32 B to the start address (+2 in the encoded field).
 __device__ __forceinline__ uint64_t make_smem_desc_sw128(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
   d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
   d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 46;  // version = 1
-  d |= (uint64_t)2 << 61;  // layout_type = SWIZZLE_128B
+  d |= (uint64_t)1 << 62;  // layout_type = SWIZZLE_128B
   return d;
 }
-// Instruction descriptor for kind::f16 with fp16 (or, per operand, bf16) A/B and fp32 accumulate.
-__host__ __device__ constexpr uint32_t make_idesc_f16(uint32_t M, uint32_t N, bool a_mn_major, bool b_mn_major,
-                                                      bool a_bf16 = false, bool b_bf16 = false) {
-  return (1u << 4)                          // c_format = F32
-         | ((a_bf16 ? 1u : 0u) << 7)        // a_format: 0 = F16, 1 = BF16
-         | ((b_bf16 ? 1u : 0u) << 10)       // b_format
-         | ((a_mn_major ? 1u : 0u) << 15)   // a_major
-         | ((b_mn_major ? 1u : 0u) << 16)   // b_major
-         | ((N >> 3) << 17)                 // n_dim
-         | ((M >> 4) << 24);                // m_dim
-}
 
-// legacy warp-level MMA (fp16 x fp16 -> fp32), used where a problem is far below a tcgen05 tile (16-frame temporal
+// warp-level MMA (fp16 x fp16 -> fp32), used where a problem is far below a 64-row warpgroup tile (16-frame temporal
 // attention, 77-key text cross-attention)
 __device__ __forceinline__ void mma_16816(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
   asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
                : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
                : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
 }
-
-// byte offset of logical element (row r, 16-byte chunk c16 in [0,8)) inside a SWIZZLE_128B K-major tile whose base is
-// 1024-byte aligned: Swizzle<3,4,3> XORs address bits [4,7) with bits [7,10).
-__device__ __forceinline__ uint32_t sw128_offset(uint32_t r, uint32_t c16) { return r * 128u + ((c16 ^ (r & 7u)) << 4); }
 
 }  // namespace a3d

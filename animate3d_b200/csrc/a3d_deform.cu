@@ -507,7 +507,7 @@ extern "C" int a3d_deform_backward(const a3d_deform_args* a, const float* g_mean
   const long long n = (long long)a->P * a->T;
   const size_t smem = (3 * kHid * kHid + 3 * 4 * kHid + 3 * kBwdThreads * kLdS + kBwdThreads * 4 + 3 * kOwn * kBwdThreads) * sizeof(float);
   static bool attr = false;
-  static int sms = 148;
+  static int sms = 0;
   if (!attr) {
     A3D_CUDA_CHECK(cudaFuncSetAttribute(deform_backward_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     int dev = 0;

@@ -1,7 +1,8 @@
-// a3d_gemm: C = epilogue(A * B^T) on 5th-gen tensor cores.
-//   * persistent, warp-specialised: warp 0 = TMA producer, warp 1 = tcgen05.mma issuer, warps 2..5 = epilogue
-//   * operands staged by TMA into 128B-swizzled shared memory (K-major), accumulators double-buffered in TMEM so the
-//     epilogue of tile i overlaps the main loop of tile i+1
+// a3d_gemm: C = epilogue(A * B^T) on Hopper tensor cores (wgmma).
+//   * persistent, warp-specialised: warp 8 = TMA producer, warpgroups 0 and 1 = consumers; each consumer warpgroup owns 64 rows
+//     of the 128-row tile, issues wgmma.mma_async on the staged operands and runs the epilogue straight from its fp32
+//     accumulator registers while the producer already fills the ring for the next tile
+//   * operands staged by TMA into 128B-swizzled shared memory (K-major) through a ring of mbarrier-guarded stages
 //   * A3D_A_CONV3: the A operand is an implicit 3x3 im2col of an NHWC image -- each k-block is one (tap, 64-channel)
 //     slice fetched with a rank-4 TMA box whose out-of-bounds rows/cols are zero-filled by the hardware (= padding 1);
 //     stride-2 convolutions use the tensor map's traversal strides
@@ -11,6 +12,7 @@
 
 #include "a3d_common.cuh"
 #include "a3d_host.cuh"
+#include "a3d_wgmma.cuh"
 
 namespace a3d {
 
@@ -31,9 +33,6 @@ struct GemmDev {
   const float* bias;
   const float* rowbias;
   int64_t rb_ld, rb_div, rb_mod;
-  int rb_stage;   // row-bias table rows a 128-row tile touches are staged in shared memory: 0 = no (global loads),
-                  // 1 = slot = row_in_tile / rb_div (rb_div >= 8 divides 128, or rb_div % 128 == 0), 2 = slot = row_in_tile % rb_mod
-  int rb_slots;   // distinct table rows per tile (<= 16)
   float acc_scale;
   const __half* R1; int64_t ldr1; float r1_scale;
   const __half* R2; int64_t ldr2;
@@ -41,16 +40,13 @@ struct GemmDev {
   int geglu, out_f32;
   int64_t perm_a, perm_b;
   long long* trace;   // debug: per-tile clock64 timestamps of CTA 0 (null in production), see a3d_debug_set_gemm_trace
-  int dbg_nostore;    // debug (A3D_GEMM_NOSTORE=1): compute the epilogue but skip the global stores -- timing experiments only
-  int tma_store;      // epilogue writes through shared memory + TMA bulk stores (full 128-byte lines, asynchronous)
-  int stages;         // depth of the TMA -> MMA operand ring
 };
 
 // gelu(x) = 0.5 x (1 + erf(x / sqrt 2)) with erf from Abramowitz-Stegun 7.1.26 (|err| <= 1.5e-7, far below fp16 output
 // resolution): 1 rcp + 1 ex2 on the XU pipe + 11 FMA-pipe instructions instead of erff's ~30 (the GEGLU epilogue is ALU-bound)
 __device__ __forceinline__ float gelu_erf(float x) {
   // gelu(x) = x/2 + |x|/2 erf(|x| / sqrt 2);  erf(z) = 1 - (a1 t + .. + a5 t^5) exp(-z^2), t = 1 / (1 + 0.3275911 z).  Constants folded so
-  // that one evaluation is 7 FFMA + 4 FMUL + MUFU.RCP + MUFU.EX2 (the K = 320 GEGLU tiles are bound by epilogue instruction issue)
+  // that one evaluation is 7 FFMA + 4 FMUL + MUFU.RCP + MUFU.EX2
   float t;
   asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(t) : "f"(fmaf(0.3275911f * 0.70710678118654752f, fabsf(x), 1.0f)));
   float poly = fmaf(1.061405429f, t, -1.453152027f);
@@ -72,52 +68,40 @@ __device__ __forceinline__ int64_t perm_row(int64_t m, int64_t a, int64_t b) {
 
 constexpr int kBM = 128;
 constexpr int kBK = 64;
+constexpr int kGemmThreads = 288;   // 2 consumer warpgroups + 1 producer warp
 
 template <int BN>
 struct GemmCfg {
-  // Ring depth is a launch parameter (GemmDev::stages): short-K GEMMs do not react to it at all (measured 2/3/4 stages at
-  // BN = 256, profiles/r01_gemm_epilogue.txt) and give one stage to the TMA-store staging; the long-K implicit convolutions
-  // (5-D TMA boxes, longer latency) keep the deep ring and store directly.
-  static constexpr int kMaxStages = (BN == 256) ? 4 : (BN == 160 ? 5 : 6);
-  static constexpr int kStagesStaged = (BN == 256) ? 3 : (BN == 160 ? 5 : 5);
   static constexpr int kABytes = kBM * kBK * 2;
   static constexpr int kBBytes = BN * kBK * 2;
   static constexpr int kStageBytes = kABytes + kBBytes;
-  static constexpr int kTmemCols = (2 * BN <= 256) ? 256 : 512;
-  static constexpr int kStageOut = 2048;   // 2 x 256 fp32 bias values (double-buffered with the accumulator)
-  static constexpr int kRbLd = BN + 8;      // padded row of the staged row-bias slice (staggers the banks of the <=16 slots)
-  static constexpr int kRbBytes = 16 * kRbLd * 4;
-  // output staging for the TMA-store epilogue: one 32-row x 64-column (128 B per row, 128B-swizzled) box per epilogue warp
-  static constexpr int kOutStage = (BN == 160) ? 0 : 8 * 4096;
-  static constexpr int kTail = kStageOut + kRbBytes + 1024 /*align slack*/ + 256 /*barriers*/;
-  static constexpr int smem_bytes(bool staged) { return (staged ? kStagesStaged * kStageBytes + kOutStage : kMaxStages * kStageBytes) + kTail; }
-  static constexpr int kSmemBytes = smem_bytes(true) > smem_bytes(false) ? smem_bytes(true) : smem_bytes(false);
+  // as many stages as fit next to nothing else: the epilogue works from registers and needs no shared memory
+  static constexpr int kStages = (227 * 1024 - 1024 - 256) / kStageBytes > 6 ? 6 : (227 * 1024 - 1024 - 256) / kStageBytes;
+  static constexpr int kSmemBytes = kStages * kStageBytes + 1024 /*align slack*/ + 256 /*barriers*/;
   static_assert(kSmemBytes <= 227 * 1024, "shared memory budget");
 };
 
-// EPI: 0 = bias/row-bias only, 1 = + residuals / row permutation, 2 = GEGLU, 3 = fp32 output (register pressure and dead
-// code differ enough that one runtime-branched epilogue spilled)
+template <int BN>
+__device__ __forceinline__ void wgmma_tile(float (&d)[BN / 2], uint64_t adesc, uint64_t bdesc, uint32_t acc) {
+  if constexpr (BN == 256) wgmma_ss_n256<0>(d, adesc, bdesc, acc);
+  else if constexpr (BN == 160) wgmma_ss_n160<0>(d, adesc, bdesc, acc);
+  else wgmma_ss_n128<0>(d, adesc, bdesc, acc);
+}
+
+// EPI: 0 = bias/row-bias only, 1 = + residuals / row permutation, 2 = GEGLU, 3 = fp32 output
 enum { kEpiPlain = 0, kEpiRes = 1, kEpiGeglu = 2, kEpiF32 = 3 };
 
 template <int BN, int EPI>
-__global__ void __launch_bounds__(320, 1)
-gemm_tc_kernel(const GemmDev p, const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB,
-               const __grid_constant__ CUtensorMap mapC) {
+__global__ void __launch_bounds__(kGemmThreads, 1)
+gemm_tc_kernel(const GemmDev p, const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB) {
   using Cfg = GemmCfg<BN>;
+  constexpr int kStages = Cfg::kStages;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* smem_a = smem;
-  const int kStages = p.stages;
   uint8_t* smem_b = smem + kStages * Cfg::kABytes;
-  uint8_t* smem_out = smem + kStages * Cfg::kStageBytes;           // [8 warps][32 rows][128 B], 1024-byte aligned
-  uint8_t* smem_stage = smem_out + (p.tma_store ? Cfg::kOutStage : 0);
-  float* smem_rb = reinterpret_cast<float*>(smem_stage + Cfg::kStageOut);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem_stage + Cfg::kStageOut + Cfg::kRbBytes);
-  uint64_t* full_bar = bars;                       // [kStages]
-  uint64_t* empty_bar = bars + kStages;            // [kStages]
-  uint64_t* tfull_bar = bars + 2 * kStages;        // [2]
-  uint64_t* tempty_bar = tfull_bar + 2;            // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty_bar + 2);
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + kStages * Cfg::kStageBytes);   // [kStages]
+  uint64_t* empty_bar = full_bar + kStages;                                              // [kStages]
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -128,23 +112,14 @@ gemm_tc_kernel(const GemmDev p, const __grid_constant__ CUtensorMap mapA, const 
     tma_prefetch_desc(&mapB);
     for (int i = 0; i < kStages; ++i) {
       mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tfull_bar[i], 1);
-      mbar_init(&tempty_bar[i], 8);  // one arrive per epilogue warp
+      mbar_init(&empty_bar[i], 8);   // one arrive per consumer warp
     }
     mbar_fence_init();
   }
-  if (warp == 9) tmem_alloc<Cfg::kTmemCols>(tmem_slot);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
   if (warp == 8) {
-    // ------------------------------------------------------------------ TMA producer (highest warp ids: the scheduler
-    // prefers them, so the single-thread control warps are not starved by the 8 busy epilogue warps)
+    // ------------------------------------------------------------------ TMA producer (one thread)
     if (lane == 0) {
       int stage = 0;
       uint32_t phase = 0;
@@ -172,378 +147,100 @@ gemm_tc_kernel(const GemmDev p, const __grid_constant__ CUtensorMap mapA, const 
         }
       }
     }
-  } else if (warp == 9) {
-    // ------------------------------------------------------------------ MMA issuer (single thread)
-    if (lane == 0) {
-      constexpr uint32_t idesc = make_idesc_f16(kBM, BN, false, false);
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      int tcount = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++tcount) {
-        const bool tr = p.trace && blockIdx.x == 0 && tcount < 60;
-        if (tr) p.trace[tcount * 16 + 8] = clock64();
-        mbar_wait(&tempty_bar[acc], acc_phase ^ 1);
-        if (tr) p.trace[tcount * 16 + 9] = clock64();
-        tc_fence_after();
-        const uint32_t tmem_d = tmem_base + acc * BN;
-        for (int kb = 0; kb < p.num_k_blocks; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          const uint64_t adesc = make_smem_desc_sw128(smem_u32(smem_a + stage * Cfg::kABytes), 16, 1024);
-          const uint64_t bdesc = make_smem_desc_sw128(smem_u32(smem_b + stage * Cfg::kBBytes), 16, 1024);
+    return;
+  }
+
+  // -------------------------------------------------------------------- consumers: 2 warpgroups x 64 rows
+  const int wg = warp >> 2;
+  const int g = lane >> 2, t = lane & 3;
+  int stage = 0;
+  uint32_t phase = 0;
+  int tcount = 0;
+  float acc[BN / 2];
+  for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++tcount) {
+    const int mt = tile / p.tiles_n, nt = tile % p.tiles_n;
+    const bool tr = p.trace && blockIdx.x == 0 && threadIdx.x == 0 && tcount < 60;
+    if (tr) p.trace[tcount * 16 + 0] = clock64();
+    // ---- main loop: one wgmma group in flight; the stage of k-block kb-1 is released once group kb-1 has retired
+    int prev_stage = -1;
+    for (int kb = 0; kb < p.num_k_blocks; ++kb) {
+      mbar_wait(&full_bar[stage], phase);
+      const uint32_t a0 = smem_u32(smem_a + stage * Cfg::kABytes + wg * (64 * 128));
+      const uint32_t b0 = smem_u32(smem_b + stage * Cfg::kBBytes);
+      wgmma_fence();
 #pragma unroll
-          for (int k = 0; k < kBK / 16; ++k) {
-            // advance 16 halves (32 B) along K inside the 128B swizzle atom: +2 in the (addr >> 4) field
-            umma_f16(tmem_d, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), idesc, (kb | k) ? 1u : 0u);
-          }
-          umma_commit(&empty_bar[stage]);
-          if (kb == 0 && tr) p.trace[tcount * 16 + 10] = clock64();
-          if (kb == p.num_k_blocks - 1) umma_commit(&tfull_bar[acc]);
-          if (++stage == kStages) { stage = 0; phase ^= 1; }
-        }
-        if (tr) p.trace[tcount * 16 + 11] = clock64();
-        if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-      }
+      for (int k = 0; k < kBK / 16; ++k)
+        wgmma_tile<BN>(acc, make_smem_desc_sw128(a0 + 32 * k, 16, 1024), make_smem_desc_sw128(b0 + 32 * k, 16, 1024),
+                       (kb | k) ? 1u : 0u);
+      wgmma_commit();
+      wgmma_wait<1>();
+      if (prev_stage >= 0 && lane == 0) mbar_arrive(&empty_bar[prev_stage]);
+      prev_stage = stage;
+      if (++stage == kStages) { stage = 0; phase ^= 1; }
     }
-  } else {
-    // ------------------------------------------------------------------ epilogue (8 warps: 2 per TMEM lane quadrant)
-    // TMEM -> registers (one accumulator row per thread) -> bias / row-bias / scale / residuals in fp32 -> fp16 ->
-    // 256-bit global stores: every store instruction writes whole 32-byte sectors (the first version's 16-byte slivers
-    // of 32 different lines ran the output at < 0.7 TB/s).  Residual tiles are fetched with 256-bit loads issued before
-    // the TMEM wait.  The two warps of a quadrant split the tile's columns in units of 32.
-    const int quad = warp & 3;
-    const int half = warp >> 2;
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    int tcount = 0;
-    // row-bias table rows of a tile are FETCHED one tile ahead into registers (their global-load latency then hides behind the
-    // previous tile's epilogue instead of standing in front of this one) and only copied to shared memory at the tile's top
-    constexpr int kRbVec = BN / 4;
-    constexpr int kRbPf = (16 * kRbVec + 255) / 256;      // float4 per thread for <= 16 staged rows
-    float4 rb_pf[kRbPf];
-    auto rb_fetch = [&](int t) {
-      const int64_t tile_row0 = (int64_t)(t / p.tiles_n) * kBM;
-      const int ntf = t % p.tiles_n;
-#pragma unroll
-      for (int k = 0; k < kRbPf; ++k) {
-        const int i = threadIdx.x + 256 * k;
-        rb_pf[k] = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (i < p.rb_slots * kRbVec) {
-          const int slot = i / kRbVec, c4 = i % kRbVec;
-          const int64_t rep = tile_row0 + (p.rb_stage == 1 ? (int64_t)slot * p.rb_div : (int64_t)slot);
-          const int64_t trow = (rep / p.rb_div) % p.rb_mod;
-          const int64_t col = (int64_t)ntf * BN + c4 * 4;
-          if (col + 4 <= p.N && rep < p.M) rb_pf[k] = __ldg(reinterpret_cast<const float4*>(p.rowbias + trow * p.rb_ld + col));
-        }
-      }
-    };
-    constexpr bool kRbAhead = EPI == kEpiPlain;      // (the residual epilogue has no registers to spare; it fetches in place)
-    constexpr bool rb_ahead = kRbAhead;
-    if (rb_ahead && p.rb_stage && (int)blockIdx.x < num_tiles) rb_fetch(blockIdx.x);
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++tcount) {
-      const int mt = tile / p.tiles_n, nt = tile % p.tiles_n;
-      const bool tr = p.trace && blockIdx.x == 0 && threadIdx.x == 0 && tcount < 60;
-      if (tr) p.trace[tcount * 16 + 0] = clock64();
-      // everything that does not read the accumulator (bias / row-bias staging, the residual tile) is started BEFORE the wait
-      // for the tile's MMAs, so its latency hides behind them
-      auto wait_acc = [&]() {
-        mbar_wait(&tfull_bar[acc], acc_phase);
-        if (tr) p.trace[tcount * 16 + 1] = clock64();
-        tc_fence_after();
-      };
-      const int64_t row0 = (int64_t)mt * kBM + quad * 32;
-      const int64_t row = row0 + lane;
-      const bool row_ok = row < p.M;
-      const int64_t rbrow = (p.rowbias && row_ok) ? ((row / p.rb_div) % p.rb_mod) : 0;
-      const uint32_t taddr = tmem_base + ((uint32_t)(quad * 32) << 16) + acc * BN;
-      const int64_t n_out = (EPI == kEpiGeglu) ? p.N / 2 : p.N;
-      const bool tile_full = (int64_t)(nt + 1) * BN <= p.N;       // no ragged columns in this tile: the per-unit bounds tests fold away
-      // the tile's BN bias values: one coalesced load by the 256 epilogue threads, then broadcast reads from shared memory
-      float* sb = reinterpret_cast<float*>(smem_stage) + acc * 256;
-      // Row-bias (positional-encoding / time-embedding tables, fp32 [table rows, N]): a 128-row tile touches at most 16
-      // distinct table rows.  Staged once per tile with coalesced loads instead of 128 x BN scattered 4-byte L2 reads (the
-      // K=320 QKV projections with a table were 2x slower than the plain ones).  Single buffer: the barrier in front keeps
-      // a fast warp from overwriting slots a slow warp still reads for the previous tile.
-      const float* rbs = nullptr;
-      if (p.rb_stage) {
-        asm volatile("bar.sync 1, 256;" ::: "memory");
-        if (!rb_ahead) rb_fetch(tile);
-#pragma unroll
-        for (int k = 0; k < kRbPf; ++k) {
-          const int i = threadIdx.x + 256 * k;
-          if (i < p.rb_slots * kRbVec) *reinterpret_cast<float4*>(smem_rb + (i / kRbVec) * Cfg::kRbLd + (i % kRbVec) * 4) = rb_pf[k];
-        }
-        if (rb_ahead && tile + (int)gridDim.x < num_tiles) rb_fetch(tile + gridDim.x);
-        const int rit = quad * 32 + lane;
-        const int slot = p.rb_stage == 1 ? (int)(rit / p.rb_div) : (int)(rit % p.rb_mod);
-        rbs = smem_rb + slot * Cfg::kRbLd;
-      }
-      if (p.bias) {
-        const int64_t bc = (int64_t)nt * BN + threadIdx.x;
-        if (threadIdx.x < BN) sb[threadIdx.x] = bc < p.N ? __ldg(p.bias + bc) : 0.f;
-      }
-      if (p.bias || p.rb_stage) asm volatile("bar.sync 1, 256;" ::: "memory");
-      if (tr) p.trace[tcount * 16 + 2] = clock64();
+    wgmma_wait<0>();
+    reg_fence(acc);
+    if (lane == 0) mbar_arrive(&empty_bar[prev_stage]);
+    if (tr) p.trace[tcount * 16 + 1] = clock64();
 
-      // fp32 values of NC (16 or 32) consecutive accumulator columns -> + bias + rowbias, * scale
-      auto finish = [&](float* v, int64_t col0, auto nc_tag) {
-        constexpr int NC = decltype(nc_tag)::value;
-        if (tile_full || col0 + NC <= p.N) {
-          if (p.bias) {
-            const float4* bs = reinterpret_cast<const float4*>(sb + (col0 - (int64_t)nt * BN));
+    // ---- epilogue from registers: row r_h = 16 w + g + 8 h of the warpgroup's 64 rows; columns 8 j + 2 t, +1
+    const int64_t col_base = (int64_t)nt * BN + 2 * t;
 #pragma unroll
-            for (int i = 0; i < NC / 4; ++i) {
-              const float4 bv = bs[i];
-              v[4 * i] += bv.x; v[4 * i + 1] += bv.y; v[4 * i + 2] += bv.z; v[4 * i + 3] += bv.w;
-            }
-          }
-          if (rbs) {
-            const float4* rb = reinterpret_cast<const float4*>(rbs + (col0 - (int64_t)nt * BN));
-#pragma unroll
-            for (int i = 0; i < NC / 4; ++i) {
-              const float4 bv = rb[i];
-              v[4 * i] += bv.x; v[4 * i + 1] += bv.y; v[4 * i + 2] += bv.z; v[4 * i + 3] += bv.w;
-            }
-          } else if (p.rowbias) {
-            const float4* rb = reinterpret_cast<const float4*>(p.rowbias + rbrow * p.rb_ld + col0);
-#pragma unroll
-            for (int i = 0; i < NC / 4; ++i) {
-              const float4 bv = __ldg(rb + i);
-              v[4 * i] += bv.x; v[4 * i + 1] += bv.y; v[4 * i + 2] += bv.z; v[4 * i + 3] += bv.w;
-            }
-          }
-        } else {
-          for (int i = 0; i < NC; ++i) {
-            if (col0 + i < p.N) {
-              if (p.bias) v[i] += __ldg(p.bias + col0 + i);
-              if (p.rowbias) v[i] += __ldg(p.rowbias + rbrow * p.rb_ld + col0 + i);
-            }
-          }
-        }
-        if (p.acc_scale != 1.0f) {
-#pragma unroll
-          for (int i = 0; i < NC; ++i) v[i] *= p.acc_scale;
-        }
+    for (int h = 0; h < 2; ++h) {
+      const int64_t row = (int64_t)mt * kBM + wg * 64 + (warp & 3) * 16 + g + 8 * h;
+      if (row >= p.M) continue;
+      const float* rb = p.rowbias ? p.rowbias + ((row / p.rb_div) % p.rb_mod) * p.rb_ld : nullptr;
+      auto finish = [&](float v, int64_t n) {
+        if (p.bias) v += __ldg(p.bias + n);
+        if (rb) v += __ldg(rb + n);
+        return v * p.acc_scale;
       };
-      using N16 = std::integral_constant<int, 16>;
-      using N32 = std::integral_constant<int, 32>;
-      const int64_t orow = (EPI == kEpiRes && row_ok) ? perm_row(row, p.perm_a, p.perm_b) : row;
-      // NC finished fp32 values of this thread's row -> (+ residuals) -> fp16 -> 256-bit stores (whole 32-byte sectors)
-      auto store = [&](float* v, const uint32_t* r1, const uint32_t* r2, int64_t ocol, auto nc_tag) {
-        constexpr int NC = decltype(nc_tag)::value;
-        if (EPI == kEpiRes && p.R1) {
+      if constexpr (EPI == kEpiGeglu) {
+        // accumulator columns come as (u[32] | g[32]) blocks: n-block j (j % 8 < 4) holds u, n-block j + 4 its gate
+        __half* crow = reinterpret_cast<__half*>(p.C) + row * p.ldc;
 #pragma unroll
-          for (int i = 0; i < NC / 2; ++i) {
-            const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&r1[i]));
-            v[2 * i] += p.r1_scale * f.x; v[2 * i + 1] += p.r1_scale * f.y;
-          }
+        for (int j = 0; j < BN / 8; ++j) {
+          if ((j & 7) >= 4) continue;
+          const int64_t n = col_base + 8 * j;
+          if (n >= p.N) continue;
+          const float u0 = finish(acc[4 * j + 2 * h], n), u1 = finish(acc[4 * j + 2 * h + 1], n + 1);
+          const float g0 = finish(acc[4 * (j + 4) + 2 * h], n + 32), g1 = finish(acc[4 * (j + 4) + 2 * h + 1], n + 33);
+          const int64_t oc = (int64_t)nt * (BN / 2) + (j >> 3) * 32 + 8 * (j & 7) + 2 * t;
+          *reinterpret_cast<uint32_t*>(crow + oc) = pack_f16x2(u0 * gelu_erf(g0), u1 * gelu_erf(g1));
         }
-        if (EPI == kEpiRes && p.R2) {
+      } else if constexpr (EPI == kEpiF32) {
+        float* crow = reinterpret_cast<float*>(p.C) + row * p.ldc;
 #pragma unroll
-          for (int i = 0; i < NC / 2; ++i) {
-            const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&r2[i]));
-            v[2 * i] += f.x; v[2 * i + 1] += f.y;
-          }
-        }
-        uint32_t h[NC / 2];
-#pragma unroll
-        for (int i = 0; i < NC / 2; ++i) h[i] = pack_f16x2(v[2 * i], v[2 * i + 1]);
-        if (p.dbg_nostore && h[0] != 0x12345678u) return;
-        if (Cfg::kOutStage && p.tma_store) {
-          // this row's NC halves into the warp's staging box: 16-byte chunks (ocol % 64) / 8 .. of row `lane`
-          uint8_t* box = smem_out + (warp & 7) * 4096;
-          const int c16 = (int)(ocol & 63) >> 3;      // tiles start on multiples of 64 columns (BN = 128 / 256)
-#pragma unroll
-          for (int i = 0; i < NC / 8; ++i)
-            *reinterpret_cast<uint4*>(box + sw128_offset(lane, c16 + i)) = *reinterpret_cast<const uint4*>(h + 4 * i);
-          return;
-        }
-        __half* o = reinterpret_cast<__half*>(p.C) + orow * p.ldc + ocol;
-        if (tile_full || ocol + NC <= n_out) {
-#pragma unroll
-          for (int i = 0; i < NC / 16; ++i) st_global_256(o + 16 * i, h + 8 * i);
-        } else {
-          for (int i = 0; i < NC; ++i) if (ocol + i < n_out) o[i] = reinterpret_cast<const __half*>(h)[i];
-        }
-      };
-      // residual tiles: 16 columns (one 256-bit load each) per unit
-      auto load_res = [&](uint32_t* r1, uint32_t* r2, int64_t ocol) {
-        if (!tile_full && ocol + 16 > n_out) {   // ragged tail: scalar fill
-          for (int i = 0; i < 16; ++i) {
-            const bool ok = ocol + i < n_out;
-            if (p.R1) reinterpret_cast<__half*>(r1)[i] = ok ? p.R1[row * p.ldr1 + ocol + i] : __float2half(0.f);
-            if (p.R2) reinterpret_cast<__half*>(r2)[i] = ok ? p.R2[orow * p.ldr2 + ocol + i] : __float2half(0.f);
-          }
-          return;
-        }
-        if (p.R1) ld_global_256(p.R1 + row * p.ldr1 + ocol, r1);
-        if (p.R2) ld_global_256(p.R2 + orow * p.ldr2 + ocol, r2);
-      };
-      auto load_one = [&](const __half* src, int64_t ld, int64_t r, uint32_t* dst, int64_t ocol) {   // 16 columns of one residual
-        if (!tile_full && ocol + 16 > n_out) {
-          for (int i = 0; i < 16; ++i) reinterpret_cast<__half*>(dst)[i] = ocol + i < n_out ? src[r * ld + ocol + i] : __float2half(0.f);
-        } else {
-          ld_global_256(src + r * ld + ocol, dst);
-        }
-      };
-
-      if constexpr (EPI == kEpiF32) {
-        // fp32 output (time-embedding table only)
-        constexpr int U = BN / 32;
-        const int u0 = half ? (U + 1) / 2 : 0, u1 = half ? U : (U + 1) / 2;
-        wait_acc();
-#pragma unroll 1
-        for (int ch = u0; ch < u1; ++ch) {
-          uint32_t r[32];
-          tmem_ld32(taddr + ch * 32, r);
-          tmem_wait_ld();
-          const int64_t col0 = (int64_t)nt * BN + ch * 32;
-          if (row_ok && col0 < p.N) {
-            finish(reinterpret_cast<float*>(r), col0, N32{});
-            float* o = reinterpret_cast<float*>(p.C) + row * p.ldc + col0;
-            for (int i = 0; i < 32; ++i) if (col0 + i < p.N) o[i] = __uint_as_float(r[i]);
-          }
+        for (int j = 0; j < BN / 8; ++j) {
+          const int64_t n = col_base + 8 * j;
+          if (n >= p.N) continue;
+          crow[n] = finish(acc[4 * j + 2 * h], n);
+          crow[n + 1] = finish(acc[4 * j + 2 * h + 1], n + 1);
         }
       } else {
-        // Units of accumulator columns, split between the two warps of a quadrant.  Plain: 32 output columns per unit;
-        // residual epilogue: 16 (keeps accumulators + two residual tiles double-buffered inside the register budget);
-        // GEGLU: accumulator columns come as (u[32] | g[32]) blocks and a unit is half a block (16 u + 16 g columns -> 16
-        // outputs).  The TMEM load (and the residual loads) of unit u+1 are issued BEFORE unit u is finished and stored:
-        // with two epilogue warps per sub-partition nothing else hides the TMEM / L2 latency, and the K = 320 GEMMs of
-        // level 0 were bound by exactly this chain.
-        constexpr bool kG = EPI == kEpiGeglu;
-        constexpr bool kR = EPI == kEpiRes;
-        constexpr int W = kR ? 16 : 32;          // accumulator columns per unit (GEGLU: 16 + 16)
-        constexpr int U = BN / W;
-        const int u0 = half ? (U + 1) / 2 : 0, u1 = half ? U : (U + 1) / 2;
-        auto acc_col = [&](int u) -> int64_t {   // first accumulator column of the unit's (first) column group
-          return (int64_t)nt * BN + (kG ? (u >> 1) * 64 + 16 * (u & 1) : u * W);
-        };
-        auto issue = [&](uint32_t* r, uint32_t* r1, uint32_t* r2, int u) {
-          if (kG) {
-            tmem_ld16p(taddr + (u >> 1) * 64 + 16 * (u & 1), r);
-            tmem_ld16p(taddr + (u >> 1) * 64 + 32 + 16 * (u & 1), r + 16);
-          } else if (kR) {
-            tmem_ld16p(taddr + u * 16, r);
-            if (row_ok && (tile_full || acc_col(u) < p.N)) load_res(r1, r2, acc_col(u));
-          } else {
-            tmem_ld32p(taddr + u * 32, r);
-          }
-        };
-        auto process = [&](uint32_t* r, uint32_t* r1, uint32_t* r2, int u) {
-          const int64_t col0 = acc_col(u);
-          if (!row_ok || (!tile_full && col0 >= p.N)) return;
-          float* v = reinterpret_cast<float*>(r);
-          if (kG) {
-            finish(v, col0, N16{});
-            finish(v + 16, col0 + 32, N16{});
+        const int64_t orow = (EPI == kEpiRes) ? perm_row(row, p.perm_a, p.perm_b) : row;
+        __half* crow = reinterpret_cast<__half*>(p.C) + orow * p.ldc;
 #pragma unroll
-            for (int i = 0; i < 16; ++i) v[i] *= gelu_erf(v[16 + i]);
-            store(v, r1, r2, ((int64_t)nt * BN + (u >> 1) * 64) / 2 + 16 * (u & 1), N16{});
-          } else if (kR) {
-            finish(v, col0, N16{});
-            store(v, r1, r2, col0, N16{});
-          } else {
-            finish(v, col0, N32{});
-            store(v, r1, r2, col0, N32{});
-          }
-        };
-        // TMA-store epilogue: a 64-column group of the warp's 32 rows (one 128-byte line per row) is complete after the
-        // unit whose columns end on a multiple of 64; lane 0 then hands the box to the TMA engine and the warp moves on.
-        // Stores leave the SM as whole lines, asynchronously (the direct 256-bit stores -- 32 different lines per
-        // instruction -- cost the K = 320 GEMMs a third of their time, profiles/r01_gemm_epilogue.txt).
-        const bool staged = Cfg::kOutStage && p.tma_store;
-        auto group_done = [&](int u) {
-          if (!staged) return;
-          const int64_t cend = acc_col(u) + W;                       // one past the unit's last accumulator column
-          if ((cend - (int64_t)nt * BN) % 64 != 0) return;
-          const int64_t gcol = cend - 64;
-          fence_proxy_async_smem();
-          __syncwarp();
-          if (lane == 0 && (tile_full || gcol < n_out)) {
-            tma_store_5d(&mapC, smem_out + (warp & 7) * 4096, (int)gcol, (int)row0, 0, 0, 0);
-            tma_store_commit();
-          }
-        };
-        // before the first write of a group: the TMA engine must have finished READING the warp's box (previous group)
-        auto group_begin = [&](int u) {
-          if (!staged || (acc_col(u) - (int64_t)nt * BN) % 64 != 0) return;
-          if (lane == 0) tma_store_wait_read();
-          __syncwarp();
-        };
-        if constexpr (kR) {
-          // Residual epilogue: ALL residual (R2) columns this thread will add are requested before the accumulator wait -- they
-          // do not depend on the MMAs, and with one 256-bit load in flight per 16-column unit the K = 320 / 640 projections
-          // (+ residual) spent their epilogue on a chain of exposed L2 / HBM latencies (one per unit).
-          constexpr int UH = (U + 1) / 2;
-          uint32_t r2all[UH][8];
-          const bool pre = p.R2 != nullptr && row_ok;
-          if (pre) {
-#pragma unroll
-            for (int k = 0; k < UH; ++k) {
-              const int u = u0 + k;
-              if (u < u1 && (tile_full || acc_col(u) < p.N)) load_one(p.R2, p.ldr2, orow, r2all[k], acc_col(u));
-              // (R1 -- unused by the model since the output GEMMs were merged -- stays on the per-unit path below)
+        for (int j = 0; j < BN / 8; ++j) {
+          const int64_t n = col_base + 8 * j;
+          if (n >= p.N) continue;
+          float v0 = finish(acc[4 * j + 2 * h], n), v1 = finish(acc[4 * j + 2 * h + 1], n + 1);
+          if constexpr (EPI == kEpiRes) {
+            if (p.R1) {
+              const float2 f = __half22float2(*reinterpret_cast<const __half2*>(p.R1 + row * p.ldr1 + n));
+              v0 += p.r1_scale * f.x; v1 += p.r1_scale * f.y;
+            }
+            if (p.R2) {
+              const float2 f = __half22float2(*reinterpret_cast<const __half2*>(p.R2 + orow * p.ldr2 + n));
+              v0 += f.x; v1 += f.y;
             }
           }
-          wait_acc();
-          uint32_t ra[16], rb[16];
-          uint32_t r1a[8], r1b[8], r2d[8];
-          auto issue_r = [&](uint32_t* r, uint32_t* r1, int u) {
-            tmem_ld16p(taddr + u * 16, r);
-            if (p.R1 && row_ok && (tile_full || acc_col(u) < p.N)) load_one(p.R1, p.ldr1, row, r1, acc_col(u));
-          };
-          if (u0 < u1) issue_r(ra, r1a, u0);
-#pragma unroll
-          for (int k = 0; k < UH; ++k) {
-            const int u = u0 + k;
-            if (u < u1) {
-              uint32_t* cur = (k & 1) ? rb : ra;
-              uint32_t* nxt = (k & 1) ? ra : rb;
-              uint32_t* cur1 = (k & 1) ? r1b : r1a;
-              uint32_t* nxt1 = (k & 1) ? r1a : r1b;
-              tmem_wait_ld();
-              if (u + 1 < u1) issue_r(nxt, nxt1, u + 1);
-              group_begin(u);
-              process(cur, cur1, pre ? r2all[k] : r2d, u);
-              group_done(u);
-            }
-          }
-        } else {
-          wait_acc();
-          uint32_t ra[32], rb[32];
-          uint32_t r1a[1], r2a[1], r1b[1], r2b[1];
-          if (u0 < u1) issue(ra, r1a, r2a, u0);
-#pragma unroll 1
-          for (int u = u0; u < u1; u += 2) {
-            tmem_wait_ld();
-            if (u + 1 < u1) issue(rb, r1b, r2b, u + 1);
-            group_begin(u);
-            process(ra, r1a, r2a, u);
-            group_done(u);
-            if (u + 1 < u1) {
-              tmem_wait_ld();
-              if (u + 2 < u1) issue(ra, r1a, r2a, u + 2);
-              group_begin(u + 1);
-              process(rb, r1b, r2b, u + 1);
-              group_done(u + 1);
-            }
-          }
+          *reinterpret_cast<uint32_t*>(crow + n) = pack_f16x2(v0, v1);
         }
       }
-      if (tr) p.trace[tcount * 16 + 3] = clock64();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tempty_bar[acc]);
-      if (++acc == 2) { acc = 0; acc_phase ^= 1; }
     }
+    if (tr) p.trace[tcount * 16 + 2] = clock64();
   }
-  if (Cfg::kOutStage && p.tma_store && warp < 8 && lane == 0) tma_store_wait_all();
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 9) tmem_dealloc<Cfg::kTmemCols>(tmem_base);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -597,8 +294,7 @@ __global__ void gemm_simt_kernel(const GemmDev p, const __half* __restrict__ A, 
 }
 
 template <int BN, int EPI>
-static int launch_tc_epi(const GemmDev& dev, const CUtensorMap* mapA, const CUtensorMap* mapB, const CUtensorMap* mapC,
-                         cudaStream_t st) {
+static int launch_tc_epi(const GemmDev& dev, const CUtensorMap* mapA, const CUtensorMap* mapB, cudaStream_t st) {
   using Cfg = GemmCfg<BN>;
   static bool attr_set = false;
   if (!attr_set) {
@@ -607,27 +303,24 @@ static int launch_tc_epi(const GemmDev& dev, const CUtensorMap* mapA, const CUte
   }
   const int tiles = dev.tiles_m * dev.tiles_n;
   const int grid = tiles < sm_count() ? tiles : sm_count();
-  GemmDev d2 = dev;
-  d2.stages = dev.tma_store ? Cfg::kStagesStaged : Cfg::kMaxStages;
-  gemm_tc_kernel<BN, EPI><<<grid, 320, Cfg::smem_bytes(dev.tma_store != 0), st>>>(d2, *mapA, *mapB, *mapC);
+  gemm_tc_kernel<BN, EPI><<<grid, kGemmThreads, Cfg::kSmemBytes, st>>>(dev, *mapA, *mapB);
   A3D_LAUNCH_CHECK();
   return A3D_OK;
 }
 
 template <int BN>
-static int launch_tc(const GemmDev& dev, const CUtensorMap* mapA, const CUtensorMap* mapB, const CUtensorMap* mapC,
-                     cudaStream_t st) {
-  if (dev.out_f32) return launch_tc_epi<BN, kEpiF32>(dev, mapA, mapB, mapC, st);
-  if (dev.geglu) return launch_tc_epi<BN, kEpiGeglu>(dev, mapA, mapB, mapC, st);
-  if (dev.R1 || dev.R2 || dev.perm_a) return launch_tc_epi<BN, kEpiRes>(dev, mapA, mapB, mapC, st);
-  return launch_tc_epi<BN, kEpiPlain>(dev, mapA, mapB, mapC, st);
+static int launch_tc(const GemmDev& dev, const CUtensorMap* mapA, const CUtensorMap* mapB, cudaStream_t st) {
+  if (dev.out_f32) return launch_tc_epi<BN, kEpiF32>(dev, mapA, mapB, st);
+  if (dev.geglu) return launch_tc_epi<BN, kEpiGeglu>(dev, mapA, mapB, st);
+  if (dev.R1 || dev.R2 || dev.perm_a) return launch_tc_epi<BN, kEpiRes>(dev, mapA, mapB, st);
+  return launch_tc_epi<BN, kEpiPlain>(dev, mapA, mapB, st);
 }
 
 static long long* g_gemm_trace = nullptr;
 
 }  // namespace a3d
 
-// debug hook (not part of the product path): per-tile clock64 timestamps of CTA 0 of the following tcgen05 GEMM launches
+// debug hook (not part of the product path): per-tile clock64 timestamps of CTA 0 of the following tensor-core GEMM launches
 extern "C" int a3d_debug_set_gemm_trace(void* device_buffer_1024_int64) {
   a3d::g_gemm_trace = reinterpret_cast<long long*>(device_buffer_1024_int64);
   return A3D_OK;
@@ -651,11 +344,6 @@ extern "C" int a3d_gemm(const a3d_gemm_args* a, void* stream) {
   d.C = a->C; d.ldc = a->ldc; d.geglu = a->geglu; d.out_f32 = a->out_f32;
   d.perm_a = a->perm_a; d.perm_b = a->perm_b;
   d.trace = g_gemm_trace;
-  {
-    static int nostore = -1;
-    if (nostore < 0) { const char* e = getenv("A3D_GEMM_NOSTORE"); nostore = e ? atoi(e) : 0; }
-    d.dbg_nostore = nostore;
-  }
   if (a->geglu && (a->out_f32 || a->R1 || a->R2 || a->perm_a || (a->N % 128)))
     return fail(A3D_EINVAL, "a3d_gemm: GEGLU epilogue takes bias / row-bias only, fp16 output, N %% 128 == 0");
   if (a->out_f32 && (a->R1 || a->R2 || a->perm_a))
@@ -700,7 +388,7 @@ extern "C" int a3d_gemm(const a3d_gemm_args* a, void* stream) {
   int impl = a->impl;
   if (impl == A3D_GEMM_AUTO) impl = tc_ok ? A3D_GEMM_TCGEN05 : A3D_GEMM_SIMT;
   if (impl == A3D_GEMM_TCGEN05 && !tc_ok)
-    return fail(A3D_EINVAL, "a3d_gemm: shape/alignment not supported by the tcgen05 path (M=%lld N=%lld K=%lld)",
+    return fail(A3D_EINVAL, "a3d_gemm: shape/alignment not supported by the tensor-core path (M=%lld N=%lld K=%lld)",
                 (long long)a->M, (long long)a->N, (long long)a->K);
 
   if (impl == A3D_GEMM_SIMT) {
@@ -735,13 +423,6 @@ extern "C" int a3d_gemm(const a3d_gemm_args* a, void* stream) {
   d.tiles_n = (int)((a->N + BN - 1) / BN);
   d.cpb = a->a_mode == A3D_A_CONV3 ? cv.c / kBK : 0;
   d.tpi = tpi; d.boh = boh; d.bimg = bimg; d.tpr = tpr; d.conv_pad = cv.pad;
-  d.rb_stage = 0; d.rb_slots = 0;
-  if (a->rowbias && (a->N % 4 == 0) && (a->rb_ld % 4 == 0) && ((reinterpret_cast<uintptr_t>(a->rowbias) & 15) == 0)) {
-    if (d.rb_div % kBM == 0) { d.rb_stage = 1; d.rb_slots = 1; }                                  // one table row per tile
-    else if (d.rb_div >= 8 && kBM % d.rb_div == 0) { d.rb_stage = 1; d.rb_slots = (int)(kBM / d.rb_div); }
-    else if (d.rb_div == 1 && d.rb_mod <= 16 && kBM % d.rb_mod == 0) { d.rb_stage = 2; d.rb_slots = (int)d.rb_mod; }
-  }
-
   const CUtensorMap *mapA = nullptr, *mapB = nullptr;
   {
     MapKey kb;
@@ -766,26 +447,9 @@ extern "C" int a3d_gemm(const a3d_gemm_args* a, void* stream) {
     ka.estr[1] = cv.s; ka.estr[2] = cv.s;
     if (int r = get_tensor_map(ka, &mapA)) return r;
   }
-  // output through shared memory + TMA bulk stores where the epilogue allows it (plain / residual, no row permutation)
-  const CUtensorMap* mapC = mapA;
-  d.tma_store = 0;
-  {
-    static int want = -1;
-    if (want < 0) { const char* e = getenv("A3D_GEMM_TMA_STORE"); want = e ? atoi(e) : 1; }
-    // short-K GEMMs are bound by their output stores; the long-K ones (convolutions) keep the deeper operand ring instead
-    if (want && BN != 160 && a->K <= 1280 && !a->geglu && !a->out_f32 && !a->perm_a && (a->ldc % 8 == 0) &&
-        ((reinterpret_cast<uintptr_t>(a->C) & 15) == 0) && (a->N % 8 == 0)) {
-      const uint64_t dims[5] = {(uint64_t)a->N, (uint64_t)a->M, 1, 1, 1};
-      const uint64_t str[4] = {(uint64_t)a->ldc, (uint64_t)a->ldc * a->M, (uint64_t)a->ldc * a->M, (uint64_t)a->ldc * a->M};
-      const uint32_t box[5] = {64, 32, 1, 1, 1};
-      MapKey kc = make_key(a->C, dims, str, box);
-      if (int r = get_tensor_map(kc, &mapC)) return r;
-      d.tma_store = 1;
-    }
-  }
   switch (BN) {
-    case 256: return launch_tc<256>(d, mapA, mapB, mapC, st);
-    case 160: return launch_tc<160>(d, mapA, mapB, mapC, st);
-    default: return launch_tc<128>(d, mapA, mapB, mapC, st);
+    case 256: return launch_tc<256>(d, mapA, mapB, st);
+    case 160: return launch_tc<160>(d, mapA, mapB, st);
+    default: return launch_tc<128>(d, mapA, mapB, st);
   }
 }

@@ -510,7 +510,7 @@ __global__ void temporal_attn_kernel(const __half* __restrict__ qkv, __half* __r
 }
 
 // F == 16 (the shipped motion modules): one block per pixel, one warp per head, the whole 16 x 16 attention of a head as
-// mma.sync.m16n8k16 tiles (a 16-frame problem is far below a tcgen05 tile; the legacy warp-level MMA is the right size).
+// mma.sync.m16n8k16 tiles (a 16-frame problem is far below a 64-row wgmma tile; the warp-level MMA is the right size).
 // The pixel's [16 frames, 3C] slab is staged in shared memory with coalesced 16-byte loads (rows padded by 16 B so the
 // fragment loads of the 8 row groups hit different banks); S and P never leave registers (the accumulator fragment of QK^T
 // is exactly the A fragment of P V); the normalised O goes back over the head's dead Q slice and leaves with coalesced
@@ -807,7 +807,8 @@ static void gn_geometry(int C, int64_t samples, int64_t rows_per_sample, int* ro
   *rows_par = rp;
   *threads = ((rp * vpr + 31) / 32) * 32;   // <= 256 (C / 8 <= 160 for the UNet's widths) or one row per block
   int cr = 128;
-  while (cr > 4 * rp && ((rows_per_sample + cr - 1) / cr) * samples < 592) cr /= 2;
+  const int64_t fill = 4 * (int64_t)sm_count();   // blocks for about four waves per SM
+  while (cr > 4 * rp && ((rows_per_sample + cr - 1) / cr) * samples < fill) cr /= 2;
   *chunk_rows = cr;
   *chunks = (int)((rows_per_sample + cr - 1) / cr);
 }

@@ -8,7 +8,7 @@
 
 Hot path = `compute_mvdream_recon_loss` (391-513): noise frames 1.., ONE classifier-free-guided UNet evaluation with no
 grad (422-459; (cond, uncond) order, `text + s*(text - uncond)`), x0 through the DDIM scheduler (466), std-rescale
-(468-487), x0-reconstruction MSE (497-501).  The UNet evaluation runs on the sm_100a engine (`MVUNetMotionModel`); the
+(468-487), x0-reconstruction MSE (497-501).  The UNet evaluation runs on the sm_90a engine (`MVUNetMotionModel`); the
 remaining arithmetic is a handful of elementwise/reduction ops on [B*Nv*F, 4, 32, 32] latents that must stay on the
 autograd tape (the loss's gradient flows to `latents` and from there through the VAE encoder to the rasterizer), so they
 are torch ops.

@@ -44,7 +44,7 @@ class Node(nn.Module):
         return self.weight.shape[1]
 
     def forward(self, *a, **k):
-        raise RuntimeError("animate3d_b200 modules hold parameters for the sm_100a engine; they are not executed one by one "
+        raise RuntimeError("animate3d_b200 modules hold parameters for the sm_90a engine; they are not executed one by one "
                            "-- call MVUNetMotionModel.forward")
 
 
@@ -173,7 +173,7 @@ class AttentionNode(Node):
         kind = type(processor).__name__
         if kind != cur.kind:
             raise ValueError(f"this attention slot runs {cur.kind} in the released model (inference.py:107-174); got {kind}. "
-                             "The B200 engine implements the released wiring only.")
+                             "The H100 engine implements the released wiring only.")
         want = cur.signature()
         got = _foreign_signature(processor)
         if got != want:

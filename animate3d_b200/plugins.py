@@ -1,4 +1,4 @@
-"""Import this module from a threestudio application to register the B200 replacements of the reference's plugins
+"""Import this module from a threestudio application to register the H100 replacements of the reference's plugins
 (the reference registers them by importing every directory under `custom/`, launch.py:70-102):
 
     import animate3d_b200.plugins            # -> threestudio.find("animatemv-diffusion-guidance"), ...

@@ -2,7 +2,7 @@
 
     processor(attn, hidden_states, encoder_hidden_states=None, attention_mask=None, temb=None) -> Tensor
 
-(animatediff/models/attention_processor.py:39-48, 169-178, 325-334, 541-550) on the sm_100a kernels of liba3d.so: one fused
+(animatediff/models/attention_processor.py:39-48, 169-178, 325-334, 541-550) on the sm_90a kernels of liba3d.so: one fused
 projection GEMM, the strided-view attention kernel (the "(b n f) l c -> (b f) (n l) c" regroupings are TMA strides, never copies),
 one merged output GEMM.  `MVUNetMotionModel.forward` fuses the same arithmetic into the whole-network schedule; this module is the
 boundary for code that drives a single `Attention` layer with one of the processors -- e.g. a diffusers `Attention.forward`, or
@@ -194,7 +194,7 @@ _DISPATCH = {"MVDreamI2VXFormersAttnProcessor": _mv_i2v, "IPAdapterXFormersAttnP
 def run(proc, attn, hidden_states, encoder_hidden_states=None, attention_mask=None, temb=None, **kwargs):
     L.load()
     if not hidden_states.is_cuda:
-        raise L.A3DError("the attention processors run on an sm_100a device only; there is no CPU path")
+        raise L.A3DError("the attention processors run on an sm_90a device only; there is no CPU path")
     _check_common(attn, attention_mask)
     if hidden_states.ndim != 3:
         raise NotImplementedError("4-D (b, c, h, w) inputs never reach these processors in the reference (Transformer2DModel "

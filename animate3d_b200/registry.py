@@ -6,7 +6,7 @@ The reference's guidance / renderer / geometry are threestudio extensions: class
 `BaseObject.__init__(cfg) -> parse_structured(Config, cfg) -> configure(...)` (threestudio/utils/base.py:77-86).
 
 When `threestudio` is importable this module re-exports ITS `register` / `find` / `BaseObject`, so importing
-`animate3d_b200.plugins` makes the B200 classes discoverable exactly like the reference's `custom/` directory
+`animate3d_b200.plugins` makes the H100 classes discoverable exactly like the reference's `custom/` directory
 (launch.py:70-102).  When it is not (this container, the GPU box), a local registry with the same semantics keeps the
 classes constructible and testable; nothing else in the package depends on which of the two is active."""
 from __future__ import annotations

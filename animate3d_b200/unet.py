@@ -1,5 +1,5 @@
 """Host-side mirror of the reference's `MVUNetMotionModel` (animatediff/models/unet_motion_mv_model.py:55-867) whose forward
-runs entirely on the sm_100a kernels of liba3d.so.
+runs entirely on the sm_90a kernels of liba3d.so.
 
 Same constructor geometry, same state-dict keys (incl. the processors' `<attn>.processor.*` parameters installed by
 inference.py:107-174), same `forward(sample, timestep, encoder_hidden_states, ..., camera, num_views, i2v_cond_time_zero)`
@@ -9,7 +9,7 @@ signature and `UNet3DConditionOutput(sample=...)` result.  What differs is every
     fold into conv_in / conv_out, and every "(b n f) l c -> (b f) (n l) c" / "(b l) f c -> (b f) l c" regroup and the
     frame-0 K/V broadcast of the processors (attention_processor.py:340, 389-397, 557, 669) become strides of a rank-5 TMA
     view read in place by the attention kernel -- nothing is ever rearranged or cloned
-  * every Linear/Conv is one tcgen05 GEMM (implicit im2col for 3x3) with bias / time-embedding / residual / GEGLU /
+  * every Linear/Conv is one wgmma GEMM (implicit im2col for 3x3) with bias / time-embedding / residual / GEGLU /
     alpha-blend / row-permute fused into its epilogue; q,k,v(,q_i2v) projections are one GEMM per attention
   * positional encodings are folded into the projections: (x + pe) W = x W + (pe W), the second term is a per-position
     row-bias table computed once at load
@@ -131,8 +131,7 @@ class MVUNetMotionModel(torch.nn.Module):
         self._graphs: Dict[tuple, torch.cuda.CUDAGraph] = {}
         self._static: Dict[tuple, dict] = {}
         # View-sharded forwards run eagerly: capturing the asynchronous NCCL all-gathers of torch 2.11 / NCCL 2.28 in a CUDA graph
-        # deadlocks on this stack (measured on 2 x B200: profiles/r02_multi_gpu_2.log); the kernels between two gathers are long
-        # enough for the launch stream to stay ahead.
+        # deadlocks on this stack; the kernels between two gathers are long enough for the launch stream to stay ahead.
         self.use_cuda_graph = view_group is None
         self.gemm_impl = L.IMPL_AUTO
         self.attn_impl = L.IMPL_AUTO
@@ -163,7 +162,7 @@ class MVUNetMotionModel(torch.nn.Module):
                 device = a.device
         if device is not None and torch.device(device) != self._device:
             if torch.device(device).type != "cuda":
-                raise RuntimeError("MVUNetMotionModel runs on an sm_100a device only; there is no CPU path")
+                raise RuntimeError("MVUNetMotionModel runs on an sm_90a device only; there is no CPU path")
             super().to(device)
             self._device = torch.device(device)
             self._prepared = False

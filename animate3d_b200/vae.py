@@ -1,11 +1,11 @@
-"""SD-1.5 `AutoencoderKL` on the sm_100a engine (SURVEY 8f-1): the module that sits immediately either side of the UNet.
+"""SD-1.5 `AutoencoderKL` on the sm_90a engine (SURVEY 8f-1): the module that sits immediately either side of the UNet.
 
   * `encode(x).latent_dist.sample()` -- with INPUT GRADIENT: in the 4D-SDS step the encoder runs on the 64 rendered 256^2 views
     and is the only autograd path from `loss_sds` back to the rasterizer (animatemv_guidance.py:365-373, 533-542; the VAE
     parameters are frozen, 301-302, so only d/d input is needed: ~17 TFLOP forward + ~17 TFLOP dgrad per step)
   * `decode(z).sample` -- forward only (pipeline.py:554-567 `decode_latents`, guidance_eval)
 
-Same layout and kernels as the UNet: activations NHWC fp16, every 3x3 convolution is the implicit-GEMM tcgen05 kernel
+Same layout and kernels as the UNet: activations NHWC fp16, every 3x3 convolution is the implicit-GEMM wgmma kernel
 (`a3d_gemm`, A3D_A_CONV3) -- the input gradient of a convolution is the same kernel with the flipped / transposed weights (the
 stride-2 downsampler's through a zero-inserted copy of the output gradient) --, GroupNorm(+SiLU) forward / backward are
 `a3d_group_norm` / `a3d_group_norm_backward`, the 3- / 4- / 8-channel edge convolutions are `a3d_conv_in` / `a3d_conv_out`.

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py -- MV-VDM denoise-steps/s at 4 views x 16 frames x 256^2 (BASELINE.json metric) on N B200s of one node.
+"""bench.py -- MV-VDM denoise-steps/s at 4 views x 16 frames x 256^2 (BASELINE.json metric) on N H100s of one node.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl native|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl native|reference] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 A "step" = one denoise step of the reference sampler (animatediff/pipelines/pipeline.py:1006-1031): classifier-free-guided
@@ -13,7 +13,7 @@ N > 1: every rank denoises its own prompt (the (prompt x view-group) batch is pa
 JSON line keys beyond the base contract:
   roofline     the fused cross-view attention kernel at level 0 (L = 4 views * 32*32 = 4096 tokens, head_dim 40, 8 heads,
                2*16 (CFG x frame) batches) timed alone with CUDA events; achieved = 4*L^2*C*batches FLOP / duration against
-               the measured bf16 tensor peak of MEASURED_PEAKS.json
+               the fp16 tensor peak (MEASURED_PEAKS.json when present, else the H100 SXM data sheet's dense figure)
   cpu_baseline the oracle port (oracle/unet_oracle.py) on the host cores for a bounded sample, extrapolated by FLOPs
   e2e          the same step through pipeline.denoise_step_host with pinned HOST buffers (H2D of the step inputs + D2H of
                the updated latents inside the timed region)
@@ -28,6 +28,8 @@ JSON line keys beyond the base contract:
   view_sharded (N > 1) ONE prompt spread over the N ranks -- CFG branches over 2 ranks and / or the 4 views over 4 ranks with
                the cross-view K|V all-gather over NCCL -- as a strong-scaling number next to the weak-scaling `value`, with the
                exposed communication time (same forward with the collectives skipped)
+--dump-outputs DIR (native) writes the latents the last timed step returned as DIR/latents.npy (float32); the inputs are seeded,
+so two builds run with the same arguments can be compared output for output.
 --impl reference times the oracle port (the reference's diffusers CPU path is not installable here: SURVEY section 8c) on a
 BOUNDED sample per step (one forward of 4 views x 1 frame: the real L = 4096 cross-view attention shape); `ms_per_step` is the
 measured time of that sample, `value` the steps/s extrapolated by FLOPs -- flagged `extrapolated` / `same_config: false`.
@@ -59,8 +61,9 @@ def peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
-        return d.get("bf16_tflops", 1590.0), d.get("hbm_gbs", 6650.0), "measured (MEASURED_PEAKS.json, burst)"
-    return 1590.0, 6650.0, "fallback (B200_PROFILING.md)"
+        return d.get("bf16_tflops", 989.0), d.get("hbm_gbs", 3350.0), "measured (MEASURED_PEAKS.json, burst)"
+    # NVIDIA H100 SXM data sheet: 989 TFLOP/s dense fp16 / bf16, 3.35 TB/s HBM3 (a 700 W card; a lower power limit lowers both)
+    return 989.0, 3350.0, "H100 SXM data sheet (not measured)"
 
 
 class ClockSampler:
@@ -181,22 +184,24 @@ def run_reference(args, rank, world):
         "dtype": "f32", "data": "synthetic", "extrapolated": True, "same_config": False,
         "config": {"workload": "MV-VDM CFG denoise step, 1 prompt x 2 CFG x 4 views x 16 frames x 32x32x4 latents",
                    "sample": sample_desc, "sample_tflop": fl / 1e12, "step_tflop": sf / 1e12, "extrapolation_factor": factor,
-                   "full_step_evidence": "profiles/r02_cpu_oracle_full_forward.txt (one full 4-view x 16-frame branch forward timed on "
-                                         "the GPU box inside tests/test_unet_gpu.py)",
                    "note": "reference's diffusers CPU path is not installable here; oracle port (oracle/unet_oracle.py) timed"},
         "cpu_baseline": {"value": val, "unit": UNIT, "cores": cores, "kind": "port", "sample": sample_desc},
         "e2e": {"value": val, "unit": UNIT, "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0},
         "gpu_launches": 0}))
 
 
+def sm_count():
+    import torch
+    return torch.cuda.get_device_properties(torch.cuda.current_device()).multi_processor_count
+
+
 def mufu_note(att_flops, att_ms, clocks):
-    """The pipe that bounds this kernel at head_dim 40 (DESIGN.md section 6): one ex2 per score, MUFU.EX2 = 8 cycles per warp
-    instruction per SM sub-partition.  The fp16 pack (F2FP, 4 cycles) runs beside it, not on it: 2 MUFU + 1 F2FP measure 16.0
-    cycles, not 20 (profiles/r02_pipes_ubench.txt; round 1 had assumed a shared pipe and a 25 % higher floor)."""
+    """Lower bound of this kernel at head_dim 40 from its exponentials: one ex2 per score on the MUFU pipe, which retires 16
+    results per clock per SM (one warp instruction every 8 cycles per SM sub-partition)."""
     try:
         scores = att_flops / (4.0 * 40.0)                       # 4 * d FLOP per (query, key) pair
-        cycles = (scores / 32.0 * 8.0) / (148 * 4)
-        mhz = float(clocks.get("sm_mhz") or 1965.0)
+        cycles = (scores / 32.0 * 8.0) / (sm_count() * 4)
+        mhz = float(clocks.get("sm_mhz") or 1980.0)
         floor_ms = cycles / (mhz * 1e3)
         return {"floor_ms": floor_ms, "frac_of_floor": floor_ms / att_ms, "sm_mhz_used": mhz}
     except Exception as e:                                      # never let a diagnostic field break the bench line
@@ -344,7 +349,7 @@ def splat_bench(torch, rank, world, peak_hbm, sm_mhz, iters=5):
     b_bin = pairs * 12.0 + passes * 2 * 12.0 * pairs
     t_bin = (st["scan_duplicate"] + st["radix_sort"] + st["ranges"]) * 1e-3
     evals = float(pairs) * 256.0                                   # pixel-gaussian evaluations (upper bound: early exit at T < 1e-4)
-    mufu_evals_s = 148 * 16 * sm_mhz * 1e6                          # one ex2 per evaluation, 16 per clock per SM
+    mufu_evals_s = sm_count() * 16 * sm_mhz * 1e6                   # one ex2 per evaluation, 16 per clock per SM
     out = {"config": {"gaussians": P, "cameras": ncam_total, "cameras_per_rank": ncam, "H": H, "W": W,
                       "scene": "SURVEY 8(d) config 3 (seeded synthetic), k-planes + 3 MLPs deformation per timestamp",
                       "parallelism": "single GPU" if world == 1 else f"cameras r::{world}, 1 flat all-reduce of the deformation-field gradients"},
@@ -505,6 +510,14 @@ def view_sharded_bench(torch, args, rank, world, local_rank, base_model, timeste
             "cuda_graph": bool(model._graphs), "finite": finite}
 
 
+def dump_outputs(directory, arrays):
+    """Save each tensor as directory/<name>.npy in float32."""
+    import numpy as np
+    os.makedirs(directory, exist_ok=True)
+    for name, t in arrays.items():
+        np.save(os.path.join(directory, f"{name}.npy"), t.detach().float().cpu().numpy())
+
+
 def run_native(args, rank, world, local_rank):
     import torch
     import torch.distributed as dist
@@ -556,6 +569,8 @@ def run_native(args, rank, world, local_rank):
     torch.cuda.synchronize()
     ms = e0.elapsed_time(e1)
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, {"latents": lat})
     if world > 1:
         t = torch.tensor([ms], device=dev)
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
@@ -605,10 +620,6 @@ def run_native(args, rank, world, local_rank):
     sf = step_flops()
     att_ms, att_flops = time_attention_l0(torch)
     att_tf = att_flops / (att_ms * 1e-3) / 1e12
-    traffic = None
-    tp = os.path.join(ROOT, "profiles", "roofline_traffic.json")
-    if os.path.exists(tp):
-        traffic = json.load(open(tp)).get("attn_l0_dram_bytes_per_launch")     # ncu dram__bytes_read+write per launch (r01 capture)
     gemm_rf = gemm_rooflines(torch, peak_tf, peak_hbm)
     sds = None
     if world == 1:
@@ -632,17 +643,14 @@ def run_native(args, rank, world, local_rank):
                                "(BASELINE configs[1]); random-init SD1.5+motion-module weights (1.53 B params)",
                    "parallelism": f"prompt-sharded dp{world}, no data-path collective",
                    "step_tflop": sf / 1e12, "achieved_tflops_per_gpu": sf / 1e12 / (ms_step * 1e-3),
-                   "l2": "working set (3.1 GB fp16 weights + activations) >> 126 MB L2; no flush needed",
+                   "l2": "working set (3.1 GB fp16 weights + activations) >> 50 MB L2; no flush needed",
                    "cuda_graph": bool(model.use_cuda_graph)},
         "roofline": {"bound": "tensor", "kernel": "a3d_attention head_dim 40 (fused cross-view attention, L=4096, 32 batches x 8 heads)",
-                     "achieved": att_tf, "peak": peak_tf, "unit": "TFLOP/s", "frac": att_tf / peak_tf, "traffic": traffic,
-                     "traffic_source": "ncu --set full dram__bytes_read+write of this kernel, round-2 capture (profiles/roofline_traffic.json, "
-                                       "profiles/r02_ncu_attn5.txt); algorithmic bytes 386 MB",
+                     "achieved": att_tf, "peak": peak_tf, "unit": "TFLOP/s", "frac": att_tf / peak_tf,
                      "ms_per_launch": att_ms, "flop_per_launch": att_flops, "peak_source": peak_src,
                      "mufu": mufu_note(att_flops, att_ms, clocks),
-                     "note": "0.6x of the tensor peak is not reachable at head_dim 40: every score needs one exponential; the XU "
-                             "pipe (MUFU.EX2, 8 cycles / warp instruction / sub-partition) floors the kernel at `mufu.floor_ms` "
-                             "(tensor-only bound would be 0.31 ms); logits here are randn, the in-step kernel time agrees within 2 %"},
+                     "note": "at head_dim 40 every score needs one exponential: the MUFU pipe floors the kernel at `mufu.floor_ms`, "
+                             "well above the tensor-only bound; logits here are randn"},
         "roofline_gemm": gemm_rf,
         "splat": splat,
         "sds_step": sds,
@@ -693,6 +701,8 @@ def main():
     ap.add_argument("--steps", type=int, default=10)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="native", choices=["native", "reference"])
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step computed as DIR/<name>.npy (native only)")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -703,6 +713,8 @@ def main():
         cmd = [sys.executable, "-m", "torch.distributed.run", "--nnodes=1", f"--nproc-per-node={args.gpus}", "--master-addr",
                "127.0.0.1", "--master-port", port, os.path.abspath(__file__), "--gpus", str(args.gpus), "--steps", str(args.steps),
                "--warmup", str(args.warmup), "--impl", args.impl]
+        if args.dump_outputs:
+            cmd += ["--dump-outputs", args.dump_outputs]
         sys.exit(subprocess.call(cmd))
     if args.impl == "reference":
         run_reference(args, rank, world)

@@ -1,4 +1,4 @@
-/* animate3d_b200 -- C ABI of the B200-native hot path (liba3d.so).
+/* animate3d_b200 -- C ABI of the H100-native (sm_90a) hot path (liba3d.so).
  *
  * Plain pointers and sizes only; every pointer is a DEVICE pointer unless its name ends in _host.  All entry points
  * enqueue work on `stream` (a cudaStream_t passed as void*) and return 0 on success or a negative A3D_E* code; the
@@ -30,15 +30,15 @@ extern "C" {
 #define A3D_OK 0
 #define A3D_EINVAL (-1)   /* bad argument / unsupported shape */
 #define A3D_ECUDA (-2)    /* CUDA runtime or driver error     */
-#define A3D_ENOTSUP (-3)  /* device is not sm_100             */
+#define A3D_ENOTSUP (-3)  /* device is not sm_90              */
 
 const char* a3d_last_error(void);
 int a3d_version(void);
-/* 0 when the current device is sm_100 and the driver entry points needed for TMA are available. */
+/* 0 when the current device is sm_90 and the driver entry points needed for TMA are available. */
 int a3d_init(void);
 
 /* ---------------------------------------------------------------- GEMM / implicit-GEMM convolution ----------- */
-/* C[M,N] = epilogue( A[M,K] * B[N,K]^T ), fp16 operands, fp32 accumulation in tensor memory (tcgen05).
+/* C[M,N] = epilogue( A[M,K] * B[N,K]^T ), fp16 operands, fp32 accumulation on the tensor cores (wgmma).
  * A operand modes: A3D_A_PLAIN  row-major [M, lda]
  *                  A3D_A_CONV3  NHWC image [n_img, H, W, C] gathered as a 3x3 (pad 1, stride 1|2) im2col, K = 9*C,
  *                               k index = (ky*3+kx)*C + c ; M = n_img*OH*OW
@@ -49,6 +49,7 @@ int a3d_init(void);
  * Row permutation (perm_a, perm_b > 0): om = (m / (a*b))*(a*b) + (m % b)*a + (m / b) % a   ("(x a b) -> (x b a)").
  */
 enum { A3D_A_PLAIN = 0, A3D_A_CONV3 = 1 };
+/* A3D_GEMM_TCGEN05 selects the tensor-core (wgmma) kernels; the name is kept for ABI compatibility. */
 enum { A3D_GEMM_AUTO = 0, A3D_GEMM_TCGEN05 = 1, A3D_GEMM_SIMT = 2 };
 
 typedef struct a3d_gemm_args {
@@ -80,7 +81,7 @@ typedef struct a3d_gemm_args {
  * 425-441, 600-655, 686-717), with their bias, residual, positional-table and layout epilogues fused. */
 int a3d_gemm(const a3d_gemm_args* args, void* stream);
 
-/* ---------------------------------------------------------------- fused attention (tcgen05) ------------------ */
+/* ---------------------------------------------------------------- fused attention (wgmma) -------------------- */
 /* O = softmax(scale * Q K^T) V per (batch, head); Q/K/V are read in place from projection outputs through rank-5
  * strided views so that the reference's "(b n f) l c -> (b f) (n l) c" regroupings never materialise.
  * A view addresses element (col, i1, i2, i3, i4) at base + col + i1*s1 + i2*s2 + i3*s3 + i4*s4 (element strides).
@@ -273,22 +274,16 @@ int a3d_knn_graph(const float* points, int n, int K, int32_t* nbr, float* dist2,
 int a3d_arap(const float* nodes, int Nt, int Nv, const int32_t* nbr, int K, const float* weight, const int32_t* sample, int Ns,
              float* err, float* grad, void* stream);
 
-/* debug hook: a device uint64 counter the tcgen05 attention kernels bump once per (warp, key step) that takes the
-   lazy-rescale branch of the single-pass softmax (NULL = off; tests use it to prove adversarial inputs reach that branch).
-   The buffer must hold 8 + 4*32*8 + 32 uint64: words 8.. receive a clock64 timeline of four softmax warps of CTA (0,0,0) of the
-   head-dim-40 kernel (tools/attn_timeline.py) */
+/* debug hook: a device uint64 counter the tensor-core attention kernel bumps once per (warp, key step) that takes the
+   lazy-rescale branch of the single-pass softmax (NULL = off; tests use it to prove adversarial inputs reach that branch). */
 int a3d_debug_set_attn_trace(void* device_counter_u64);
-/* tuning hook of the head-dim-40 attention kernel (default 15 = all on): bit 0 one-step-ahead non-blocking barrier tests, bit 1
-   probabilities through tensor memory (TS-mode P V), bit 2 one 128-query tile per CTA with two CTAs per SM, bit 3 (TS) no explicit
-   "P buffer consumed" wait (implied by the arrival of the step's scores: tcgen05 operations retire in issue order) */
-int a3d_debug_set_attn_poly(int flags);
 /* measurement hooks of the rasterizer (bench.py's splat roofline): with timing enabled every forward / backward records CUDA
    events at its stage boundaries; a3d_debug_raster_stage_ms returns the milliseconds of the last forward's stages
    [0] preprocess [1] scan + counts + duplicate [2] radix sort [3] tile ranges [4] render and the last backward's [5] render
    backward [6] preprocess backward ([7] unused) */
 int a3d_debug_raster_timing(int enable);
 int a3d_debug_raster_stage_ms(float* out_host8);
-/* same for the tcgen05 GEMM: per-tile timestamps of CTA 0 (epilogue warp 0 and the MMA-issuing thread) */
+/* same for the tensor-core GEMM: per-tile clock64 timestamps of CTA 0 (thread 0: tile start, main loop done, epilogue done) */
 int a3d_debug_set_gemm_trace(void* device_buffer_1024_int64);
 
 #ifdef __cplusplus

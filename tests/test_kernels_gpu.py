@@ -1,4 +1,4 @@
-"""Per-kernel parity on a real B200: every CUDA kernel behind the C ABI vs a plain fp32 torch restatement of the same op
+"""Per-kernel parity on a real H100: every CUDA kernel behind the C ABI vs a plain fp32 torch restatement of the same op
 on the same seeded fp16 inputs.  Tolerances: outputs are fp16 with fp32 accumulation -> rtol 1e-2 (north_star's budget)
 on top of an absolute term scaled to the output magnitude."""
 import math
@@ -87,8 +87,6 @@ def gemm_ref(A, B, flags, bias, rowbias, rb_div, rb_mod, acc_scale, R1, r1s, R2,
 def test_gemm(case, impl):
     ops, L = _ops()
     M, N, K, flags = case
-    if impl == "simt" and M * N * K > 3e9:
-        pytest.skip("SIMT reference kernel only checked on the small cases")
     g = torch.Generator(device=DEV).manual_seed(M + N + K)
     A = (torch.randn(M, K, device=DEV, generator=g) * 0.5).half()
     B = (torch.randn(N, K, device=DEV, generator=g) * 0.05).half()
@@ -154,8 +152,6 @@ def test_conv3x3_stride2_asymmetric_padding(case, impl):
     """SD-VAE Downsample2D: F.pad(x, (0, 1, 0, 1)) then conv(stride 2, padding 0) -- `conv_nopad_lo`."""
     ops, L = _ops()
     n, H, W, Cin, Cout = case
-    if impl == "simt" and H > 64:
-        pytest.skip("SIMT reference kernel only checked on the small cases")
     g = torch.Generator(device=DEV).manual_seed(sum(case))
     x = (torch.randn(n, H, W, Cin, device=DEV, generator=g) * 0.5).half()
     w = torch.randn(Cout, Cin, 3, 3, device=DEV, generator=g) * 0.05
@@ -219,8 +215,6 @@ def test_cross_view_attention(case, impl, layout):
     ops, L = _ops()
     name, B, Nv, Fr, hw, d = case
     heads = 8
-    if impl == "simt" and hw * Nv > 1024:
-        pytest.skip("SIMT reference kernel only checked on the small cases")
     gen = torch.Generator(device=DEV).manual_seed(hash(name) % 1000)
     dqk, dv = dqk_of(d), dv_of(d)
     rows = B * Nv * Fr * hw

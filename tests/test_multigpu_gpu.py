@@ -105,7 +105,7 @@ WORKER = textwrap.dedent(r'''
 ''')
 
 
-@pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs >= 2 GPUs on the box (gpurun --gpus 2)")
+@pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs >= 2 GPUs on one machine")
 def test_view_cfg_and_camera_sharding_over_nccl(tmp_path):
     script = tmp_path / "mgpu_worker.py"
     script.write_text(WORKER)

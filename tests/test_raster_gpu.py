@@ -1,4 +1,4 @@
-"""Rasterizer parity on a B200 against oracle/raster_oracle.py: sorted (tile|depth) keys, point_list and tile ranges
+"""Rasterizer parity on an H100 against oracle/raster_oracle.py: sorted (tile|depth) keys, point_list and tile ranges
 bit-exact per camera; colour/depth/alpha and every gradient tensor within fp32 tolerance; batched cameras with per-camera
 geometry; SH colour path; the diff_gaussian_rasterization-style single-camera API."""
 import ctypes as C

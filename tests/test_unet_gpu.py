@@ -1,4 +1,4 @@
-"""End-to-end parity of the B200 UNet engine against the fp32 CPU oracle (same seeded random weights and inputs).
+"""End-to-end parity of the H100 UNet engine against the fp32 CPU oracle (same seeded random weights and inputs).
 north_star tolerance: fp16 latents within 1e-2 relative (rel-L2 and max-abs/max-ref both asserted)."""
 import os
 

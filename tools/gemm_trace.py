@@ -1,4 +1,4 @@
-"""Per-tile timeline (SM clock cycles) of CTA 0 of the tcgen05 GEMM for one short-K shape."""
+"""Per-tile timeline (SM clock cycles) of CTA 0 of the tensor-core GEMM for one short-K shape."""
 import ctypes as C
 import os
 import sys
@@ -25,8 +25,8 @@ else:
 lib.a3d_debug_set_gemm_trace(C.c_void_p(None))
 t = buf.cpu().view(64, 16)
 t0 = int(t[0, 0])
-names = {0: "e:top", 1: "e:tfull", 2: "e:bias_bar", 3: "e:units_done", 8: "m:top", 9: "m:tempty", 10: "m:kb0_issued", 11: "m:tile_issued"}
-order = [0, 1, 2, 3, 8, 9, 10, 11]
+names = {0: "tile_start", 1: "mainloop_done", 2: "epilogue_done"}
+order = [0, 1, 2]
 print("tile " + " ".join(f"{names[k]:>13s}" for k in order))
 for j in list(range(0, 14)) + [30, 31, 32]:
     print(f"{j:4d} " + " ".join(f"{int(t[j, k]) - t0:13d}" for k in order))
