@@ -563,7 +563,7 @@ static int launch_shortkeys(const a3d_attn_args* a, int dqk, int dv, int kv_div,
   dim3 grid((unsigned)((Lq + rows_per_block - 1) / rows_per_block), (unsigned)a->heads, (unsigned)batches);
   attn_shortkeys_kernel<D><<<grid, 128, Cfg::kSmem, st>>>(q, k, v, reinterpret_cast<__half*>(a->out), a->os1, a->os2, a->os3, a->os4,
                                                           dqk, dv, a->scale * 1.4426950408889634f, kv_div, a->kv_i3_zero,
-                                                          a->accumulate, a->out_scale == 0.f ? 1.f : a->out_scale, rows_per_block);
+                                                          a->accumulate, a->out_scale, rows_per_block);
   A3D_LAUNCH_CHECK();
   return A3D_OK;
 }
@@ -651,7 +651,7 @@ extern "C" int a3d_attention(const a3d_attn_args* a, void* stream) {
     attn_simt_kernel<<<(unsigned)((total + 63) / 64), 64, 0, st>>>(q, k, v, reinterpret_cast<__half*>(a->out), a->os1, a->os2,
                                                                   a->os3, a->os4, a->heads, d, dqk, dv, a->scale, kv_div,
                                                                   a->kv_i3_zero, a->accumulate,
-                                                                  a->out_scale == 0.f ? 1.f : a->out_scale);
+                                                                  a->out_scale);
     A3D_LAUNCH_CHECK();
     return A3D_OK;
   }
@@ -671,7 +671,7 @@ extern "C" int a3d_attention(const a3d_attn_args* a, void* stream) {
     ViewDev v{reinterpret_cast<const __half*>(a->v.base), a->v.s1, a->v.s2, a->v.s3, a->v.s4, a->v.e1, a->v.e2, a->v.e3, a->v.e4};
     const int64_t total = (int64_t)batches * a->heads * a->q.e1 * a->q.e2;
     const unsigned blocks = (unsigned)((total + 255) / 256);
-    const float sl2 = a->scale * 1.4426950408889634f, osc = a->out_scale == 0.f ? 1.f : a->out_scale;
+    const float sl2 = a->scale * 1.4426950408889634f, osc = a->out_scale;
     __half* o = reinterpret_cast<__half*>(a->out);
     if (d == 40)
       attn_fewkeys_kernel<40><<<blocks, 256, 0, st>>>(q, k, v, o, a->os1, a->os2, a->os3, a->os4, a->heads, dqk, dv, sl2, kv_div,
@@ -712,7 +712,7 @@ extern "C" int a3d_attention(const a3d_attn_args* a, void* stream) {
   dev.out = reinterpret_cast<__half*>(a->out);
   dev.os1 = a->os1; dev.os2 = a->os2; dev.os3 = a->os3; dev.os4 = a->os4;
   dev.accumulate = a->accumulate;
-  dev.out_scale = a->out_scale == 0.f ? 1.f : a->out_scale;
+  dev.out_scale = a->out_scale;
   dev.dbg = g_attn_dbg;
   const CUtensorMap* mq;
   if (int r = view_map(a->q, qb1, qb2, &mq)) return r;

@@ -275,18 +275,21 @@ __global__ void gemm_simt_kernel(const GemmDev p, const __half* __restrict__ A, 
     return acc;
   };
   const int64_t orow = perm_row(m, p.perm_a, p.perm_b);
+  const float* rb = p.rowbias ? p.rowbias + ((m / p.rb_div) % p.rb_mod) * p.rb_ld : nullptr;
+  auto finish = [&](int64_t n) {   // same epilogue order as the tensor-core kernel's finish()
+    float v = dot(n);
+    if (p.bias) v += p.bias[n];
+    if (rb) v += rb[n];
+    return v * p.acc_scale;
+  };
   if (p.geglu) {
     const int64_t blk = j / 32, e = j % 32;
     const int64_t nu = blk * 64 + e, ng = nu + 32;
-    float u = dot(nu), g = dot(ng);
-    if (p.bias) { u += p.bias[nu]; g += p.bias[ng]; }
+    const float u = finish(nu), g = finish(ng);
     reinterpret_cast<__half*>(p.C)[orow * p.ldc + j] = __float2half_rn(u * gelu_erf(g));
     return;
   }
-  float v = dot(j);
-  if (p.bias) v += p.bias[j];
-  if (p.rowbias) v += p.rowbias[((m / p.rb_div) % p.rb_mod) * p.rb_ld + j];
-  v *= p.acc_scale;
+  float v = finish(j);
   if (p.R1) v += p.r1_scale * __half2float(p.R1[m * p.ldr1 + j]);
   if (p.R2) v += __half2float(p.R2[orow * p.ldr2 + j]);
   if (p.out_f32) reinterpret_cast<float*>(p.C)[orow * p.ldc + j] = v;

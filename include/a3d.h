@@ -106,7 +106,7 @@ typedef struct a3d_attn_args {
   int heads, d;             /* true head dim (40/80/160) */
   float scale;
   int kv_div, kv_i3_zero;
-  int accumulate; float out_scale;
+  int accumulate; float out_scale;  /* MUST be set (1.0 if unused; 0.0 is honoured, not remapped: accumulate leaves out as is) */
   int impl;                 /* A3D_GEMM_AUTO / _TCGEN05 / _SIMT */
 } a3d_attn_args;
 
@@ -270,7 +270,7 @@ int a3d_knn_graph(const float* points, int n, int K, int32_t* nbr, float* dist2,
  * R_i(t) = the weighted Procrustes rotation of the node's frame-0 edges onto its frame-t edges (no gradient through R).
  * nodes [Nt,Nv,3]; nbr [Nv,K] (-1 = no edge); weight [Nv,K] or NULL (1 on existing edges, the reference's call);
  * sample [Ns] node indices or NULL (all nodes).  err: device scalar; grad [Nt,Nv,3] = d err / d nodes or NULL.  Both are
- * zeroed here.  STATUS: arithmetic validated on the CPU (tests/test_arap_cpu.py); GPU run pending. */
+ * zeroed here.  Checked on the CPU (tests/test_arap_cpu.py) and on the GPU against the reference goldens (tests/test_arap_gpu.py). */
 int a3d_arap(const float* nodes, int Nt, int Nv, const int32_t* nbr, int K, const float* weight, const int32_t* sample, int Ns,
              float* err, float* grad, void* stream);
 

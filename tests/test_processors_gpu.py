@@ -64,6 +64,21 @@ def test_ip_adapter_processor_protocol(c, l):
         proc(attn, x.cuda(), encoder_hidden_states=text.cuda())
 
 
+def test_ip_adapter_processor_scale_zero():
+    """scale = 0 switches the image branch off: the processor equals its text-only attention."""
+    from animate3d_b200.modules import IPAdapterXFormersAttnProcessor
+    from oracle import unet_oracle as O
+    c, l, n = 320, 256, 6
+    proc = IPAdapterXFormersAttnProcessor(hidden_size=c, cross_attention_dim=768, num_tokens=(4,), scale=0.0, device="cuda")
+    attn, sd = _attn_and_sd(c, 768, c + 5, proc)
+    g = torch.Generator().manual_seed(7)
+    x, text, ip = torch.randn(n, l, c, generator=g), torch.randn(n, 77, 768, generator=g), torch.randn(n, 4, 768, generator=g)
+    got = proc(attn, x.cuda(), encoder_hidden_states=(text.cuda(), [ip.cuda()]))
+    ref = O.proc_ip_adapter(sd, "a", x, text, ip, HEADS, 0.0)
+    _close(got, ref, "IPAdapter scale=0")
+    assert ((O.proc_ip_adapter(sd, "a", x, text, ip, HEADS, 1.0) - ref).norm() / ref.norm()).item() > 1e-2
+
+
 @pytest.mark.parametrize("c,fs", [(320, 16), (1280, 4)])
 def test_spatiotemporal_processor_protocol(c, fs):
     from animate3d_b200.modules import SpatioTemporalI2VXFormersAttnProcessor

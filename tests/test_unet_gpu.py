@@ -8,17 +8,17 @@ import torch
 pytestmark = pytest.mark.gpu
 
 
-def _run(nv, nf, groups, seed=0, cond_zero=False, t=500, graph=True):
+def _run(nv, nf, groups, seed=0, cond_zero=False, t=500, graph=True, ip_scale=1.0):
     from animate3d_b200.unet import MVUNetMotionModel
     from animate3d_b200.unet_config import UNetConfig
     from oracle import unet_oracle as O
-    ocfg = O.UNetConfig(num_views=nv, num_frames=nf)
+    ocfg = O.UNetConfig(num_views=nv, num_frames=nf, ip_scale=ip_scale)
     sd = O.make_state_dict(ocfg, seed)
     sample, text, camera, img = O.synthetic_inputs(ocfg, groups, nv, nf, seed)
     torch.set_num_threads(min(16, os.cpu_count() or 1))   # many-core hosts: the fp32 oracle is fastest far below cpu_count
     with torch.no_grad():
         ref = O.unet_forward(sd, ocfg, sample, t, text, camera, img, nv, i2v_cond_time_zero=cond_zero)
-    model = MVUNetMotionModel(UNetConfig(num_views=nv, num_frames=nf))
+    model = MVUNetMotionModel(UNetConfig(num_views=nv, num_frames=nf, ip_scale=ip_scale))
     model.use_cuda_graph = graph
     missing, unexpected = model.load_state_dict(sd)
     assert not missing and not unexpected
@@ -47,6 +47,15 @@ def test_unet_plumbing_config_matches_oracle():
     # no float atomics anywhere on the path (GroupNorm statistics are a fixed-order tree): replays are bit-identical
     assert torch.equal(outs[1], outs[2])
     assert model.launches_per_forward > 500
+
+
+def test_unet_ip_scale_zero_matches_oracle():
+    """ip_scale = 0 turns the IP-adapter image branch off (attention_processor.py:283: hidden + scale * ip_hidden); the
+    accumulated attention call must add nothing, not the branch at full weight."""
+    ref, outs, _ = _run(1, 4, 1, seed=6, graph=False, ip_scale=0.0)
+    _check(ref, outs[0], "ip_scale = 0")
+    ref1, _, _ = _run(1, 4, 1, seed=6, graph=False, ip_scale=1.0)
+    assert ((ref1 - ref).norm() / ref.norm()).item() > 1e-2, "the image branch must matter for this check to mean anything"
 
 
 def test_unet_multiview_cfg_batch_matches_oracle():
