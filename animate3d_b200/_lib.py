@@ -54,7 +54,7 @@ class RasterArgs(C.Structure):
     _fields_ = [("P", C.c_int), ("H", C.c_int), ("W", C.c_int), ("num_cams", C.c_int), ("cams", C.c_void_p),
                 ("means3D", C.c_void_p), ("scales", C.c_void_p), ("rotations", C.c_void_p), ("opacities", C.c_void_p),
                 ("shs", C.c_void_p), ("colors_precomp", C.c_void_p), ("sh_degree", C.c_int), ("sh_coeffs", C.c_int),
-                ("per_cam_geometry", C.c_int), ("scale_modifier", C.c_float), ("bg", C.c_float * 3)]
+                ("per_cam_geometry", C.c_int), ("scale_modifier", C.c_float), ("bg", C.c_float * 3), ("deterministic", C.c_int)]
 
 
 _lib: Optional[C.CDLL] = None
@@ -77,6 +77,12 @@ def load(require_gpu: bool = True) -> C.CDLL:
         lib.a3d_group_norm_ws_bytes.restype = C.c_size_t
         lib.a3d_raster_workspace_bytes.restype = C.c_size_t
         lib.a3d_raster_workspace_bytes.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int64]
+        lib.a3d_raster_backward_scratch_bytes.restype = C.c_size_t
+        lib.a3d_raster_backward_scratch_bytes.argtypes = [C.c_void_p, C.c_int64]
+        lib.a3d_deform_backward_scratch_bytes.restype = C.c_size_t
+        lib.a3d_deform_backward_scratch_bytes.argtypes = [C.c_void_p]
+        lib.a3d_arap_deterministic_scratch_bytes.restype = C.c_size_t
+        lib.a3d_arap_deterministic_scratch_bytes.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int]
         _lib = lib
     if require_gpu and not _inited:
         if not torch.cuda.is_available():
@@ -97,3 +103,13 @@ def stream_ptr() -> C.c_void_p:
 
 def ptr(t: Optional[torch.Tensor]) -> Optional[int]:
     return None if t is None else t.data_ptr()
+
+
+def deterministic() -> int:
+    """1 when torch.use_deterministic_algorithms(True) is in effect: the 4D-path kernels then sum in a fixed order."""
+    return int(torch.are_deterministic_algorithms_enabled())
+
+
+def scratch(nbytes: int, device) -> Optional[torch.Tensor]:
+    """Caller-owned device scratch for the deterministic entry points (None when a size query returned 0)."""
+    return torch.empty(nbytes, dtype=torch.uint8, device=device) if nbytes else None

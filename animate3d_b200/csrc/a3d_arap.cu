@@ -6,6 +6,7 @@
 // hardware yet (round-1 GPU budget exhausted) -- tests/test_arap_gpu.py runs it in a subprocess.
 #include "a3d_host.cuh"
 #include "a3d_arap_math.h"
+#include "a3d_segsort.cuh"
 
 namespace a3d {
 
@@ -97,6 +98,123 @@ __global__ void __launch_bounds__(128) arap_kernel(const float* __restrict__ nod
   if (threadIdx.x == 0) atomicAdd(err, red[0] + red[1] + red[2] + red[3]);
 }
 
+// ---- deterministic variant: records instead of atomics, then fixed-order reductions
+// energy [(Nt-1)*Ns]; rec_t / rec_0 [(Nt-1)*Ns][K][3]: the frame-t and frame-0 edge gradients (+ to node i, - to neighbour j)
+__global__ void __launch_bounds__(128) arap_records_kernel(const float* __restrict__ nodes, int Nt, int Nv, const int* __restrict__ nbr,
+                                                           int K, const float* __restrict__ weight, const int* __restrict__ sample,
+                                                           int Ns, float* __restrict__ energy, float* __restrict__ rec_t,
+                                                           float* __restrict__ rec_0) {
+  const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= (int64_t)(Nt - 1) * Ns) return;
+  const int t = 1 + (int)(idx / Ns);
+  const int si = (int)(idx % Ns);
+  const int i = sample ? sample[si] : si;
+  float e0[kArapMaxK][3], et[kArapMaxK][3], g0[kArapMaxK][3], gt[kArapMaxK][3], w[kArapMaxK];
+  bool valid[kArapMaxK];
+  float en = 0.f;
+  const bool node_ok = i >= 0 && i < Nv;
+  if (node_ok) {
+    const float* p0 = nodes;
+    const float* pt = nodes + (int64_t)t * Nv * 3;
+#pragma unroll
+    for (int n = 0; n < kArapMaxK; ++n) {
+      const int j = n < K ? nbr[(int64_t)i * K + n] : -1;
+      valid[n] = j >= 0 && j < Nv;
+      w[n] = (n < K) ? (weight ? weight[(int64_t)i * K + n] : (valid[n] ? 1.f : 0.f)) : 0.f;
+#pragma unroll
+      for (int c = 0; c < 3; ++c) {
+        e0[n][c] = valid[n] ? p0[3 * (int64_t)i + c] - p0[3 * (int64_t)j + c] : 0.f;
+        et[n][c] = valid[n] ? pt[3 * (int64_t)i + c] - pt[3 * (int64_t)j + c] : 0.f;
+      }
+    }
+    en = arap_node(K, e0, et, valid, w, gt, g0);
+  }
+  energy[idx] = en;
+  for (int n = 0; n < K; ++n)
+    for (int c = 0; c < 3; ++c) {
+      const bool ok = node_ok && valid[n];
+      rec_t[(idx * K + n) * 3 + c] = ok ? gt[n][c] : 0.f;
+      rec_0[(idx * K + n) * 3 + c] = ok ? g0[n][c] : 0.f;
+    }
+}
+
+// one CTA: per-thread strided sums, then a fixed shared-memory tree
+__global__ void __launch_bounds__(1024) arap_energy_sum_kernel(const float* __restrict__ energy, int64_t n, float* __restrict__ err) {
+  __shared__ float s[1024];
+  float a = 0.f;
+  for (int64_t k = threadIdx.x; k < n; k += 1024) a += energy[k];
+  s[threadIdx.x] = a;
+  __syncthreads();
+  for (int h = 512; h > 0; h >>= 1) {
+    if ((int)threadIdx.x < h) s[threadIdx.x] += s[threadIdx.x + h];
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) *err = s[0];
+}
+
+// entry e = (si*K + n)*2 + side of the edge list: side 0 targets node i (+), side 1 its neighbour j (-); invalid -> key Nv
+__global__ void arap_targets_kernel(const int* __restrict__ nbr, int K, int Nv, const int* __restrict__ sample, int Ns,
+                                    uint32_t* __restrict__ keys, uint32_t* __restrict__ vals) {
+  const int e = blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= 2 * Ns * K) return;
+  const int si = e / (2 * K), n = (e >> 1) % K;
+  const int i = sample ? sample[si] : si;
+  int target = Nv;
+  if (i >= 0 && i < Nv) {
+    const int j = nbr[(int64_t)i * K + n];
+    if (j >= 0 && j < Nv) target = (e & 1) ? j : i;
+  }
+  keys[e] = (uint32_t)target;
+  vals[e] = (uint32_t)e;
+}
+
+// grad[t, v] = sum over v's entries in sorted order; frame 0 adds the frame-0 records of frames 1 .. Nt-1 in frame order
+__global__ void arap_gather_kernel(const uint2* __restrict__ ranges, const uint32_t* __restrict__ entries, const float* __restrict__ rec_t,
+                                   const float* __restrict__ rec_0, int Nt, int Nv, int64_t edges_per_frame, float* __restrict__ grad) {
+  const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= (int64_t)Nt * Nv) return;
+  const int t = (int)(idx / Nv), v = (int)(idx % Nv);
+  const uint2 r = ranges[v];
+  float g[3] = {0.f, 0.f, 0.f};
+  const int t_lo = t == 0 ? 1 : t, t_hi = t == 0 ? Nt - 1 : t;
+  const float* rec = t == 0 ? rec_0 : rec_t;
+  for (int tt = t_lo; tt <= t_hi; ++tt)
+    for (uint32_t k = r.x; k < r.y; ++k) {
+      const uint32_t e = entries[k];
+      // record of (frame tt, sample si, edge n) = (tt-1) * Ns*K + si*K + n, and e >> 1 = si*K + n
+      const float* rp = rec + 3 * ((int64_t)(tt - 1) * edges_per_frame + (e >> 1));
+      if (e & 1) { g[0] -= rp[0]; g[1] -= rp[1]; g[2] -= rp[2]; }
+      else       { g[0] += rp[0]; g[1] += rp[1]; g[2] += rp[2]; }
+    }
+  grad[3 * idx] = g[0]; grad[3 * idx + 1] = g[1]; grad[3 * idx + 2] = g[2];
+}
+
+struct ArapScratch {
+  float *energy, *rec_t, *rec_0;
+  uint32_t *keys_in, *vals_in, *keys_out, *vals_out;
+  uint2* ranges;
+  void* temp;
+  size_t temp_bytes;
+};
+
+static size_t carve_arap(void* base, int Nt, int Nv, int K, int Ns, ArapScratch* s) {
+  Carve c{static_cast<char*>(base)};
+  const size_t recs = (size_t)(Nt - 1) * Ns, entries = 2 * (size_t)Ns * K;
+  ArapScratch w;
+  w.energy = c.take<float>(recs);
+  w.rec_t = c.take<float>(recs * K * 3);
+  w.rec_0 = c.take<float>(recs * K * 3);
+  w.keys_in = c.take<uint32_t>(entries);
+  w.vals_in = c.take<uint32_t>(entries);
+  w.keys_out = c.take<uint32_t>(entries);
+  w.vals_out = c.take<uint32_t>(entries);
+  w.ranges = c.take<uint2>(Nv);
+  w.temp_bytes = seg_sort_temp_bytes((int)entries, (uint32_t)Nv);
+  w.temp = c.take<char>(w.temp_bytes);
+  if (s) *s = w;
+  return c.bytes();
+}
+
 }  // namespace a3d
 
 using namespace a3d;
@@ -124,5 +242,45 @@ extern "C" int a3d_arap(const float* nodes, int Nt, int Nv, const int32_t* nbr, 
     arap_kernel<<<(unsigned)((total + 127) / 128), 128, 0, st>>>(nodes, Nt, Nv, nbr, K, weight, sample, Ns, err, grad);
     A3D_LAUNCH_CHECK();
   }
+  return A3D_OK;
+}
+
+extern "C" size_t a3d_arap_deterministic_scratch_bytes(int Nt, int Nv, int K, int Ns) {
+  if (Nt < 1 || Nv < 1 || K < 1 || Ns < 1) return 0;
+  return carve_arap(nullptr, Nt, Nv, K, Ns, nullptr);
+}
+
+extern "C" int a3d_arap_deterministic(const float* nodes, int Nt, int Nv, const int32_t* nbr, int K, const float* weight,
+                                      const int32_t* sample, int Ns, float* err, float* grad, void* scratch, size_t scratch_bytes,
+                                      void* stream) {
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  if (!nodes || !nbr || !err || Nt < 1 || Nv < 1 || K < 1 || K > kArapMaxK)
+    return fail(A3D_EINVAL, "a3d_arap_deterministic: bad arguments (Nt=%d Nv=%d K=%d)", Nt, Nv, K);
+  if (!sample) Ns = Nv;
+  if (Ns < 1) return fail(A3D_EINVAL, "a3d_arap_deterministic: empty node sample");
+  if ((int64_t)Ns * K * 2 > 0x7fffffffll) return fail(A3D_EINVAL, "a3d_arap_deterministic: too many edges");
+  ArapScratch s;
+  const size_t need = carve_arap(scratch, Nt, Nv, K, Ns, &s);
+  if (!scratch || scratch_bytes < need) return fail(A3D_EINVAL, "a3d_arap_deterministic: scratch %zu < %zu bytes", scratch_bytes, need);
+  const int64_t total = (int64_t)(Nt - 1) * Ns;
+  if (total == 0) {
+    A3D_CUDA_CHECK(cudaMemsetAsync(err, 0, sizeof(float), st));
+    if (grad) A3D_CUDA_CHECK(cudaMemsetAsync(grad, 0, sizeof(float) * (size_t)Nt * Nv * 3, st));
+    return A3D_OK;
+  }
+  arap_records_kernel<<<(unsigned)((total + 127) / 128), 128, 0, st>>>(nodes, Nt, Nv, nbr, K, weight, sample, Ns, s.energy, s.rec_t,
+                                                                      s.rec_0);
+  A3D_LAUNCH_CHECK();
+  arap_energy_sum_kernel<<<1, 1024, 0, st>>>(s.energy, total, err);
+  A3D_LAUNCH_CHECK();
+  if (!grad) return A3D_OK;
+  const int entries = 2 * Ns * K;
+  arap_targets_kernel<<<(entries + 255) / 256, 256, 0, st>>>(nbr, K, Nv, sample, Ns, s.keys_in, s.vals_in);
+  A3D_LAUNCH_CHECK();
+  if (int r = seg_sort(s.keys_in, s.vals_in, s.keys_out, s.vals_out, entries, (uint32_t)Nv, s.ranges, s.temp, s.temp_bytes, st)) return r;
+  const int64_t nodes_total = (int64_t)Nt * Nv;
+  arap_gather_kernel<<<(unsigned)((nodes_total + 255) / 256), 256, 0, st>>>(s.ranges, s.vals_out, s.rec_t, s.rec_0, Nt, Nv,
+                                                                            (int64_t)Ns * K, grad);
+  A3D_LAUNCH_CHECK();
   return A3D_OK;
 }

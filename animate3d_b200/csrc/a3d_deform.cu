@@ -3,12 +3,15 @@
 //   over scales -> 32 features -> three bias-free MLPs 32 -> 32 (ReLU) -> {3, 4, 3} -> xyz + d, exp(s + d), normalize(q + d)
 // forward and backward (gradients to the plane grids and MLP weights; the static gaussians are frozen buffers in
 // Animate3D, gaussian_4d.py:262-297).  The `use_global_trans` branch (gaussian_4d.py:499-511, 525-539) needs the MEAN feature
-// vector of a frame before any output can be formed: kMode 2 computes those means (one extra pass over the L2-resident
-// planes), the host evaluates the two 32-wide global MLPs + Euler matrix on [T, 32], and the main pass takes the rotated
-// base quaternions as `rot_base`; backward returns d/d rot_base and folds d/d mean-feature back into the plane gradients.  Replaces, per (frame, gaussian), the 12 grid_sample + 6 GEMM + elementwise launches the
+// vector of a frame before any output can be formed: deform_featmean_kernel computes those means (one extra pass over the
+// L2-resident planes, summed in a fixed order), the host evaluates the two 32-wide global MLPs + Euler matrix on [T, 32],
+// and the main pass takes the rotated base quaternions as `rot_base`; backward returns d/d rot_base and folds d/d mean-feature back into the plane gradients.  Replaces, per (frame, gaussian), the 12 grid_sample + 6 GEMM + elementwise launches the
 // reference issues PER CAMERA (custom/threestudio-animate3d/geometry/gaussian_4d.py:39-64, 450-548;
 // renderer/diff_gaussian_rasterizer_advanced_4d.py:77-83, 119-135) and de-duplicates the 4 views of a frame.
+#include <cooperative_groups.h>
+
 #include "a3d_host.cuh"
+#include "a3d_segsort.cuh"
 
 namespace a3d {
 
@@ -53,34 +56,24 @@ struct DeformGlobal {
   const float* rot_base;      // [T,P,4] per-frame base quaternions (replace `rotation`) or null
   float* g_rot_base;          // backward: d/d rot_base, [T,P,4], or null
   const float* g_featmean;    // backward: d/d (mean feature of frame t), [T, nfeat], or null
-  float* featmean;            // kMode 2: [T, nfeat], pre-zeroed; receives sum / P
 };
 
-// kMode: 0 = forward, 2 = per-frame mean of the k-planes features only (backward: deform_backward_kernel)
-template <int kMode>
 __global__ void __launch_bounds__(128)
 deform_kernel(DeformGrids G, DeformMlp M, DeformGlobal X, const float* __restrict__ xyz, const float* __restrict__ scaling,
               const float* __restrict__ rotation, const float* __restrict__ times, int P, int T, int deform_scale,
-              float* __restrict__ out_means, float* __restrict__ out_scales, float* __restrict__ out_rots,
-              const float* __restrict__ g_means, const float* __restrict__ g_scales, const float* __restrict__ g_rots) {
-  constexpr bool kBackward = false;
-  static_assert(kMode == 0 || kMode == 2, "backward is a separate kernel");
+              float* __restrict__ out_means, float* __restrict__ out_scales, float* __restrict__ out_rots) {
   extern __shared__ __align__(16) float sm[];
   // shared copies of the MLP weights
   float* sw1 = sm;                                   // [3][32][32]
   float* sw2 = sw1 + 3 * kHid * kHid;                // [3][4][32] (padded to 4 outputs)
   const int nfeat = G.scales * kFeat;
-  if (kMode != 2) {
-    for (int i = threadIdx.x; i < 3 * kHid * kHid; i += blockDim.x) {
-      const int m = i / (kHid * kHid), r = i % (kHid * kHid);
-      sw1[i] = (r % kHid < nfeat) ? M.w1[m][(r / kHid) * nfeat + r % kHid] : 0.f;
-    }
-    for (int i = threadIdx.x; i < 3 * 4 * kHid; i += blockDim.x) {
-      const int m = i / (4 * kHid), r = (i % (4 * kHid)) / kHid, c = i % kHid;
-      sw2[i] = r < out_dim(m) ? M.w2[m][r * kHid + c] : 0.f;
-    }
-  } else {
-    for (int i = threadIdx.x; i < 2 * kHid; i += blockDim.x) sm[i] = 0.f;   // [2 frames a block may straddle][32]
+  for (int i = threadIdx.x; i < 3 * kHid * kHid; i += blockDim.x) {
+    const int m = i / (kHid * kHid), r = i % (kHid * kHid);
+    sw1[i] = (r % kHid < nfeat) ? M.w1[m][(r / kHid) * nfeat + r % kHid] : 0.f;
+  }
+  for (int i = threadIdx.x; i < 3 * 4 * kHid; i += blockDim.x) {
+    const int m = i / (4 * kHid), r = (i % (4 * kHid)) / kHid, c = i % kHid;
+    sw2[i] = r < out_dim(m) ? M.w2[m][r * kHid + c] : 0.f;
   }
   __syncthreads();
   const int idx = blockIdx.x * blockDim.x + threadIdx.x;
@@ -107,26 +100,6 @@ deform_kernel(DeformGrids G, DeformMlp M, DeformGlobal X, const float* __restric
           feat[s * kFeat + c] *= v;
         }
       }
-  }
-  if (kMode == 2) {
-    // block-level sum per frame (a 128-thread block touches at most two frames when P >= 128), then one atomic per value
-    const int t_first = (blockIdx.x * blockDim.x) / P;
-    if (active) {
-      const int slot = t - t_first;
-      if (slot < 2) {
-#pragma unroll
-        for (int c = 0; c < kHid; ++c) if (c < nfeat) atomicAdd(&sm[slot * kHid + c], feat[c]);
-      } else {
-#pragma unroll
-        for (int c = 0; c < kHid; ++c) if (c < nfeat) atomicAdd(&X.featmean[(size_t)t * nfeat + c], feat[c] / (float)P);
-      }
-    }
-    __syncthreads();
-    for (int k = threadIdx.x; k < 2 * kHid; k += blockDim.x) {
-      const int slot = k / kHid, c = k % kHid;
-      if (c < nfeat && t_first + slot < T && sm[k] != 0.f) atomicAdd(&X.featmean[(size_t)(t_first + slot) * nfeat + c], sm[k] / (float)P);
-    }
-    return;
   }
   // ---- three MLPs
   // the weights are broadcast reads from shared memory: 16-byte loads (4 FMAs per load) -- with scalar loads the kernel sat on
@@ -168,16 +141,12 @@ deform_kernel(DeformGrids G, DeformMlp M, DeformGlobal X, const float* __restric
     qn = fmaxf(sqrtf(q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3]), 1e-12f);
     for (int k = 0; k < 3; ++k) sc[k] = expf(scaling[3 * i + k] + (deform_scale ? outv[2][k] : 0.f));
   }
-  if (!kBackward) {
-    if (active) {
-      const size_t o = (size_t)t * P + i;
-      for (int k = 0; k < 3; ++k) out_means[3 * o + k] = pt[k] + outv[0][k];
-      for (int k = 0; k < 3; ++k) out_scales[3 * o + k] = sc[k];
-      for (int k = 0; k < 4; ++k) out_rots[4 * o + k] = q[k] / qn;
-    }
-    return;
+  if (active) {
+    const size_t o = (size_t)t * P + i;
+    for (int k = 0; k < 3; ++k) out_means[3 * o + k] = pt[k] + outv[0][k];
+    for (int k = 0; k < 3; ++k) out_scales[3 * o + k] = sc[k];
+    for (int k = 0; k < 4; ++k) out_rots[4 * o + k] = q[k] / qn;
   }
-  // kMode 1 (backward) lives in deform_backward_kernel below
 }
 
 
@@ -209,10 +178,63 @@ __device__ __forceinline__ float plane_sample(const float* __restrict__ gc, cons
          (__ldg(gc + b.y1 * W + b.x0) * (1.f - b.wx) + __ldg(gc + b.y1 * W + b.x1) * b.wx) * b.wy;
 }
 
+// Per-frame mean feature in a fixed order: a cluster of kFmCtas CTAs per frame; each thread sums a strided subset of the
+// gaussians, each CTA sums its threads in thread order, and CTA rank 0 adds the cluster's CTA sums in rank order through
+// distributed shared memory.  No atomics and no scratch: bit-reproducible for a given launch geometry.
+constexpr int kFmCtas = 8, kFmThreads = 256;
+
+__global__ void __cluster_dims__(kFmCtas, 1, 1) __launch_bounds__(kFmThreads)
+deform_featmean_kernel(DeformGrids G, const float* __restrict__ xyz, const float* __restrict__ times, int P, float* __restrict__ featmean) {
+  namespace cg = cooperative_groups;
+  cg::cluster_group cluster = cg::this_cluster();
+  __shared__ float s_rows[kFmThreads][kHid + 1];
+  __shared__ float s_cta[kHid];
+  const int rank = (int)cluster.block_rank(), t = blockIdx.y, nfeat = G.scales * kFeat;
+  float acc[kHid];
+#pragma unroll
+  for (int c = 0; c < kHid; ++c) acc[c] = 0.f;
+  const float tm = times[t];
+  for (int i = rank * kFmThreads + threadIdx.x; i < P; i += kFmCtas * kFmThreads) {
+    const float pt[4] = {xyz[3 * i], xyz[3 * i + 1], xyz[3 * i + 2], tm};
+    float feat[kHid];
+#pragma unroll
+    for (int c = 0; c < kHid; ++c) feat[c] = 1.f;
+    for (int sc = 0; sc < G.scales; ++sc)
+      for (int pl = 0; pl < kPlanes; ++pl) {
+        const int W = G.w[sc][pl], H = G.h[sc][pl];
+        const Bilerp b = bilerp_setup(pt[c_comb[pl][0]], pt[c_comb[pl][1]], W, H);
+#pragma unroll
+        for (int c = 0; c < kFeat; ++c) feat[sc * kFeat + c] *= plane_sample(G.plane[sc][pl] + (size_t)c * H * W, b, W);
+      }
+#pragma unroll
+    for (int c = 0; c < kHid; ++c) acc[c] += feat[c];
+  }
+#pragma unroll
+  for (int c = 0; c < kHid; ++c) s_rows[threadIdx.x][c] = acc[c];
+  __syncthreads();
+  if (threadIdx.x < kHid) {
+    float a = 0.f;
+    for (int r = 0; r < kFmThreads; ++r) a += s_rows[r][threadIdx.x];
+    s_cta[threadIdx.x] = a;
+  }
+  cluster.sync();
+  if (rank == 0 && threadIdx.x < nfeat) {
+    float a = 0.f;
+    for (int r = 0; r < kFmCtas; ++r) a += cluster.map_shared_rank(s_cta, r)[threadIdx.x];
+    featmean[(size_t)t * nfeat + threadIdx.x] = a / (float)P;
+  }
+  cluster.sync();   // the other CTAs' shared memory must outlive rank 0's reads
+}
+
+// kDet: plane gradients are not scattered; every (scale, plane, frame, gaussian) stores its 16-channel factor
+// (d loss / d feature x product of the other planes' samples) to fac[plane][point][16], and the per-thread weight-gradient
+// entries go to part[CTA][...] instead of global atomics
+template <bool kDet>
 __global__ void __launch_bounds__(kBwdThreads, 2)
 deform_backward_kernel(DeformGrids G, DeformMlp M, DeformGlobal X, const float* __restrict__ xyz, const float* __restrict__ scaling,
                        const float* __restrict__ rotation, const float* __restrict__ times, int P, int T, int deform_scale,
-                       const float* __restrict__ g_means, const float* __restrict__ g_scales, const float* __restrict__ g_rots) {
+                       const float* __restrict__ g_means, const float* __restrict__ g_scales, const float* __restrict__ g_rots,
+                       float* __restrict__ fac, float* __restrict__ part) {
   extern __shared__ __align__(16) float sm[];
   float* sw1 = sm;                                   // [3][32][32]
   float* sw2 = sw1 + 3 * kHid * kHid;                // [3][4][32]
@@ -389,6 +411,13 @@ deform_backward_kernel(DeformGrids G, DeformMlp M, DeformGlobal X, const float* 
               pre *= smp[pl];
             }
           }
+          if (kDet) {
+#pragma unroll
+            for (int pl = 0; pl < kPlanes; ++pl)
+              *reinterpret_cast<float4*>(fac + ((size_t)(s * kPlanes + pl) * total + idx) * kFeat + c0) =
+                  make_float4(ds[pl][0], ds[pl][1], ds[pl][2], ds[pl][3]);
+            continue;
+          }
 #pragma unroll
           for (int pl = 0; pl < kPlanes; ++pl) {
             const float d0 = ds[pl][0], d1 = ds[pl][1], d2 = ds[pl][2], d3 = ds[pl][3];
@@ -407,6 +436,10 @@ deform_backward_kernel(DeformGrids G, DeformMlp M, DeformGlobal X, const float* 
     }
   }
   __syncthreads();
+  if (kDet) {   // this CTA's partials, reduced in CTA order by deform_wgrad_reduce_kernel
+    for (int e = threadIdx.x; e < 3 * kOwn * kBwdThreads; e += kBwdThreads) part[(size_t)blockIdx.x * 3 * kOwn * kBwdThreads + e] = s_acc[e];
+    return;
+  }
   // ---- one global atomic per owned weight-gradient entry
   for (int m = 0; m < 3; ++m) {
     if (M.gw1[m]) {
@@ -425,19 +458,75 @@ deform_backward_kernel(DeformGrids G, DeformMlp M, DeformGlobal X, const float* 
   }
 }
 
+// entry e of the [3][kOwn][kBwdThreads] partials: MLP m, owned slot j of thread tid (see deform_backward_kernel)
+__global__ void deform_wgrad_reduce_kernel(DeformMlp M, const float* __restrict__ part, int ctas, int nfeat) {
+  const int e = blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= 3 * kOwn * kBwdThreads) return;
+  float a = 0.f;
+  for (int b = 0; b < ctas; ++b) a += part[(size_t)b * 3 * kOwn * kBwdThreads + e];
+  const int m = e / (kOwn * kBwdThreads), j = (e / kBwdThreads) % kOwn, tid = e % kBwdThreads;
+  if (j < 8) {
+    const int r1 = tid >> 2, c1 = (tid & 3) * 8;
+    if (M.gw1[m] && c1 + j < nfeat) M.gw1[m][r1 * nfeat + c1 + j] += a;
+  } else {
+    const int ee = tid + (j - 8) * kBwdThreads;
+    if (M.gw2[m] && (ee >> 5) < out_dim(m)) M.gw2[m][(ee >> 5) * kHid + (ee & 31)] += a;
+  }
+}
+
+// key of point idx for one plane: its lower-left cell y0 * W + x0
+__global__ void deform_cell_keys_kernel(const float* __restrict__ xyz, const float* __restrict__ times, int P, long long total, int ca,
+                                        int cb, int W, int H, uint32_t* __restrict__ keys, uint32_t* __restrict__ vals) {
+  const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= total) return;
+  const int t = (int)(idx / P), i = (int)(idx % P);
+  const float pt[4] = {xyz[3 * i], xyz[3 * i + 1], xyz[3 * i + 2], times[t]};
+  const Bilerp b = bilerp_setup(pt[ca], pt[cb], W, H);
+  keys[idx] = (uint32_t)(b.y0 * W + b.x0);
+  vals[idx] = (uint32_t)idx;
+}
+
+// gradient of texel (y, x), 4 channels per thread: the points of cells (y-1, x-1), (y-1, x), (y, x-1), (y, x) in that order,
+// each cell's points in their stable sorted order; a point's weight on this texel is its bilinear weight of the matching corner
+__global__ void deform_plane_gather_kernel(const float* __restrict__ xyz, const float* __restrict__ times, int P, int ca, int cb,
+                                           int W, int H, const uint2* __restrict__ ranges, const uint32_t* __restrict__ pts,
+                                           const float* __restrict__ fac, float* __restrict__ gplane) {
+  const int idx = blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= H * W * 4) return;
+  const int c0 = (idx & 3) * 4, texel = idx >> 2, y = texel / W, x = texel % W;
+  float a[4] = {0.f, 0.f, 0.f, 0.f};
+  for (int cy = y - 1; cy <= y; ++cy)
+    for (int cx = x - 1; cx <= x; ++cx) {
+      if (cy < 0 || cx < 0) continue;
+      const uint2 r = ranges[cy * W + cx];
+      for (uint32_t k = r.x; k < r.y; ++k) {
+        const uint32_t p = pts[k];
+        const int t = (int)(p / (uint32_t)P), i = (int)(p % (uint32_t)P);
+        const float pt[4] = {xyz[3 * i], xyz[3 * i + 1], xyz[3 * i + 2], times[t]};
+        const Bilerp b = bilerp_setup(pt[ca], pt[cb], W, H);
+        // corner (y1, x1) of a cell on the last row / column coincides with (y0, x0) and has weight 0 there
+        const float w = (cy == y ? 1.f - b.wy : b.wy) * (cx == x ? 1.f - b.wx : b.wx);
+        const float4 f = *reinterpret_cast<const float4*>(fac + (size_t)p * kFeat + c0);
+        a[0] += f.x * w; a[1] += f.y * w; a[2] += f.z * w; a[3] += f.w * w;
+      }
+    }
+  float4* dst = reinterpret_cast<float4*>(gplane + (size_t)texel * kFeat + c0);
+  float4 v = *dst;
+  v.x += a[0]; v.y += a[1]; v.z += a[2]; v.w += a[3];
+  *dst = v;
+}
+
 }  // namespace a3d
 
 using namespace a3d;
 
-static DeformGlobal globals(const a3d_deform_args* a, float* featmean) {
+static DeformGlobal globals(const a3d_deform_args* a) {
   DeformGlobal X;
-  X.rot_base = a->rot_base; X.g_rot_base = a->grad_rot_base; X.g_featmean = a->grad_featmean; X.featmean = featmean;
+  X.rot_base = a->rot_base; X.g_rot_base = a->grad_rot_base; X.g_featmean = a->grad_featmean;
   return X;
 }
 
 static int fill(const a3d_deform_args* a, DeformGrids* G, DeformMlp* M) {
-  const bool bwd = a && a->grad_w1[0] != nullptr;
-  (void)bwd;
   if (!a || a->P <= 0 || a->T <= 0) return fail(A3D_EINVAL, "a3d_deform: bad sizes");
   if (a->num_scales < 1 || a->num_scales > kMaxScales || a->channels != kFeat || a->hidden != kHid)
     return fail(A3D_EINVAL, "a3d_deform: supports 1-2 scales x 16 channels and 32-wide MLPs (got %d x %d, hidden %d)", a->num_scales,
@@ -468,8 +557,8 @@ extern "C" int a3d_deform_forward(const a3d_deform_args* a, float* means, float*
   if (int r = fill(a, &G, &M)) return r;
   const int n = a->P * a->T;
   const size_t smem = (3 * kHid * kHid + 3 * 4 * kHid) * sizeof(float);
-  deform_kernel<0><<<(n + 127) / 128, 128, smem, st>>>(G, M, globals(a, nullptr), a->xyz, a->scaling, a->rotation, a->times, a->P, a->T,
-                                                      a->deform_scale, means, scales, rots, nullptr, nullptr, nullptr);
+  deform_kernel<<<(n + 127) / 128, 128, smem, st>>>(G, M, globals(a), a->xyz, a->scaling, a->rotation, a->times, a->P, a->T,
+                                                   a->deform_scale, means, scales, rots);
   A3D_LAUNCH_CHECK();
   return A3D_OK;
 }
@@ -479,18 +568,60 @@ extern "C" int a3d_deform_featmean(const a3d_deform_args* a, float* featmean, vo
   DeformGrids G; DeformMlp M;
   if (int r = fill(a, &G, &M)) return r;
   if (!featmean) return fail(A3D_EINVAL, "a3d_deform_featmean: null output");
-  if (a->P < 128) return fail(A3D_EINVAL, "a3d_deform_featmean: needs at least 128 gaussians (got %d)", a->P);
-  const int n = a->P * a->T;
-  A3D_CUDA_CHECK(cudaMemsetAsync(featmean, 0, sizeof(float) * a->T * a->num_scales * kFeat, st));
-  const size_t smem = (3 * kHid * kHid + 3 * 4 * kHid) * sizeof(float);
-  deform_kernel<2><<<(n + 127) / 128, 128, smem, st>>>(G, M, globals(a, featmean), a->xyz, a->scaling, a->rotation, a->times, a->P, a->T,
-                                                      a->deform_scale, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr);
+  if (a->T > 65535) return fail(A3D_EINVAL, "a3d_deform_featmean: at most 65535 frames (got %d)", a->T);
+  deform_featmean_kernel<<<dim3(kFmCtas, a->T), kFmThreads, 0, st>>>(G, a->xyz, a->times, a->P, featmean);
   A3D_LAUNCH_CHECK();
   return A3D_OK;
 }
 
-extern "C" int a3d_deform_backward(const a3d_deform_args* a, const float* g_means, const float* g_scales, const float* g_rots,
-                                   void* stream) {
+// ---- backward
+constexpr size_t kBwdSmem = (3 * kHid * kHid + 3 * 4 * kHid + 3 * kBwdThreads * kLdS + kBwdThreads * 4 + 3 * kOwn * kBwdThreads) * sizeof(float);
+
+static long long backward_ctas(long long n) {
+  long long blocks = (n + kBwdThreads - 1) / kBwdThreads;
+  const long long cap = 2ll * sm_count();              // persistent: 2 blocks (86 KB shared each) per SM
+  return blocks > cap ? cap : blocks;
+}
+
+struct DeformDetScratch {
+  float* fac;                    // [num_scales * 6][T * P][16]
+  float* part;                   // [ctas][3 * kOwn * kBwdThreads]
+  uint32_t *keys_in, *vals_in, *keys_out, *vals_out;   // [T * P]
+  uint2* ranges;                 // [largest plane's H * W]
+  void* temp;
+  size_t temp_bytes;
+};
+
+static size_t carve_det(void* base, const a3d_deform_args* a, DeformDetScratch* s) {
+  Carve c{static_cast<char*>(base)};
+  const size_t n = (size_t)a->P * a->T;
+  uint32_t cells = 1;
+  for (int p = 0; p < a->num_scales * kPlanes; ++p) {
+    const uint32_t hw = (uint32_t)a->plane_h[p] * (uint32_t)a->plane_w[p];
+    if (hw > cells) cells = hw;
+  }
+  DeformDetScratch w;
+  w.fac = c.take<float>((size_t)a->num_scales * kPlanes * n * kFeat);
+  w.part = c.take<float>((size_t)backward_ctas((long long)n) * 3 * kOwn * kBwdThreads);
+  w.keys_in = c.take<uint32_t>(n);
+  w.vals_in = c.take<uint32_t>(n);
+  w.keys_out = c.take<uint32_t>(n);
+  w.vals_out = c.take<uint32_t>(n);
+  w.ranges = c.take<uint2>(cells);
+  w.temp_bytes = seg_sort_temp_bytes((int)n, cells);
+  w.temp = c.take<char>(w.temp_bytes);
+  if (s) *s = w;
+  return c.bytes();
+}
+
+extern "C" size_t a3d_deform_backward_scratch_bytes(const a3d_deform_args* a) {
+  DeformGrids G; DeformMlp M;
+  if (!a || !a->deterministic || fill(a, &G, &M)) return 0;
+  return carve_det(nullptr, a, nullptr);
+}
+
+extern "C" int a3d_deform_backward_ex(const a3d_deform_args* a, const float* g_means, const float* g_scales, const float* g_rots,
+                                      void* scratch, size_t scratch_bytes, void* stream) {
   // grad_planes[i]: CHANNEL-LAST scratch [H_i, W_i, 16] (zero-initialised by the caller, accumulated into); the caller transposes
   // it into the [1, 16, H, W] parameter gradient (animate3d_b200/gaussian4d.py)
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
@@ -505,20 +636,52 @@ extern "C" int a3d_deform_backward(const a3d_deform_args* a, const float* g_mean
         return fail(A3D_EINVAL, "a3d_deform_backward: plane gradient scratch must be 16-byte aligned");
   }
   const long long n = (long long)a->P * a->T;
-  const size_t smem = (3 * kHid * kHid + 3 * 4 * kHid + 3 * kBwdThreads * kLdS + kBwdThreads * 4 + 3 * kOwn * kBwdThreads) * sizeof(float);
+  const bool det = a->deterministic != 0;
+  DeformDetScratch s{};
+  if (det) {
+    if (n > 0x7fffffffll) return fail(A3D_EINVAL, "a3d_deform_backward: T * P too large for the deterministic path");
+    const size_t need = carve_det(scratch, a, &s);
+    if (!scratch || scratch_bytes < need) return fail(A3D_EINVAL, "a3d_deform_backward: deterministic scratch %zu < %zu bytes", scratch_bytes, need);
+  }
   static bool attr = false;
-  static int sms = 0;
   if (!attr) {
-    A3D_CUDA_CHECK(cudaFuncSetAttribute(deform_backward_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    A3D_CUDA_CHECK(cudaFuncSetAttribute(deform_backward_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kBwdSmem));
+    A3D_CUDA_CHECK(cudaFuncSetAttribute(deform_backward_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kBwdSmem));
     attr = true;
   }
-  long long blocks = (n + kBwdThreads - 1) / kBwdThreads;
-  if (blocks > 2ll * sms) blocks = 2ll * sms;          // persistent: 2 blocks (86 KB shared each) per SM
-  deform_backward_kernel<<<(unsigned)blocks, kBwdThreads, smem, st>>>(G, M, globals(a, nullptr), a->xyz, a->scaling, a->rotation, a->times,
-                                                                     a->P, a->T, a->deform_scale, g_means, g_scales, g_rots);
+  const long long blocks = backward_ctas(n);
+  if (!det) {
+    deform_backward_kernel<false><<<(unsigned)blocks, kBwdThreads, kBwdSmem, st>>>(G, M, globals(a), a->xyz, a->scaling, a->rotation,
+                                                                                  a->times, a->P, a->T, a->deform_scale, g_means, g_scales,
+                                                                                  g_rots, nullptr, nullptr);
+    A3D_LAUNCH_CHECK();
+    return A3D_OK;
+  }
+  deform_backward_kernel<true><<<(unsigned)blocks, kBwdThreads, kBwdSmem, st>>>(G, M, globals(a), a->xyz, a->scaling, a->rotation,
+                                                                               a->times, a->P, a->T, a->deform_scale, g_means, g_scales,
+                                                                               g_rots, s.fac, s.part);
   A3D_LAUNCH_CHECK();
+  deform_wgrad_reduce_kernel<<<(3 * kOwn * kBwdThreads + 255) / 256, 256, 0, st>>>(M, s.part, (int)blocks, G.scales * kFeat);
+  A3D_LAUNCH_CHECK();
+  for (int sc = 0; sc < G.scales; ++sc) {
+    if (!G.gplane[sc][0]) continue;
+    for (int pl = 0; pl < kPlanes; ++pl) {
+      static const int comb[kPlanes][2] = {{0, 1}, {0, 2}, {0, 3}, {1, 2}, {1, 3}, {2, 3}};   // = c_comb
+      const int W = G.w[sc][pl], H = G.h[sc][pl], ca = comb[pl][0], cb = comb[pl][1];
+      deform_cell_keys_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(a->xyz, a->times, a->P, n, ca, cb, W, H, s.keys_in, s.vals_in);
+      A3D_LAUNCH_CHECK();
+      if (int r = seg_sort(s.keys_in, s.vals_in, s.keys_out, s.vals_out, (int)n, (uint32_t)(H * W), s.ranges, s.temp, s.temp_bytes, st))
+        return r;
+      deform_plane_gather_kernel<<<(H * W * 4 + 255) / 256, 256, 0, st>>>(a->xyz, a->times, a->P, ca, cb, W, H, s.ranges, s.vals_out,
+                                                                          s.fac + (size_t)(sc * kPlanes + pl) * n * kFeat, G.gplane[sc][pl]);
+      A3D_LAUNCH_CHECK();
+    }
+  }
   return A3D_OK;
+}
+
+extern "C" int a3d_deform_backward(const a3d_deform_args* a, const float* g_means, const float* g_scales, const float* g_rots,
+                                   void* stream) {
+  if (a && a->deterministic) return fail(A3D_EINVAL, "a3d_deform_backward: deterministic = 1 needs a3d_deform_backward_ex's scratch");
+  return a3d_deform_backward_ex(a, g_means, g_scales, g_rots, nullptr, 0, stream);
 }

@@ -78,9 +78,18 @@ __device__ __forceinline__ float warp_sum(float v) {
   return v;
 }
 
+// kDet: instead of atomics, every warp parks its 10 totals of list entry j in s_part[warp][j]; after each round of 256
+// entries the CTA adds the 8 warps in warp order and stores one record per (camera, tile, gaussian) pair at the pair's slot
+// of the pre-sort (duplicate-kernel) order: offset of (camera, gaussian) + row-major index of the tile in its rect.
+constexpr int kRecord = 10;   // dmean2D x, y, dconic a, b, c, dopacity, drgb 0..2, ddepth
+constexpr int kWarps = kBlockPix / 32;
+constexpr size_t kDetSmem = (size_t)kWarps * kBlockPix * kRecord * sizeof(float);
+
+template <bool kDet>
 __global__ void __launch_bounds__(kBlockPix)
 raster_render_backward_kernel(RasterDev a, RasterWs ws, const float* __restrict__ dL_dcolor, const float* __restrict__ dL_ddepth,
-                              const float* __restrict__ dL_dalpha, float* __restrict__ dL_dopacity) {
+                              const float* __restrict__ dL_dalpha, float* __restrict__ dL_dopacity, float* __restrict__ records) {
+  extern __shared__ float s_part[];   // kDet: [kWarps][kBlockPix][kRecord]
   const int gx = (a.W + kTile - 1) / kTile, gy = (a.H + kTile - 1) / kTile;
   const int cam = blockIdx.z;
   const int tile = blockIdx.y * gx + blockIdx.x;
@@ -140,8 +149,12 @@ raster_render_backward_kernel(RasterDev a, RasterWs ws, const float* __restrict_
     }
     __syncthreads();
     const int n = (total - r * kBlockPix) < kBlockPix ? (total - r * kBlockPix) : kBlockPix;
+    float* my_part = s_part + (size_t)(tid >> 5) * kBlockPix * kRecord;
     for (int j = 0; j < n; ++j, --contributor) {
-      if (contributor > warp_last) continue;
+      if (contributor > warp_last) {
+        if (kDet && lane < kRecord) my_part[j * kRecord + lane] = 0.f;
+        continue;
+      }
       SplatGrad g;
       g.dmx = g.dmy = g.dconA = g.dconB = g.dconC = g.dopac = g.ddepth = 0.f;
       g.dcol[0] = g.dcol[1] = g.dcol[2] = 0.f;
@@ -160,7 +173,10 @@ raster_render_backward_kernel(RasterDev a, RasterWs ws, const float* __restrict_
                          dD, dA, a.bg, acc_col, acc_d, acc_a, last_alpha, last_col, last_d, g);
         }
       }
-      if (!__any_sync(0xffffffffu, active)) continue;
+      if (!__any_sync(0xffffffffu, active)) {
+        if (kDet && lane < kRecord) my_part[j * kRecord + lane] = 0.f;
+        continue;
+      }
       // Transposing butterfly: the 10 partial gradients (padded to 16) of the warp's 32 pixels are reduced with 16 shuffles
       // instead of 10 x 5; afterwards lane 2k holds the warp total of value k and lanes 0, 2, ..., 18 issue their ONE atomic
       // in parallel (the upstream kernel: one atomic per pixel and value; round 1 here: 50 shuffles + 10 serial atomics).
@@ -177,7 +193,29 @@ raster_render_backward_kernel(RasterDev a, RasterWs ws, const float* __restrict_
         }
       }
       const float total = v[0] + __shfl_xor_sync(0xffffffffu, v[0], 1);
-      if (tgt_base) atomicAdd(tgt_base + tgt_mul * (tgt_off + (size_t)s_id[j]) + tgt_add, total);
+      if (kDet) {
+        if (!(lane & 1) && lane < 2 * kRecord) my_part[j * kRecord + (lane >> 1)] = total;
+      } else if (tgt_base) {
+        atomicAdd(tgt_base + tgt_mul * (tgt_off + (size_t)s_id[j]) + tgt_add, total);
+      }
+    }
+    if (kDet) {
+      __syncthreads();
+      if (tid < n) {
+        float rec[kRecord];
+#pragma unroll
+        for (int k = 0; k < kRecord; ++k) rec[k] = 0.f;
+#pragma unroll 1
+        for (int w = 0; w < kWarps; ++w)
+#pragma unroll
+          for (int k = 0; k < kRecord; ++k) rec[k] += s_part[((size_t)w * kBlockPix + tid) * kRecord + k];
+        const size_t gi = cbase + s_id[tid];
+        const int4 rc = ws.rect[gi];
+        const size_t slot = (gi ? ws.offsets[gi - 1] : 0u) + (size_t)(blockIdx.y - rc.y) * (rc.z - rc.x) + (blockIdx.x - rc.x);
+        float2* dst = reinterpret_cast<float2*>(records + slot * kRecord);
+#pragma unroll
+        for (int k = 0; k < kRecord / 2; ++k) dst[k] = make_float2(rec[2 * k], rec[2 * k + 1]);
+      }
     }
   }
 }
@@ -311,10 +349,32 @@ extern "C" int a3d_raster_forward(const a3d_raster_args* a, float* color, float*
   return A3D_OK;
 }
 
-extern "C" int a3d_raster_backward(const a3d_raster_args* a, const float* dL_dcolor, const float* dL_ddepth, const float* dL_dalpha,
-                                   const float* alpha, const int32_t* radii, void* workspace, size_t workspace_bytes,
-                                   int64_t max_rendered, float* dL_dmeans3D, float* dL_dscales, float* dL_drotations,
-                                   float* dL_dopacity, float* dL_dcolors, float* dL_dshs, float* dL_dmeans2D, void* stream) {
+// deterministic backward scratch: one record per pair slot, then the per-(camera, gaussian) opacity partials
+static size_t carve_det(void* base, const a3d_raster_args* a, long long cap, float** records, float** op_part) {
+  size_t off = 0;
+  auto take = [&](size_t bytes) {
+    off = (off + 255) & ~(size_t)255;
+    float* p = base ? reinterpret_cast<float*>(static_cast<char*>(base) + off) : nullptr;
+    off += bytes;
+    return p;
+  };
+  float* r = take((size_t)cap * kRecord * sizeof(float));
+  float* o = take((size_t)a->num_cams * a->P * sizeof(float));
+  if (records) *records = r;
+  if (op_part) *op_part = o;
+  return (off + 255) & ~(size_t)255;
+}
+
+extern "C" size_t a3d_raster_backward_scratch_bytes(const a3d_raster_args* a, int64_t max_rendered) {
+  if (!a || !a->deterministic || check_args(a, max_rendered)) return 0;
+  return carve_det(nullptr, a, max_rendered, nullptr, nullptr);
+}
+
+extern "C" int a3d_raster_backward_ex(const a3d_raster_args* a, const float* dL_dcolor, const float* dL_ddepth, const float* dL_dalpha,
+                                      const float* alpha, const int32_t* radii, void* workspace, size_t workspace_bytes,
+                                      int64_t max_rendered, float* dL_dmeans3D, float* dL_dscales, float* dL_drotations,
+                                      float* dL_dopacity, float* dL_dcolors, float* dL_dshs, float* dL_dmeans2D, void* scratch,
+                                      size_t scratch_bytes, void* stream) {
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   (void)alpha;
   if (int r = check_args(a, max_rendered)) return r;
@@ -325,6 +385,11 @@ extern "C" int a3d_raster_backward(const a3d_raster_args* a, const float* dL_dco
   RasterWs ws;
   const size_t need = carve_workspace(workspace, a->P, a->H, a->W, a->num_cams, max_rendered, cub, &ws);
   if (need > workspace_bytes) return fail(A3D_EINVAL, "a3d_raster_backward: workspace %zu < %zu bytes", workspace_bytes, need);
+  float *records = nullptr, *op_part = nullptr;
+  if (a->deterministic) {
+    const size_t det = carve_det(scratch, a, max_rendered, &records, &op_part);
+    if (!scratch || det > scratch_bytes) return fail(A3D_EINVAL, "a3d_raster_backward: deterministic scratch %zu < %zu bytes", scratch_bytes, det);
+  }
   const RasterDev d = make_dev(a);
   const size_t n = (size_t)a->num_cams * a->P;
   A3D_CUDA_CHECK(cudaMemsetAsync(ws.g_mean2d, 0, n * 8, st));
@@ -333,14 +398,38 @@ extern "C" int a3d_raster_backward(const a3d_raster_args* a, const float* dL_dco
   A3D_CUDA_CHECK(cudaMemsetAsync(ws.g_rgb, 0, n * 12, st));
   dim3 grid(gx, gy, a->num_cams), block(kTile, kTile);
   stamp(6, st);
-  raster_render_backward_kernel<<<grid, block, 0, st>>>(d, ws, dL_dcolor, dL_ddepth, dL_dalpha, dL_dopacity);
+  if (a->deterministic) {
+    static bool attr = false;
+    if (!attr) {
+      A3D_CUDA_CHECK(cudaFuncSetAttribute(raster_render_backward_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kDetSmem));
+      attr = true;
+    }
+    raster_render_backward_kernel<true><<<grid, block, kDetSmem, st>>>(d, ws, dL_dcolor, dL_ddepth, dL_dalpha, nullptr, records);
+  } else {
+    raster_render_backward_kernel<false><<<grid, block, 0, st>>>(d, ws, dL_dcolor, dL_ddepth, dL_dalpha, dL_dopacity, nullptr);
+  }
   A3D_LAUNCH_CHECK();
   stamp(7, st);
-  launch_preprocess_backward(d, ws, radii, dL_dmeans3D, dL_dscales, dL_drotations, dL_dcolors, dL_dshs, dL_dmeans2D, st);
+  if (a->deterministic) {
+    launch_gather_records(d, ws, records, op_part, st);
+    launch_preprocess_backward_det(d, ws, radii, op_part, dL_dmeans3D, dL_dscales, dL_drotations, dL_dopacity, dL_dcolors, dL_dshs,
+                                   dL_dmeans2D, st);
+  } else {
+    launch_preprocess_backward(d, ws, radii, dL_dmeans3D, dL_dscales, dL_drotations, dL_dcolors, dL_dshs, dL_dmeans2D, st);
+  }
   A3D_LAUNCH_CHECK();
   stamp(8, st);
   g_bwd_rec = g_timing;
   return A3D_OK;
+}
+
+extern "C" int a3d_raster_backward(const a3d_raster_args* a, const float* dL_dcolor, const float* dL_ddepth, const float* dL_dalpha,
+                                   const float* alpha, const int32_t* radii, void* workspace, size_t workspace_bytes,
+                                   int64_t max_rendered, float* dL_dmeans3D, float* dL_dscales, float* dL_drotations,
+                                   float* dL_dopacity, float* dL_dcolors, float* dL_dshs, float* dL_dmeans2D, void* stream) {
+  if (a && a->deterministic) return fail(A3D_EINVAL, "a3d_raster_backward: deterministic = 1 needs a3d_raster_backward_ex's scratch");
+  return a3d_raster_backward_ex(a, dL_dcolor, dL_ddepth, dL_dalpha, alpha, radii, workspace, workspace_bytes, max_rendered, dL_dmeans3D,
+                                dL_dscales, dL_drotations, dL_dopacity, dL_dcolors, dL_dshs, dL_dmeans2D, nullptr, 0, stream);
 }
 
 extern "C" int a3d_raster_binning_tap(const void* workspace, int P, int H, int W, int num_cams, int64_t max_rendered, int cam,

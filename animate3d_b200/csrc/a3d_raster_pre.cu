@@ -154,6 +154,108 @@ __global__ void raster_preprocess_backward_kernel(RasterDev a, RasterWs ws, cons
   }
 }
 
+// deterministic backward, stage 1: every (camera, gaussian) sums the records of its pair slots in slot (= tile) order
+__global__ void raster_gather_records_kernel(RasterDev a, RasterWs ws, const float* __restrict__ records, float* __restrict__ op_part) {
+  const int idx = blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= a.num_cams * a.P) return;
+  float acc[10];
+#pragma unroll
+  for (int k = 0; k < 10; ++k) acc[k] = 0.f;
+  if (ws.tiles[idx] != 0) {
+    const size_t lo = idx ? ws.offsets[idx - 1] : 0u, hi = ws.offsets[idx];
+    for (size_t slot = lo; slot < hi; ++slot) {
+      const float2* r = reinterpret_cast<const float2*>(records + slot * 10);
+#pragma unroll
+      for (int k = 0; k < 5; ++k) {
+        const float2 v = r[k];
+        acc[2 * k] += v.x; acc[2 * k + 1] += v.y;
+      }
+    }
+  }
+  ws.g_mean2d[2 * (size_t)idx] = acc[0]; ws.g_mean2d[2 * (size_t)idx + 1] = acc[1];
+  for (int k = 0; k < 3; ++k) ws.g_conic[3 * (size_t)idx + k] = acc[2 + k];
+  op_part[idx] = acc[5];
+  for (int k = 0; k < 3; ++k) ws.g_rgb[3 * (size_t)idx + k] = acc[6 + k];
+  ws.g_depth[idx] = acc[9];
+}
+
+// deterministic backward, stage 2: one thread per gaussian walks the cameras in order (same per-camera arithmetic as
+// raster_preprocess_backward_kernel) and adds each shared gradient once
+__global__ void raster_preprocess_backward_det_kernel(RasterDev a, RasterWs ws, const int32_t* __restrict__ radii,
+                                                      const float* __restrict__ op_part, float* __restrict__ dmeans3D,
+                                                      float* __restrict__ dscales, float* __restrict__ drots,
+                                                      float* __restrict__ dopacity, float* __restrict__ dcolors,
+                                                      float* __restrict__ dshs, float* __restrict__ dmeans2D) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= a.P) return;
+  float am[3] = {0.f, 0.f, 0.f}, as[3] = {0.f, 0.f, 0.f}, ar[4] = {0.f, 0.f, 0.f, 0.f}, acol[3] = {0.f, 0.f, 0.f}, aop = 0.f;
+  float ash[16][3];
+#pragma unroll
+  for (int k = 0; k < 16; ++k) ash[k][0] = ash[k][1] = ash[k][2] = 0.f;
+  const int nb = a.colors_precomp ? 0 : (a.sh_degree + 1) * (a.sh_degree + 1);
+  for (int cam = 0; cam < a.num_cams; ++cam) {
+    const size_t idx = (size_t)cam * a.P + i;
+    aop += op_part[idx];
+    if (radii[idx] <= 0) continue;
+    const int g = a.per_cam_geometry ? cam : 0;
+    const size_t gi = (size_t)g * a.P + i;
+    const a3d_raster_cam& c = a.cams[cam];
+    const float gpx = ws.g_mean2d[2 * idx], gpy = ws.g_mean2d[2 * idx + 1];
+    float dm[3], ds[3], dr[4];
+    preprocess_backward(a.means3D + 3 * gi, a.scales + 3 * gi, a.rotations + 4 * gi, a.scale_modifier, c.viewmatrix, c.projmatrix,
+                        c.tanfovx, c.tanfovy, a.H, a.W, ws.g_conic[3 * idx], ws.g_conic[3 * idx + 1], ws.g_conic[3 * idx + 2], gpx, gpy,
+                        ws.g_depth[idx], dm, ds, dr);
+    if (a.per_cam_geometry) {   // one camera per gradient entry: written directly
+      for (int k = 0; k < 3; ++k) {
+        if (dmeans3D) dmeans3D[3 * gi + k] += dm[k];
+        if (dscales) dscales[3 * gi + k] += ds[k];
+      }
+      if (drots) for (int k = 0; k < 4; ++k) drots[4 * gi + k] += dr[k];
+    } else {
+      for (int k = 0; k < 3; ++k) { am[k] += dm[k]; as[k] += ds[k]; }
+      for (int k = 0; k < 4; ++k) ar[k] += dr[k];
+    }
+    if (dmeans2D) {
+      dmeans2D[3 * idx] = gpx * 0.5f * (float)a.W;
+      dmeans2D[3 * idx + 1] = gpy * 0.5f * (float)a.H;
+      dmeans2D[3 * idx + 2] = 0.f;
+    }
+    const float* grgb = ws.g_rgb + 3 * idx;
+    if (a.colors_precomp) {
+      for (int ch = 0; ch < 3; ++ch) acol[ch] += grgb[ch];
+    } else if (dshs) {
+      float dx = a.means3D[3 * gi] - c.campos[0], dy = a.means3D[3 * gi + 1] - c.campos[1], dz = a.means3D[3 * gi + 2] - c.campos[2];
+      const float n = sqrtf(dx * dx + dy * dy + dz * dz);
+      dx /= n; dy /= n; dz /= n;
+      float b[16];
+      sh_basis(a.sh_degree, dx, dy, dz, b);
+      const uint32_t cl = ws.clamped[idx];
+#pragma unroll
+      for (int k = 0; k < 16; ++k)
+        if (k < nb)
+#pragma unroll
+          for (int ch = 0; ch < 3; ++ch)
+            if (!(cl & (1u << ch))) ash[k][ch] += b[k] * grgb[ch];
+    }
+  }
+  if (dopacity) dopacity[i] += aop;
+  if (!a.per_cam_geometry) {
+    for (int k = 0; k < 3; ++k) {
+      if (dmeans3D) dmeans3D[3 * i + k] += am[k];
+      if (dscales) dscales[3 * i + k] += as[k];
+    }
+    if (drots) for (int k = 0; k < 4; ++k) drots[4 * i + k] += ar[k];
+  }
+  if (a.colors_precomp) {
+    if (dcolors) for (int ch = 0; ch < 3; ++ch) dcolors[3 * i + ch] += acol[ch];
+  } else if (dshs) {
+#pragma unroll
+    for (int k = 0; k < 16; ++k)
+      if (k < nb)
+        for (int ch = 0; ch < 3; ++ch) dshs[((size_t)i * a.sh_coeffs + k) * 3 + ch] += ash[k][ch];
+  }
+}
+
 void launch_preprocess(const RasterDev& a, const RasterWs& ws, int32_t* radii, cudaStream_t st) {
   const int n = a.num_cams * a.P;
   raster_preprocess_kernel<<<(n + 255) / 256, 256, 0, st>>>(a, ws, radii);
@@ -172,6 +274,17 @@ void launch_preprocess_backward(const RasterDev& a, const RasterWs& ws, const in
                                 float* drots, float* dcolors, float* dshs, float* dmeans2D, cudaStream_t st) {
   const int n = a.num_cams * a.P;
   raster_preprocess_backward_kernel<<<(n + 255) / 256, 256, 0, st>>>(a, ws, radii, dmeans3D, dscales, drots, dcolors, dshs, dmeans2D);
+}
+
+void launch_gather_records(const RasterDev& a, const RasterWs& ws, const float* records, float* op_part, cudaStream_t st) {
+  const int n = a.num_cams * a.P;
+  raster_gather_records_kernel<<<(n + 255) / 256, 256, 0, st>>>(a, ws, records, op_part);
+}
+void launch_preprocess_backward_det(const RasterDev& a, const RasterWs& ws, const int32_t* radii, const float* op_part, float* dmeans3D,
+                                    float* dscales, float* drots, float* dopacity, float* dcolors, float* dshs, float* dmeans2D,
+                                    cudaStream_t st) {
+  raster_preprocess_backward_det_kernel<<<(a.P + 127) / 128, 128, 0, st>>>(a, ws, radii, op_part, dmeans3D, dscales, drots, dopacity,
+                                                                           dcolors, dshs, dmeans2D);
 }
 
 }  // namespace a3d

@@ -85,5 +85,10 @@ void launch_duplicate(const RasterDev& a, const RasterWs& ws, int gx, int num_ti
 void launch_ranges(const RasterWs& ws, long long n, long long total_tiles, cudaStream_t st);
 void launch_preprocess_backward(const RasterDev& a, const RasterWs& ws, const int32_t* radii, float* dmeans3D, float* dscales,
                                 float* drots, float* dcolors, float* dshs, float* dmeans2D, cudaStream_t st);
+// deterministic backward: records [max_rendered][10] -> ws.g_* and op_part [cams, P]; then cameras summed in camera order
+void launch_gather_records(const RasterDev& a, const RasterWs& ws, const float* records, float* op_part, cudaStream_t st);
+void launch_preprocess_backward_det(const RasterDev& a, const RasterWs& ws, const int32_t* radii, const float* op_part, float* dmeans3D,
+                                    float* dscales, float* drots, float* dopacity, float* dcolors, float* dshs, float* dmeans2D,
+                                    cudaStream_t st);
 
 }  // namespace a3d

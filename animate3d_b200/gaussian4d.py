@@ -7,7 +7,9 @@ State (same tensors the reference keeps): static `_xyz [P,3]`, `_scaling [P,3]` 
 bias-free MLPs delta_xyz / delta_rot / delta_scaling (119-147; VanillaMLP, threestudio/models/networks.py:214-251).
 The global rotation/translation branch (`use_global_trans`, 129-142, 499-511, 525-539; on in refine_frame_16.yaml:56) runs as
 (1) a3d_deform_featmean: per-frame mean k-planes feature, (2) the two 32-wide global MLPs + Euler matrix on [T, 32] in
-torch (autograd), (3) the fused deformation launch with the rotated base quaternions; see `deform_all`."""
+torch (autograd), (3) the fused deformation launch with the rotated base quaternions; see `deform_all`.
+The mean feature is always summed in a fixed order; the backward follows torch.use_deterministic_algorithms (fixed-order
+reductions and a plane-gradient gather instead of float atomics, with 768 B of scratch per (frame, gaussian))."""
 from __future__ import annotations
 
 import ctypes as C
@@ -26,7 +28,7 @@ class DeformArgs(C.Structure):
                 ("planes", C.c_void_p * 12), ("plane_h", C.c_int * 12), ("plane_w", C.c_int * 12),
                 ("w1", C.c_void_p * 3), ("w2", C.c_void_p * 3), ("deform_scale", C.c_int),
                 ("grad_planes", C.c_void_p * 12), ("grad_w1", C.c_void_p * 3), ("grad_w2", C.c_void_p * 3),
-                ("rot_base", C.c_void_p), ("grad_rot_base", C.c_void_p), ("grad_featmean", C.c_void_p)]
+                ("rot_base", C.c_void_p), ("grad_rot_base", C.c_void_p), ("grad_featmean", C.c_void_p), ("deterministic", C.c_int)]
 
 
 def _args(xyz, scaling, rotation, times, planes, w1s, w2s, deform_scale, gplanes=None, gw1=None, gw2=None):
@@ -58,6 +60,15 @@ def _plane_grad_out(scratch: torch.Tensor, plane: torch.Tensor) -> torch.Tensor:
     return scratch.permute(2, 0, 1).reshape(plane.shape).contiguous()
 
 
+def _backward(lib, a, g_means, g_scales, g_rots, device):
+    """a3d_deform_backward_ex; with torch's deterministic flag set, the fixed-order path and its scratch."""
+    a.deterministic = L.deterministic()
+    nbytes = lib.a3d_deform_backward_scratch_bytes(C.byref(a))
+    scratch = L.scratch(nbytes, device)
+    L.check(lib.a3d_deform_backward_ex(C.byref(a), C.c_void_p(L.ptr(g_means)), C.c_void_p(L.ptr(g_scales)), C.c_void_p(L.ptr(g_rots)),
+                                       C.c_void_p(L.ptr(scratch)), C.c_size_t(nbytes), L.stream_ptr()))
+
+
 class _FeatMean(torch.autograd.Function):
     """hidden_feats.mean(0) of every frame: [T, 32]; backward folds d/d mean into the plane gradients."""
 
@@ -87,7 +98,7 @@ class _FeatMean(torch.autograd.Function):
         g_mean = g_mean.contiguous().float()
         a = _args(xyz, scaling, rotation, times, planes, w1s, w2s, True, gp, g1, g2)
         a.grad_featmean = g_mean.data_ptr()
-        L.check(lib.a3d_deform_backward(C.byref(a), None, None, None, L.stream_ptr()))
+        _backward(lib, a, None, None, None, xyz.device)
         return (None, None, None, None, None, *[_plane_grad_out(g, p) for g, p in zip(gp, planes)], None, None, None, None, None, None)
 
 
@@ -133,8 +144,7 @@ class _Deform(torch.autograd.Function):
             a.rot_base = ctx.rot_base.data_ptr()
             g_rb = torch.zeros_like(ctx.rot_base)
             a.grad_rot_base = g_rb.data_ptr()
-        L.check(lib.a3d_deform_backward(C.byref(a), C.c_void_p(L.ptr(g_means)), C.c_void_p(L.ptr(g_scales)),
-                                        C.c_void_p(L.ptr(g_rots)), L.stream_ptr()))
+        _backward(lib, a, g_means, g_scales, g_rots, xyz.device)
         return (None, None, None, None, None, None, g_rb, *[_plane_grad_out(g, p) for g, p in zip(gp, planes)], *g1, *g2)
 
 

@@ -60,6 +60,20 @@ class PrecomputedPromptUtils:
         return torch.cat([t, u], dim=0)
 
 
+def _resize_bilinear(x: torch.Tensor, size) -> torch.Tensor:
+    """F.interpolate(x, size, mode="bilinear", align_corners=False) on the SDS gradient path.  PyTorch's CUDA backward of that
+    resize scatters with atomics and raises under torch.use_deterministic_algorithms(True); there the same interpolation
+    weights (read off F.interpolate applied to identity matrices) are applied as two matmuls, whose backward is deterministic."""
+    if not (torch.are_deterministic_algorithms_enabled() and x.requires_grad):
+        return F.interpolate(x, size, mode="bilinear", align_corners=False)
+    h, w = x.shape[-2:]
+    with torch.no_grad():
+        eye = lambda n: torch.eye(n, device=x.device, dtype=x.dtype)[None, None]
+        wy = F.interpolate(eye(h), (size[0], h), mode="bilinear", align_corners=False)[0, 0]     # [Ho, h]
+        wx = F.interpolate(eye(w), (size[1], w), mode="bilinear", align_corners=False)[0, 0]     # [Wo, w]
+    return wy @ x @ wx.t()
+
+
 @register("animatemv-diffusion-guidance")
 class AnimateMVDiffusionGuidance(BaseObject):
     @dataclass
@@ -224,9 +238,9 @@ class AnimateMVDiffusionGuidance(BaseObject):
         batch_size = rgb.shape[0] // (cfg.n_view * cfg.n_frame)
         rgb_bchw = rgb.permute(0, 3, 1, 2)
         if rgb_as_latents:
-            latents = F.interpolate(rgb_bchw, (32, 32), mode="bilinear", align_corners=False)
+            latents = _resize_bilinear(rgb_bchw, (32, 32))
         else:
-            latents = self.encode_images(F.interpolate(rgb_bchw, (256, 256), mode="bilinear", align_corners=False))
+            latents = self.encode_images(_resize_bilinear(rgb_bchw, (256, 256)))
         image_embeds = kwargs.get("image_embeds")
         if image_embeds is None:
             if self.ip_image_processor is None:

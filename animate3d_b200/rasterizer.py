@@ -8,7 +8,8 @@ custom/threestudio-animate3d/renderer/diff_gaussian_rasterizer_advanced_4d.py:8-
 
 plus `rasterize_batch`, which renders ALL cameras of a batch (the reference's Python loop over cameras,
 gaussian_batch_renderer_4d.py:27) through one launch per stage.  Forward and backward run in liba3d.so; torch provides
-memory, the stream and the autograd tape."""
+memory, the stream and the autograd tape.  Under torch.use_deterministic_algorithms(True) the backward sums every gradient
+in a fixed order (bit-reproducible), at the cost of 40 B of scratch per (tile, gaussian) pair."""
 from __future__ import annotations
 
 import ctypes as C
@@ -36,6 +37,7 @@ class GaussianRasterizationSettings(NamedTuple):
 
 _cap_hint = {}
 last_num_rendered = 0      # (tile, gaussian) pairs of the most recent forward (diagnostics / bench roofline)
+last_backward_scratch_bytes = 0   # deterministic-backward scratch of the most recent backward (0 with the flag off)
 
 
 def _pack_cams(settings: Sequence[GaussianRasterizationSettings], device) -> torch.Tensor:
@@ -120,11 +122,17 @@ class _RasterizeBatch(torch.autograd.Function):
         dm2 = torch.zeros(ncam, P, 3, device=dev)
         args = _make_args(P, H, W, cams_t, means3D, scales, rotations, opacities, shs, colors_precomp, sh_degree, per_cam,
                           scale_modifier, bg)
-        L.check(lib.a3d_raster_backward(C.byref(args), C.c_void_p(g_color.data_ptr()), C.c_void_p(L.ptr(g_depth)),
-                                        C.c_void_p(L.ptr(g_alpha)), C.c_void_p(alpha.data_ptr()), C.c_void_p(radii.data_ptr()),
-                                        C.c_void_p(ws.data_ptr()), C.c_size_t(nbytes), C.c_int64(cap), C.c_void_p(dm.data_ptr()),
-                                        C.c_void_p(ds.data_ptr()), C.c_void_p(dr.data_ptr()), C.c_void_p(do.data_ptr()),
-                                        C.c_void_p(L.ptr(dc)), C.c_void_p(L.ptr(dsh)), C.c_void_p(dm2.data_ptr()), L.stream_ptr()))
+        args.deterministic = L.deterministic()
+        sbytes = lib.a3d_raster_backward_scratch_bytes(C.byref(args), C.c_int64(cap))
+        scratch = L.scratch(sbytes, dev)
+        global last_backward_scratch_bytes
+        last_backward_scratch_bytes = sbytes
+        L.check(lib.a3d_raster_backward_ex(C.byref(args), C.c_void_p(g_color.data_ptr()), C.c_void_p(L.ptr(g_depth)),
+                                           C.c_void_p(L.ptr(g_alpha)), C.c_void_p(alpha.data_ptr()), C.c_void_p(radii.data_ptr()),
+                                           C.c_void_p(ws.data_ptr()), C.c_size_t(nbytes), C.c_int64(cap), C.c_void_p(dm.data_ptr()),
+                                           C.c_void_p(ds.data_ptr()), C.c_void_p(dr.data_ptr()), C.c_void_p(do.data_ptr()),
+                                           C.c_void_p(L.ptr(dc)), C.c_void_p(L.ptr(dsh)), C.c_void_p(dm2.data_ptr()),
+                                           C.c_void_p(L.ptr(scratch)), C.c_size_t(sbytes), L.stream_ptr()))
         g_m2 = None if ctx.m2_shape is None else dm2.reshape(ctx.m2_shape)   # `viewspace_points` gradient, NDC units
         return dm, g_m2, ds, dr, do, dsh, dc, None, None
 

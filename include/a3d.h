@@ -199,6 +199,8 @@ typedef struct a3d_raster_args {
   int per_cam_geometry;      /* 1: means/scales/rotations have a leading camera dim */
   float scale_modifier;
   float bg[3];
+  int deterministic;         /* 1: the backward sums every gradient in a fixed order (bit-reproducible; needs the scratch of
+                                a3d_raster_backward_ex); 0: float atomics.  The forward is deterministic either way. */
 } a3d_raster_args;
 
 /* workspace bytes for a forward with at most max_rendered (tile,gaussian) pairs per camera */
@@ -215,6 +217,21 @@ int a3d_raster_backward(const a3d_raster_args* args, const float* dL_dcolor, con
                         size_t workspace_bytes, int64_t max_rendered, float* dL_dmeans3D, float* dL_dscales,
                         float* dL_drotations, float* dL_dopacity, float* dL_dcolors, float* dL_dshs,
                         float* dL_dmeans2D, void* stream);
+/* Scratch bytes a3d_raster_backward_ex needs: 0 when args->deterministic is 0, else 40 B per (tile, gaussian) pair slot of
+ * max_rendered plus 4 B per (camera, gaussian). */
+size_t a3d_raster_backward_scratch_bytes(const a3d_raster_args* args, int64_t max_rendered);
+/* a3d_raster_backward with caller-owned scratch (scratch may be NULL when the size query returned 0).  With
+ * args->deterministic set (torch.use_deterministic_algorithms of the caller), the render backward reduces the 8 warp
+ * partials of a list entry in warp order and stores one 10-float record per (camera, tile, gaussian) pair in the pair's
+ * pre-sort slot; a per-(camera, gaussian) kernel sums its slots in slot (= tile) order, and a per-gaussian kernel pushes
+ * every camera's gradients through the projection, summing cameras in camera order.  Same reference interface as
+ * a3d_raster_backward (rasterize_gaussians_backward, which accumulates with float atomics).  a3d_raster_backward itself
+ * rejects deterministic = 1. */
+int a3d_raster_backward_ex(const a3d_raster_args* args, const float* dL_dcolor, const float* dL_ddepth,
+                           const float* dL_dalpha, const float* alpha, const int32_t* radii, void* workspace,
+                           size_t workspace_bytes, int64_t max_rendered, float* dL_dmeans3D, float* dL_dscales,
+                           float* dL_drotations, float* dL_dopacity, float* dL_dcolors, float* dL_dshs,
+                           float* dL_dmeans2D, void* scratch, size_t scratch_bytes, void* stream);
 /* debug/parity taps of the binning stage for one camera: sorted keys [n] uint64, point_list [n] uint32, ranges [tiles] uint2 */
 int a3d_raster_binning_tap(const void* workspace, int P, int H, int W, int num_cams, int64_t max_rendered, int cam,
                            uint64_t* keys_out, uint32_t* point_list_out, uint32_t* ranges_out, void* stream);
@@ -248,17 +265,30 @@ typedef struct a3d_deform_args {
   const float* rot_base;      /* [T,P,4] per-frame base quaternions, replace `rotation` (forward and backward) */
   float* grad_rot_base;       /* backward: receives dL/d rot_base, [T,P,4] */
   const float* grad_featmean; /* backward: dL/d (per-frame mean feature), [T, num_scales*channels]; folded into grad_planes */
+  int deterministic;          /* backward: 1 = fixed summation order (needs the scratch of a3d_deform_backward_ex), 0 = atomics */
 } a3d_deform_args;
 
 int a3d_deform_forward(const a3d_deform_args* args, float* means, float* scales, float* rotations, void* stream);
 /* per-frame mean over the P gaussians of the k-planes feature vector (`hidden_feats.mean(0)`, gaussian_4d.py:501, 527):
- * featmean [T, num_scales*channels] */
+ * featmean [T, num_scales*channels].  Always summed in a fixed order (a cluster of 8 CTAs per frame, reduced through
+ * distributed shared memory in rank order), so it is bit-reproducible and needs no scratch. */
 int a3d_deform_featmean(const a3d_deform_args* args, float* featmean, void* stream);
 /* Accumulates into args->grad_w1 / grad_w2 ([out, in] like the weights) and args->grad_planes.  grad_planes[i] is a
  * CHANNEL-LAST scratch [plane_h[i], plane_w[i], channels] (zero it first; 16-byte aligned): the 16 channels of a texel are
  * written with vector reductions; transpose it into the [1, channels, H, W] parameter gradient afterwards. */
 int a3d_deform_backward(const a3d_deform_args* args, const float* dL_dmeans, const float* dL_dscales, const float* dL_drotations,
                         void* stream);
+/* Scratch bytes a3d_deform_backward_ex needs: 0 when args->deterministic is 0.  Otherwise 768 B per (frame, gaussian) for
+ * the stored upstream plane factors (0.61 GB at T = 16, P = 50 000), 16 B per (frame, gaussian) of sort buffers and the
+ * per-CTA weight-gradient partials. */
+size_t a3d_deform_backward_scratch_bytes(const a3d_deform_args* args);
+/* a3d_deform_backward with caller-owned scratch (NULL when the size query returned 0); same reference interface (the autograd
+ * backward of gaussian_4d.py:450-548, whose grid_sample backward scatters with float atomics).  With args->deterministic set:
+ * MLP weight gradients are per-CTA partials reduced in CTA order; plane gradients are a gather: per plane, the (frame,
+ * gaussian) points are stably radix-sorted by their lower-left cell, and every texel sums the stored factors (d loss / d
+ * feature x the other planes' samples, grad_featmean folded in) of the points of its <= 4 adjacent cells in sorted order. */
+int a3d_deform_backward_ex(const a3d_deform_args* args, const float* dL_dmeans, const float* dL_dscales,
+                           const float* dL_drotations, void* scratch, size_t scratch_bytes, void* stream);
 
 /* ---------------------------------------------------------------- ARAP regulariser (SURVEY 8f-3) -------------- */
 /* K nearest neighbours of every point among the same points, self excluded, squared distances ascending, ties by index:
@@ -273,6 +303,14 @@ int a3d_knn_graph(const float* points, int n, int K, int32_t* nbr, float* dist2,
  * zeroed here.  Checked on the CPU (tests/test_arap_cpu.py) and on the GPU against the reference goldens (tests/test_arap_gpu.py). */
 int a3d_arap(const float* nodes, int Nt, int Nv, const int32_t* nbr, int K, const float* weight, const int32_t* sample, int Ns,
              float* err, float* grad, void* stream);
+/* Scratch bytes of a3d_arap_deterministic for the same sizes (Ns of a NULL sample = Nv). */
+size_t a3d_arap_deterministic_scratch_bytes(int Nt, int Nv, int K, int Ns);
+/* a3d_arap (cal_arap_error, util.py:183-215) with every sum in a fixed order: the energy from per-(frame, sample) partials
+ * reduced by one CTA; the gradient from per-(frame, sample, edge) 3-vector records gathered per node after a stable sort of
+ * the (target node, record) pairs, so repeated samples add in sample order and the frame-0 gradient adds frames in order. */
+int a3d_arap_deterministic(const float* nodes, int Nt, int Nv, const int32_t* nbr, int K, const float* weight,
+                           const int32_t* sample, int Ns, float* err, float* grad, void* scratch, size_t scratch_bytes,
+                           void* stream);
 
 /* debug hook: a device uint64 counter the tensor-core attention kernel bumps once per (warp, key step) that takes the
    lazy-rescale branch of the single-pass softmax (NULL = off; tests use it to prove adversarial inputs reach that branch). */
