@@ -81,8 +81,8 @@ def load(require_gpu: bool = True) -> C.CDLL:
         lib.a3d_raster_backward_scratch_bytes.argtypes = [C.c_void_p, C.c_int64]
         lib.a3d_deform_backward_scratch_bytes.restype = C.c_size_t
         lib.a3d_deform_backward_scratch_bytes.argtypes = [C.c_void_p]
-        lib.a3d_arap_deterministic_scratch_bytes.restype = C.c_size_t
-        lib.a3d_arap_deterministic_scratch_bytes.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int]
+        lib.a3d_arap_scratch_bytes.restype = C.c_size_t
+        lib.a3d_arap_scratch_bytes.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]
         _lib = lib
     if require_gpu and not _inited:
         if not torch.cuda.is_available():
@@ -111,5 +111,5 @@ def deterministic() -> int:
 
 
 def scratch(nbytes: int, device) -> Optional[torch.Tensor]:
-    """Caller-owned device scratch for the deterministic entry points (None when a size query returned 0)."""
+    """Caller-owned device scratch of the 4D-path entry points (None when a size query returned 0)."""
     return torch.empty(nbytes, dtype=torch.uint8, device=device) if nbytes else None

@@ -7,10 +7,7 @@ called from systems/animate3d.py:215-244), on the CUDA path of liba3d.so:
 `cal_connectivity_from_points` supports the mode every shipped config uses ('nn', adaptive weighting); the KNN graph comes
 from `a3d_knn_graph`.  `cal_arap_error` runs the fused rotation-fit + energy + gradient kernel (`a3d_arap`) for all frames
 at once and is differentiable w.r.t. the node positions (the rotation itself carries no gradient, as in the reference).
-Under torch.use_deterministic_algorithms(True) it runs `a3d_arap_deterministic`, which sums energy and gradient in a fixed order.
-
-STATUS (round 1): the shared arithmetic is validated on the CPU against the reference's functions
-(tests/test_arap_cpu.py); the CUDA wrapper has not been run on hardware yet."""
+Under torch.use_deterministic_algorithms(True) it sums energy and gradient in a fixed order."""
 from __future__ import annotations
 
 import ctypes as C
@@ -66,14 +63,12 @@ class _Arap(torch.autograd.Function):
         err = torch.empty(1, device=x.device)
         grad = torch.empty_like(x)
         k, ns = nbr.shape[1], nv if sample is None else sample.numel()
-        common = (C.c_void_p(x.data_ptr()), nt, nv, C.c_void_p(nbr.data_ptr()), k, C.c_void_p(L.ptr(weight)), C.c_void_p(L.ptr(sample)),
-                  ns, C.c_void_p(err.data_ptr()), C.c_void_p(grad.data_ptr()))
-        if L.deterministic():
-            nbytes = lib.a3d_arap_deterministic_scratch_bytes(nt, nv, k, ns)
-            scratch = L.scratch(nbytes, x.device)
-            L.check(lib.a3d_arap_deterministic(*common, C.c_void_p(L.ptr(scratch)), C.c_size_t(nbytes), L.stream_ptr()))
-        else:
-            L.check(lib.a3d_arap(*common, L.stream_ptr()))
+        det = L.deterministic()
+        nbytes = lib.a3d_arap_scratch_bytes(nt, nv, k, ns, det)
+        scratch = L.scratch(nbytes, x.device)
+        L.check(lib.a3d_arap(C.c_void_p(x.data_ptr()), nt, nv, C.c_void_p(nbr.data_ptr()), k, C.c_void_p(L.ptr(weight)),
+                             C.c_void_p(L.ptr(sample)), ns, det, C.c_void_p(err.data_ptr()), C.c_void_p(grad.data_ptr()),
+                             C.c_void_p(L.ptr(scratch)), C.c_size_t(nbytes), L.stream_ptr()))
         ctx.save_for_backward(grad)
         return err[0]
 

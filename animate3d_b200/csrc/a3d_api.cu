@@ -70,7 +70,7 @@ extern "C" {
 
 const char* a3d_last_error(void) { return a3d::g_err; }
 
-int a3d_version(void) { return 100; }
+int a3d_version(void) { return 101; }
 
 int a3d_init(void) {
   int dev = 0;

@@ -2,8 +2,7 @@
 // 138-215, called from systems/animate3d.py:215-244): brute-force KNN graph of the control nodes (built once -- the
 // gaussians' rest positions are frozen) and one fused kernel for all frames that fits the per-node rotation, evaluates the
 // edge energy and scatters its gradient.  The arithmetic lives in a3d_arap_math.h (shared with the CPU harness that checks
-// it against the reference's own functions).  STATUS: the math is validated on the CPU; this wrapper has not run on
-// hardware yet (round-1 GPU budget exhausted) -- tests/test_arap_gpu.py runs it in a subprocess.
+// it against the reference's own functions).
 #include "a3d_host.cuh"
 #include "a3d_arap_math.h"
 #include "a3d_segsort.cuh"
@@ -57,28 +56,14 @@ __global__ void __launch_bounds__(128) arap_kernel(const float* __restrict__ nod
     if (i >= 0 && i < Nv) {
       float e0[kArapMaxK][3], et[kArapMaxK][3], g0[kArapMaxK][3], gt[kArapMaxK][3], w[kArapMaxK];
       bool valid[kArapMaxK];
-      int nb[kArapMaxK];
-      const float* p0 = nodes;
-      const float* pt = nodes + (int64_t)t * Nv * 3;
-#pragma unroll
-      for (int n = 0; n < kArapMaxK; ++n) {
-        const int j = n < K ? nbr[(int64_t)i * K + n] : -1;
-        nb[n] = j;
-        valid[n] = j >= 0 && j < Nv;
-        w[n] = (n < K) ? (weight ? weight[(int64_t)i * K + n] : (valid[n] ? 1.f : 0.f)) : 0.f;
-#pragma unroll
-        for (int c = 0; c < 3; ++c) {
-          e0[n][c] = valid[n] ? p0[3 * (int64_t)i + c] - p0[3 * (int64_t)j + c] : 0.f;
-          et[n][c] = valid[n] ? pt[3 * (int64_t)i + c] - pt[3 * (int64_t)j + c] : 0.f;
-        }
-      }
+      arap_gather(nodes, Nv, nbr, K, weight, i, t, e0, et, w, valid);
       energy = arap_node(K, e0, et, valid, w, gt, g0);
       if (grad) {
         float* gT = grad + (int64_t)t * Nv * 3;
 #pragma unroll
         for (int n = 0; n < kArapMaxK; ++n) {
           if (n < K && valid[n]) {
-            const int j = nb[n];
+            const int j = nbr[(int64_t)i * K + n];
 #pragma unroll
             for (int c = 0; c < 3; ++c) {
               atomicAdd(gT + 3 * (int64_t)i + c, gt[n][c]);
@@ -114,19 +99,7 @@ __global__ void __launch_bounds__(128) arap_records_kernel(const float* __restri
   float en = 0.f;
   const bool node_ok = i >= 0 && i < Nv;
   if (node_ok) {
-    const float* p0 = nodes;
-    const float* pt = nodes + (int64_t)t * Nv * 3;
-#pragma unroll
-    for (int n = 0; n < kArapMaxK; ++n) {
-      const int j = n < K ? nbr[(int64_t)i * K + n] : -1;
-      valid[n] = j >= 0 && j < Nv;
-      w[n] = (n < K) ? (weight ? weight[(int64_t)i * K + n] : (valid[n] ? 1.f : 0.f)) : 0.f;
-#pragma unroll
-      for (int c = 0; c < 3; ++c) {
-        e0[n][c] = valid[n] ? p0[3 * (int64_t)i + c] - p0[3 * (int64_t)j + c] : 0.f;
-        et[n][c] = valid[n] ? pt[3 * (int64_t)i + c] - pt[3 * (int64_t)j + c] : 0.f;
-      }
-    }
+    arap_gather(nodes, Nv, nbr, K, weight, i, t, e0, et, w, valid);
     en = arap_node(K, e0, et, valid, w, gt, g0);
   }
   energy[idx] = en;
@@ -228,44 +201,33 @@ extern "C" int a3d_knn_graph(const float* points, int n, int K, int32_t* nbr, fl
   return A3D_OK;
 }
 
+extern "C" size_t a3d_arap_scratch_bytes(int Nt, int Nv, int K, int Ns, int deterministic) {
+  if (!deterministic || Nt < 1 || Nv < 1 || K < 1 || Ns < 1) return 0;
+  return carve_arap(nullptr, Nt, Nv, K, Ns, nullptr);
+}
+
 extern "C" int a3d_arap(const float* nodes, int Nt, int Nv, const int32_t* nbr, int K, const float* weight, const int32_t* sample,
-                        int Ns, float* err, float* grad, void* stream) {
+                        int Ns, int deterministic, float* err, float* grad, void* scratch, size_t scratch_bytes, void* stream) {
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   if (!nodes || !nbr || !err || Nt < 1 || Nv < 1 || K < 1 || K > kArapMaxK)
     return fail(A3D_EINVAL, "a3d_arap: bad arguments (Nt=%d Nv=%d K=%d)", Nt, Nv, K);
   if (!sample) Ns = Nv;
   if (Ns < 1) return fail(A3D_EINVAL, "a3d_arap: empty node sample");
-  A3D_CUDA_CHECK(cudaMemsetAsync(err, 0, sizeof(float), st));
-  if (grad) A3D_CUDA_CHECK(cudaMemsetAsync(grad, 0, sizeof(float) * (size_t)Nt * Nv * 3, st));
-  const int64_t total = (int64_t)(Nt - 1) * Ns;
-  if (total > 0) {
-    arap_kernel<<<(unsigned)((total + 127) / 128), 128, 0, st>>>(nodes, Nt, Nv, nbr, K, weight, sample, Ns, err, grad);
-    A3D_LAUNCH_CHECK();
-  }
-  return A3D_OK;
-}
-
-extern "C" size_t a3d_arap_deterministic_scratch_bytes(int Nt, int Nv, int K, int Ns) {
-  if (Nt < 1 || Nv < 1 || K < 1 || Ns < 1) return 0;
-  return carve_arap(nullptr, Nt, Nv, K, Ns, nullptr);
-}
-
-extern "C" int a3d_arap_deterministic(const float* nodes, int Nt, int Nv, const int32_t* nbr, int K, const float* weight,
-                                      const int32_t* sample, int Ns, float* err, float* grad, void* scratch, size_t scratch_bytes,
-                                      void* stream) {
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  if (!nodes || !nbr || !err || Nt < 1 || Nv < 1 || K < 1 || K > kArapMaxK)
-    return fail(A3D_EINVAL, "a3d_arap_deterministic: bad arguments (Nt=%d Nv=%d K=%d)", Nt, Nv, K);
-  if (!sample) Ns = Nv;
-  if (Ns < 1) return fail(A3D_EINVAL, "a3d_arap_deterministic: empty node sample");
-  if ((int64_t)Ns * K * 2 > 0x7fffffffll) return fail(A3D_EINVAL, "a3d_arap_deterministic: too many edges");
   ArapScratch s;
-  const size_t need = carve_arap(scratch, Nt, Nv, K, Ns, &s);
-  if (!scratch || scratch_bytes < need) return fail(A3D_EINVAL, "a3d_arap_deterministic: scratch %zu < %zu bytes", scratch_bytes, need);
+  if (deterministic) {
+    if ((int64_t)Ns * K * 2 > 0x7fffffffll) return fail(A3D_EINVAL, "a3d_arap: too many edges for the deterministic path");
+    const size_t need = carve_arap(scratch, Nt, Nv, K, Ns, &s);
+    if (!scratch || scratch_bytes < need) return fail(A3D_EINVAL, "a3d_arap: deterministic scratch %zu < %zu bytes", scratch_bytes, need);
+  }
   const int64_t total = (int64_t)(Nt - 1) * Ns;
-  if (total == 0) {
+  if (!deterministic || total == 0) {   // the atomic kernel accumulates into err / grad; the fixed-order kernels overwrite them
     A3D_CUDA_CHECK(cudaMemsetAsync(err, 0, sizeof(float), st));
     if (grad) A3D_CUDA_CHECK(cudaMemsetAsync(grad, 0, sizeof(float) * (size_t)Nt * Nv * 3, st));
+  }
+  if (total == 0) return A3D_OK;
+  if (!deterministic) {
+    arap_kernel<<<(unsigned)((total + 127) / 128), 128, 0, st>>>(nodes, Nt, Nv, nbr, K, weight, sample, Ns, err, grad);
+    A3D_LAUNCH_CHECK();
     return A3D_OK;
   }
   arap_records_kernel<<<(unsigned)((total + 127) / 128), 128, 0, st>>>(nodes, Nt, Nv, nbr, K, weight, sample, Ns, s.energy, s.rec_t,

@@ -9,6 +9,7 @@
 // Jacobi eigen-solver (fixed 8 sweeps, no data-dependent branches besides the rotation guard).
 #pragma once
 #include <math.h>
+#include <stdint.h>
 
 #if defined(__CUDACC__)
 #define A3D_HD __host__ __device__ __forceinline__
@@ -78,6 +79,26 @@ A3D_HD void rotation_from_covariance(const float (&S)[3][3], float (&R)[9]) {
   R[0] = 1 - 2 * (y * y + z * z); R[1] = 2 * (x * y - w * z);     R[2] = 2 * (x * z + w * y);
   R[3] = 2 * (x * y + w * z);     R[4] = 1 - 2 * (x * x + z * z); R[5] = 2 * (y * z - w * x);
   R[6] = 2 * (x * z - w * y);     R[7] = 2 * (y * z + w * x);     R[8] = 1 - 2 * (x * x + y * y);
+}
+
+// Edges of node i at frame t (nodes [Nt,Nv,3], nbr [Nv,K]): for n < K with j = nbr[i,n] in [0, Nv) (valid[n]),
+// e0[n] = x_0[i] - x_0[j] and et[n] = x_t[i] - x_t[j]; w[n] = weight[i,n], or 1 on valid edges when weight is null (the
+// reference's call).  Absent edges and n >= K get zero edges; n >= K also zero weight.
+A3D_HD void arap_gather(const float* nodes, int Nv, const int* nbr, int K, const float* weight, int i, int t, float (*e0)[3],
+                        float (*et)[3], float* w, bool* valid) {
+  const float* p0 = nodes;
+  const float* pt = nodes + (int64_t)t * Nv * 3;
+#pragma unroll
+  for (int n = 0; n < kArapMaxK; ++n) {
+    const int j = n < K ? nbr[(int64_t)i * K + n] : -1;
+    valid[n] = j >= 0 && j < Nv;
+    w[n] = (n < K) ? (weight ? weight[(int64_t)i * K + n] : (valid[n] ? 1.f : 0.f)) : 0.f;
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+      e0[n][c] = valid[n] ? p0[3 * (int64_t)i + c] - p0[3 * (int64_t)j + c] : 0.f;
+      et[n][c] = valid[n] ? pt[3 * (int64_t)i + c] - pt[3 * (int64_t)j + c] : 0.f;
+    }
+  }
 }
 
 // One (frame, node): edges e0[n] = p0_i - p0_j(n), et[n] = pt_i - pt_j(n) for the present neighbours (valid[n]), weights w[n].

@@ -32,7 +32,11 @@ struct DeformMlp {          // row-major [out, in]
   float *gw1[3], *gw2[3];
 };
 
-__device__ __constant__ int c_comb[kPlanes][2] = {{0, 1}, {0, 2}, {0, 3}, {1, 2}, {1, 3}, {2, 3}};
+// coordinates (x, y, z, t) of each plane, the first one indexing W.  One list: kernels read c_comb, the host (which cannot
+// read __constant__ memory) kComb when it launches the per-plane gather of the fixed-order backward.
+#define A3D_PLANE_AXES {{0, 1}, {0, 2}, {0, 3}, {1, 2}, {1, 3}, {2, 3}}
+__device__ __constant__ int c_comb[kPlanes][2] = A3D_PLANE_AXES;
+constexpr int kComb[kPlanes][2] = A3D_PLANE_AXES;
 __device__ __forceinline__ int out_dim(int m) { return m == 1 ? 4 : 3; }
 
 struct Bilerp {
@@ -58,15 +62,39 @@ struct DeformGlobal {
   const float* g_featmean;    // backward: d/d (mean feature of frame t), [T, nfeat], or null
 };
 
-__global__ void __launch_bounds__(128)
-deform_kernel(DeformGrids G, DeformMlp M, DeformGlobal X, const float* __restrict__ xyz, const float* __restrict__ scaling,
-              const float* __restrict__ rotation, const float* __restrict__ times, int P, int T, int deform_scale,
-              float* __restrict__ out_means, float* __restrict__ out_scales, float* __restrict__ out_rots) {
-  extern __shared__ __align__(16) float sm[];
-  // shared copies of the MLP weights
-  float* sw1 = sm;                                   // [3][32][32]
-  float* sw2 = sw1 + 3 * kHid * kHid;                // [3][4][32] (padded to 4 outputs)
+__device__ __forceinline__ float plane_sample(const float* __restrict__ gc, const Bilerp& b, int W) {
+  return (__ldg(gc + b.y0 * W + b.x0) * (1.f - b.wx) + __ldg(gc + b.y0 * W + b.x1) * b.wx) * (1.f - b.wy) +
+         (__ldg(gc + b.y1 * W + b.x0) * (1.f - b.wx) + __ldg(gc + b.y1 * W + b.x1) * b.wx) * b.wy;
+}
+
+// (x, y, z, t) of item idx = frame t * P + gaussian i; an inactive item is (0, 0, 0, 0) with t = i = 0
+template <class Idx>
+__device__ __forceinline__ void item_point(const float* __restrict__ xyz, const float* __restrict__ times, int P, Idx idx, bool active,
+                                           float (&pt)[4], int& t, int& i) {
+  t = active ? (int)(idx / (Idx)P) : 0;
+  i = active ? (int)(idx % (Idx)P) : 0;
+  pt[0] = pt[1] = pt[2] = pt[3] = 0.f;
+  if (active) { pt[0] = xyz[3 * i]; pt[1] = xyz[3 * i + 1]; pt[2] = xyz[3 * i + 2]; pt[3] = times[t]; }
+}
+
+// k-planes feature of point pt: per scale, the product over the 6 planes of the bilinear samples of the 16 channels.
+// Channels >= nfeat are 0; an inactive item reads nothing and keeps 1 in the others.
+__device__ __forceinline__ void kplanes_feature(const DeformGrids& G, const float (&pt)[4], bool active, float (&feat)[kHid]) {
   const int nfeat = G.scales * kFeat;
+#pragma unroll
+  for (int c = 0; c < kHid; ++c) feat[c] = c < nfeat ? 1.f : 0.f;
+  if (!active) return;
+  for (int s = 0; s < G.scales; ++s)
+    for (int pl = 0; pl < kPlanes; ++pl) {
+      const int W = G.w[s][pl], H = G.h[s][pl];
+      const Bilerp b = bilerp_setup(pt[c_comb[pl][0]], pt[c_comb[pl][1]], W, H);
+#pragma unroll
+      for (int c = 0; c < kFeat; ++c) feat[s * kFeat + c] *= plane_sample(G.plane[s][pl] + (size_t)c * H * W, b, W);
+    }
+}
+
+// MLP weights into shared memory: sw1 [3][32][32] (input columns >= nfeat zeroed), sw2 [3][4][32] (padded to 4 outputs)
+__device__ __forceinline__ void stage_mlp_weights(const DeformMlp& M, int nfeat, float* sw1, float* sw2) {
   for (int i = threadIdx.x; i < 3 * kHid * kHid; i += blockDim.x) {
     const int m = i / (kHid * kHid), r = i % (kHid * kHid);
     sw1[i] = (r % kHid < nfeat) ? M.w1[m][(r / kHid) * nfeat + r % kHid] : 0.f;
@@ -75,80 +103,79 @@ deform_kernel(DeformGrids G, DeformMlp M, DeformGlobal X, const float* __restric
     const int m = i / (4 * kHid), r = (i % (4 * kHid)) / kHid, c = i % kHid;
     sw2[i] = r < out_dim(m) ? M.w2[m][r * kHid + c] : 0.f;
   }
+}
+
+// MLP m on the staged weights: hid = relu(W1 feat), out = W2 hid.  The weights are broadcast reads from shared memory:
+// 16-byte loads (4 FMAs per load) -- with scalar loads the forward sat on the shared-memory pipe (one LDS per FMA: 0.68 ms
+// for 16 frames x 50k gaussians, profiles/r02_splat_launches.txt)
+__device__ __forceinline__ void mlp_forward(const float* sw1, const float* sw2, int m, const float (&feat)[kHid], float (&hid)[kHid],
+                                            float (&out)[4]) {
+#pragma unroll
+  for (int r = 0; r < kHid; ++r) {
+    float a = 0.f;
+    const float4* wr = reinterpret_cast<const float4*>(sw1 + (m * kHid + r) * kHid);
+#pragma unroll
+    for (int c = 0; c < kHid / 4; ++c) {
+      const float4 w4 = wr[c];
+      a = fmaf(w4.x, feat[4 * c], a); a = fmaf(w4.y, feat[4 * c + 1], a);
+      a = fmaf(w4.z, feat[4 * c + 2], a); a = fmaf(w4.w, feat[4 * c + 3], a);
+    }
+    hid[r] = fmaxf(a, 0.f);
+  }
+#pragma unroll
+  for (int r = 0; r < 4; ++r) {
+    float a = 0.f;
+    const float4* wr = reinterpret_cast<const float4*>(sw2 + (m * 4 + r) * kHid);
+#pragma unroll
+    for (int c = 0; c < kHid / 4; ++c) {
+      const float4 w4 = wr[c];
+      a = fmaf(w4.x, hid[4 * c], a); a = fmaf(w4.y, hid[4 * c + 1], a);
+      a = fmaf(w4.z, hid[4 * c + 2], a); a = fmaf(w4.w, hid[4 * c + 3], a);
+    }
+    out[r] = a;
+  }
+}
+
+// y = (qb + d) / max(|qb + d|, 1e-12); returns the clamped norm
+__device__ __forceinline__ float normalized_rotation(const float* qb, const float* d, float (&y)[4]) {
+  float q[4];
+  for (int k = 0; k < 4; ++k) q[k] = qb[k] + d[k];
+  const float qn = fmaxf(sqrtf(q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3]), 1e-12f);
+  for (int k = 0; k < 4; ++k) y[k] = q[k] / qn;
+  return qn;
+}
+
+__global__ void __launch_bounds__(128)
+deform_kernel(DeformGrids G, DeformMlp M, DeformGlobal X, const float* __restrict__ xyz, const float* __restrict__ scaling,
+              const float* __restrict__ rotation, const float* __restrict__ times, int P, int T, int deform_scale,
+              float* __restrict__ out_means, float* __restrict__ out_scales, float* __restrict__ out_rots) {
+  extern __shared__ __align__(16) float sm[];
+  float* sw1 = sm;
+  float* sw2 = sw1 + 3 * kHid * kHid;
+  stage_mlp_weights(M, G.scales * kFeat, sw1, sw2);
   __syncthreads();
   const int idx = blockIdx.x * blockDim.x + threadIdx.x;
   const bool active = idx < P * T;
-  const int t = active ? idx / P : 0, i = active ? idx % P : 0;
-  float pt[4] = {0.f, 0.f, 0.f, 0.f};
-  if (active) { pt[0] = xyz[3 * i]; pt[1] = xyz[3 * i + 1]; pt[2] = xyz[3 * i + 2]; pt[3] = times[t]; }
-  // ---- features: product over planes of bilinear samples
+  int t, i;
+  float pt[4];
+  item_point(xyz, times, P, idx, active, pt, t, i);
   float feat[kHid];
-#pragma unroll
-  for (int c = 0; c < kHid; ++c) feat[c] = c < nfeat ? 1.f : 0.f;
-  if (active) {
-    for (int s = 0; s < G.scales; ++s)
-      for (int pl = 0; pl < kPlanes; ++pl) {
-        const int W = G.w[s][pl], H = G.h[s][pl];
-        const Bilerp b = bilerp_setup(pt[c_comb[pl][0]], pt[c_comb[pl][1]], W, H);
-        const float* g = G.plane[s][pl];
-#pragma unroll
-        for (int c = 0; c < kFeat; ++c) {
-          const float* gc = g + (size_t)c * H * W;
-          const float v00 = __ldg(gc + b.y0 * W + b.x0), v01 = __ldg(gc + b.y0 * W + b.x1);
-          const float v10 = __ldg(gc + b.y1 * W + b.x0), v11 = __ldg(gc + b.y1 * W + b.x1);
-          const float v = (v00 * (1.f - b.wx) + v01 * b.wx) * (1.f - b.wy) + (v10 * (1.f - b.wx) + v11 * b.wx) * b.wy;
-          feat[s * kFeat + c] *= v;
-        }
-      }
-  }
-  // ---- three MLPs
-  // the weights are broadcast reads from shared memory: 16-byte loads (4 FMAs per load) -- with scalar loads the kernel sat on
-  // the shared-memory pipe (one LDS per FMA: 0.68 ms for 16 frames x 50k gaussians, profiles/r02_splat_launches.txt)
+  kplanes_feature(G, pt, active, feat);
   float outv[3][4];
 #pragma unroll 1
   for (int m = 0; m < 3; ++m) {
     float hid[kHid];
-#pragma unroll
-    for (int r = 0; r < kHid; ++r) {
-      float a = 0.f;
-      const float4* wr = reinterpret_cast<const float4*>(sw1 + (m * kHid + r) * kHid);
-#pragma unroll
-      for (int c = 0; c < kHid / 4; ++c) {
-        const float4 w4 = wr[c];
-        a = fmaf(w4.x, feat[4 * c], a); a = fmaf(w4.y, feat[4 * c + 1], a);
-        a = fmaf(w4.z, feat[4 * c + 2], a); a = fmaf(w4.w, feat[4 * c + 3], a);
-      }
-      hid[r] = fmaxf(a, 0.f);
-    }
-#pragma unroll
-    for (int r = 0; r < 4; ++r) {
-      float a = 0.f;
-      const float4* wr = reinterpret_cast<const float4*>(sw2 + (m * 4 + r) * kHid);
-#pragma unroll
-      for (int c = 0; c < kHid / 4; ++c) {
-        const float4 w4 = wr[c];
-        a = fmaf(w4.x, hid[4 * c], a); a = fmaf(w4.y, hid[4 * c + 1], a);
-        a = fmaf(w4.z, hid[4 * c + 2], a); a = fmaf(w4.w, hid[4 * c + 3], a);
-      }
-      outv[m][r] = a;
-    }
-  }
-  float q[4] = {0.f, 0.f, 0.f, 1.f}, sc[3] = {0.f, 0.f, 0.f};
-  float qn = 1.f;
-  if (active) {
-    const float* qb = X.rot_base ? X.rot_base + 4 * ((size_t)t * P + i) : rotation + 4 * i;
-    for (int k = 0; k < 4; ++k) q[k] = qb[k] + outv[1][k];
-    qn = fmaxf(sqrtf(q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3]), 1e-12f);
-    for (int k = 0; k < 3; ++k) sc[k] = expf(scaling[3 * i + k] + (deform_scale ? outv[2][k] : 0.f));
+    mlp_forward(sw1, sw2, m, feat, hid, outv[m]);
   }
   if (active) {
     const size_t o = (size_t)t * P + i;
+    float y[4];
+    normalized_rotation(X.rot_base ? X.rot_base + 4 * o : rotation + 4 * i, outv[1], y);
     for (int k = 0; k < 3; ++k) out_means[3 * o + k] = pt[k] + outv[0][k];
-    for (int k = 0; k < 3; ++k) out_scales[3 * o + k] = sc[k];
-    for (int k = 0; k < 4; ++k) out_rots[4 * o + k] = q[k] / qn;
+    for (int k = 0; k < 3; ++k) out_scales[3 * o + k] = expf(scaling[3 * i + k] + (deform_scale ? outv[2][k] : 0.f));
+    for (int k = 0; k < 4; ++k) out_rots[4 * o + k] = y[k];
   }
 }
-
 
 // ---------------------------------------------------------------------------------------------------------------
 // Backward (round 2).  The round-1 backward was deform_kernel<1>: every thread pushed its 3 x (32x32 + 4x32) weight-gradient
@@ -173,11 +200,6 @@ __device__ __forceinline__ void red_add_v4(float* addr, float a, float b, float 
   asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(addr), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
 }
 
-__device__ __forceinline__ float plane_sample(const float* __restrict__ gc, const Bilerp& b, int W) {
-  return (__ldg(gc + b.y0 * W + b.x0) * (1.f - b.wx) + __ldg(gc + b.y0 * W + b.x1) * b.wx) * (1.f - b.wy) +
-         (__ldg(gc + b.y1 * W + b.x0) * (1.f - b.wx) + __ldg(gc + b.y1 * W + b.x1) * b.wx) * b.wy;
-}
-
 // Per-frame mean feature in a fixed order: a cluster of kFmCtas CTAs per frame; each thread sums a strided subset of the
 // gaussians, each CTA sums its threads in thread order, and CTA rank 0 adds the cluster's CTA sums in rank order through
 // distributed shared memory.  No atomics and no scratch: bit-reproducible for a given launch geometry.
@@ -197,15 +219,7 @@ deform_featmean_kernel(DeformGrids G, const float* __restrict__ xyz, const float
   for (int i = rank * kFmThreads + threadIdx.x; i < P; i += kFmCtas * kFmThreads) {
     const float pt[4] = {xyz[3 * i], xyz[3 * i + 1], xyz[3 * i + 2], tm};
     float feat[kHid];
-#pragma unroll
-    for (int c = 0; c < kHid; ++c) feat[c] = 1.f;
-    for (int sc = 0; sc < G.scales; ++sc)
-      for (int pl = 0; pl < kPlanes; ++pl) {
-        const int W = G.w[sc][pl], H = G.h[sc][pl];
-        const Bilerp b = bilerp_setup(pt[c_comb[pl][0]], pt[c_comb[pl][1]], W, H);
-#pragma unroll
-        for (int c = 0; c < kFeat; ++c) feat[sc * kFeat + c] *= plane_sample(G.plane[sc][pl] + (size_t)c * H * W, b, W);
-      }
+    kplanes_feature(G, pt, true, feat);
 #pragma unroll
     for (int c = 0; c < kHid; ++c) acc[c] += feat[c];
   }
@@ -244,14 +258,7 @@ deform_backward_kernel(DeformGrids G, DeformMlp M, DeformGlobal X, const float* 
   float* s_do = s_df + kBwdThreads * kLdS;           // [128][4]: dout of the current MLP
   float* s_acc = s_do + kBwdThreads * 4;             // [3][kOwn][128]: the weight-gradient entries each thread owns
   const int nfeat = G.scales * kFeat;
-  for (int i = threadIdx.x; i < 3 * kHid * kHid; i += blockDim.x) {
-    const int m = i / (kHid * kHid), r = i % (kHid * kHid);
-    sw1[i] = (r % kHid < nfeat) ? M.w1[m][(r / kHid) * nfeat + r % kHid] : 0.f;
-  }
-  for (int i = threadIdx.x; i < 3 * 4 * kHid; i += blockDim.x) {
-    const int m = i / (4 * kHid), r = (i % (4 * kHid)) / kHid, c = i % kHid;
-    sw2[i] = r < out_dim(m) ? M.w2[m][r * kHid + c] : 0.f;
-  }
+  stage_mlp_weights(M, nfeat, sw1, sw2);
   for (int i = threadIdx.x; i < 3 * kOwn * kBwdThreads; i += blockDim.x) s_acc[i] = 0.f;
   // weight-gradient entries this thread owns: W1[m][r1][c1 .. c1+7] and W2[m][e / 32][e % 32] for e = tid, tid+128, tid+256
   const int r1 = threadIdx.x >> 2, c1 = (threadIdx.x & 3) * 8;
@@ -260,23 +267,11 @@ deform_backward_kernel(DeformGrids G, DeformMlp M, DeformGlobal X, const float* 
   for (long long base = (long long)blockIdx.x * kBwdThreads; base < total; base += (long long)gridDim.x * kBwdThreads) {
     const long long idx = base + threadIdx.x;
     const bool active = idx < total;
-    const int t = active ? (int)(idx / P) : 0, i = active ? (int)(idx % P) : 0;
-    float pt[4] = {0.f, 0.f, 0.f, 0.f};
-    if (active) { pt[0] = xyz[3 * i]; pt[1] = xyz[3 * i + 1]; pt[2] = xyz[3 * i + 2]; pt[3] = times[t]; }
-    // ---- features
+    int t, i;
+    float pt[4];
+    item_point(xyz, times, P, idx, active, pt, t, i);
     float feat[kHid];
-#pragma unroll
-    for (int c = 0; c < kHid; ++c) feat[c] = c < nfeat ? 1.f : 0.f;
-    if (active) {
-      for (int s = 0; s < G.scales; ++s)
-        for (int pl = 0; pl < kPlanes; ++pl) {
-          const int W = G.w[s][pl], H = G.h[s][pl];
-          const Bilerp b = bilerp_setup(pt[c_comb[pl][0]], pt[c_comb[pl][1]], W, H);
-          const float* g = G.plane[s][pl];
-#pragma unroll
-          for (int c = 0; c < kFeat; ++c) feat[s * kFeat + c] *= plane_sample(g + (size_t)c * H * W, b, W);
-        }
-    }
+    kplanes_feature(G, pt, active, feat);
     __syncthreads();                                  // previous chunk's readers of the staged tiles are done
 #pragma unroll
     for (int c = 0; c < kHid; c += 4) {
@@ -286,27 +281,8 @@ deform_backward_kernel(DeformGrids G, DeformMlp M, DeformGlobal X, const float* 
 #pragma unroll 1
     for (int m = 0; m < 3; ++m) {
       // forward of MLP m (hidden layer kept; the output only enters the rotation / scale Jacobians)
-      float hid[kHid];
-#pragma unroll
-      for (int r = 0; r < kHid; ++r) {
-        float a = 0.f;
-        const float4* wr = reinterpret_cast<const float4*>(sw1 + (m * kHid + r) * kHid);
-#pragma unroll
-        for (int c = 0; c < kHid / 4; ++c) {
-          const float4 w4 = wr[c];
-          a = fmaf(w4.x, feat[4 * c], a); a = fmaf(w4.y, feat[4 * c + 1], a);
-          a = fmaf(w4.z, feat[4 * c + 2], a); a = fmaf(w4.w, feat[4 * c + 3], a);
-        }
-        hid[r] = fmaxf(a, 0.f);
-      }
-      float outv[4], dout[4] = {0.f, 0.f, 0.f, 0.f};
-#pragma unroll
-      for (int r = 0; r < 4; ++r) {
-        float a = 0.f;
-#pragma unroll
-        for (int c = 0; c < kHid; ++c) a = fmaf(sw2[(m * 4 + r) * kHid + c], hid[c], a);
-        outv[r] = a;
-      }
+      float hid[kHid], outv[4], dout[4] = {0.f, 0.f, 0.f, 0.f};
+      mlp_forward(sw1, sw2, m, feat, hid, outv);
       if (active) {
         const size_t o = (size_t)t * P + i;
         if (m == 0) {
@@ -315,11 +291,9 @@ deform_backward_kernel(DeformGrids G, DeformMlp M, DeformGlobal X, const float* 
           if (deform_scale && g_scales)
             for (int k = 0; k < 3; ++k) dout[k] = g_scales[3 * o + k] * expf(scaling[3 * i + k] + outv[k]);           // d exp
         } else if (g_rots) {   // y = q / |q|: dq = (g - y (y.g)) / |q|
-          const float* qb = X.rot_base ? X.rot_base + 4 * o : rotation + 4 * i;
-          float q[4], y[4], dot = 0.f;
-          for (int k = 0; k < 4; ++k) q[k] = qb[k] + outv[k];
-          const float qn = fmaxf(sqrtf(q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3]), 1e-12f);
-          for (int k = 0; k < 4; ++k) { y[k] = q[k] / qn; dot += y[k] * g_rots[4 * o + k]; }
+          float y[4], dot = 0.f;
+          const float qn = normalized_rotation(X.rot_base ? X.rot_base + 4 * o : rotation + 4 * i, outv, y);
+          for (int k = 0; k < 4; ++k) dot += y[k] * g_rots[4 * o + k];
           for (int k = 0; k < 4; ++k) dout[k] = (g_rots[4 * o + k] - y[k] * dot) / qn;
           if (X.g_rot_base) for (int k = 0; k < 4; ++k) X.g_rot_base[4 * o + k] = dout[k];   // q = rot_base + delta
         }
@@ -479,8 +453,9 @@ __global__ void deform_cell_keys_kernel(const float* __restrict__ xyz, const flo
                                         int cb, int W, int H, uint32_t* __restrict__ keys, uint32_t* __restrict__ vals) {
   const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= total) return;
-  const int t = (int)(idx / P), i = (int)(idx % P);
-  const float pt[4] = {xyz[3 * i], xyz[3 * i + 1], xyz[3 * i + 2], times[t]};
+  int t, i;
+  float pt[4];
+  item_point(xyz, times, P, idx, true, pt, t, i);
   const Bilerp b = bilerp_setup(pt[ca], pt[cb], W, H);
   keys[idx] = (uint32_t)(b.y0 * W + b.x0);
   vals[idx] = (uint32_t)idx;
@@ -501,8 +476,9 @@ __global__ void deform_plane_gather_kernel(const float* __restrict__ xyz, const 
       const uint2 r = ranges[cy * W + cx];
       for (uint32_t k = r.x; k < r.y; ++k) {
         const uint32_t p = pts[k];
-        const int t = (int)(p / (uint32_t)P), i = (int)(p % (uint32_t)P);
-        const float pt[4] = {xyz[3 * i], xyz[3 * i + 1], xyz[3 * i + 2], times[t]};
+        int t, i;
+        float pt[4];
+        item_point(xyz, times, P, p, true, pt, t, i);
         const Bilerp b = bilerp_setup(pt[ca], pt[cb], W, H);
         // corner (y1, x1) of a cell on the last row / column coincides with (y0, x0) and has weight 0 there
         const float w = (cy == y ? 1.f - b.wy : b.wy) * (cx == x ? 1.f - b.wx : b.wx);
@@ -620,8 +596,8 @@ extern "C" size_t a3d_deform_backward_scratch_bytes(const a3d_deform_args* a) {
   return carve_det(nullptr, a, nullptr);
 }
 
-extern "C" int a3d_deform_backward_ex(const a3d_deform_args* a, const float* g_means, const float* g_scales, const float* g_rots,
-                                      void* scratch, size_t scratch_bytes, void* stream) {
+extern "C" int a3d_deform_backward(const a3d_deform_args* a, const float* g_means, const float* g_scales, const float* g_rots,
+                                   void* scratch, size_t scratch_bytes, void* stream) {
   // grad_planes[i]: CHANNEL-LAST scratch [H_i, W_i, 16] (zero-initialised by the caller, accumulated into); the caller transposes
   // it into the [1, 16, H, W] parameter gradient (animate3d_b200/gaussian4d.py)
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
@@ -666,8 +642,7 @@ extern "C" int a3d_deform_backward_ex(const a3d_deform_args* a, const float* g_m
   for (int sc = 0; sc < G.scales; ++sc) {
     if (!G.gplane[sc][0]) continue;
     for (int pl = 0; pl < kPlanes; ++pl) {
-      static const int comb[kPlanes][2] = {{0, 1}, {0, 2}, {0, 3}, {1, 2}, {1, 3}, {2, 3}};   // = c_comb
-      const int W = G.w[sc][pl], H = G.h[sc][pl], ca = comb[pl][0], cb = comb[pl][1];
+      const int W = G.w[sc][pl], H = G.h[sc][pl], ca = kComb[pl][0], cb = kComb[pl][1];
       deform_cell_keys_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(a->xyz, a->times, a->P, n, ca, cb, W, H, s.keys_in, s.vals_in);
       A3D_LAUNCH_CHECK();
       if (int r = seg_sort(s.keys_in, s.vals_in, s.keys_out, s.vals_out, (int)n, (uint32_t)(H * W), s.ranges, s.temp, s.temp_bytes, st))
@@ -678,10 +653,4 @@ extern "C" int a3d_deform_backward_ex(const a3d_deform_args* a, const float* g_m
     }
   }
   return A3D_OK;
-}
-
-extern "C" int a3d_deform_backward(const a3d_deform_args* a, const float* g_means, const float* g_scales, const float* g_rots,
-                                   void* stream) {
-  if (a && a->deterministic) return fail(A3D_EINVAL, "a3d_deform_backward: deterministic = 1 needs a3d_deform_backward_ex's scratch");
-  return a3d_deform_backward_ex(a, g_means, g_scales, g_rots, nullptr, 0, stream);
 }

@@ -239,6 +239,26 @@ static size_t cub_temp_bytes(int n_scan, long long cap, int end_bit) {
   return (b1 > b2 ? b1 : b2) + 256;
 }
 
+// Launch and workspace layout of a call: tile grid, sort key bits, CUB temp bytes and the carved workspace (base may be null
+// for a size query).  The forward, the backward and the binning tap must all agree on it.
+struct RasterLayout {
+  int gx, gy;
+  long long total_tiles;
+  int end_bit;
+  size_t bytes;
+  RasterWs ws;
+};
+
+static RasterLayout raster_layout(void* base, int P, int H, int W, int cams, long long cap) {
+  RasterLayout l;
+  l.gx = (W + kTile - 1) / kTile;
+  l.gy = (H + kTile - 1) / kTile;
+  l.total_tiles = (long long)cams * l.gx * l.gy;
+  l.end_bit = sort_bits(l.total_tiles);
+  l.bytes = carve_workspace(base, P, H, W, cams, cap, cub_temp_bytes(cams * P, cap, l.end_bit), &l.ws);
+  return l;
+}
+
 static RasterDev make_dev(const a3d_raster_args* a) {
   RasterDev d;
   d.P = a->P; d.H = a->H; d.W = a->W; d.num_cams = a->num_cams; d.cams = a->cams;
@@ -301,9 +321,7 @@ extern "C" int a3d_debug_raster_stage_ms(float* out_host8) {
 }
 
 extern "C" size_t a3d_raster_workspace_bytes(int P, int H, int W, int num_cams, int64_t max_rendered) {
-  const int gx = (W + kTile - 1) / kTile, gy = (H + kTile - 1) / kTile;
-  const size_t cub = cub_temp_bytes(num_cams * P, max_rendered, sort_bits((long long)num_cams * gx * gy));
-  return carve_workspace(nullptr, P, H, W, num_cams, max_rendered, cub, nullptr);
+  return raster_layout(nullptr, P, H, W, num_cams, max_rendered).bytes;
 }
 
 extern "C" int a3d_raster_forward(const a3d_raster_args* a, float* color, float* depth, float* alpha, int32_t* radii,
@@ -312,17 +330,13 @@ extern "C" int a3d_raster_forward(const a3d_raster_args* a, float* color, float*
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   if (int r = check_args(a, max_rendered)) return r;
   if (!color || !depth || !alpha || !radii || !workspace) return fail(A3D_EINVAL, "a3d_raster_forward: null output");
-  const int gx = (a->W + kTile - 1) / kTile, gy = (a->H + kTile - 1) / kTile;
-  const long long total_tiles = (long long)a->num_cams * gx * gy;
-  const int end_bit = sort_bits(total_tiles);
-  const size_t cub = cub_temp_bytes(a->num_cams * a->P, max_rendered, end_bit);
-  RasterWs ws;
-  const size_t need = carve_workspace(workspace, a->P, a->H, a->W, a->num_cams, max_rendered, cub, &ws);
-  if (need > workspace_bytes) return fail(A3D_EINVAL, "a3d_raster_forward: workspace %zu < %zu bytes", workspace_bytes, need);
+  const RasterLayout l = raster_layout(workspace, a->P, a->H, a->W, a->num_cams, max_rendered);
+  if (l.bytes > workspace_bytes) return fail(A3D_EINVAL, "a3d_raster_forward: workspace %zu < %zu bytes", workspace_bytes, l.bytes);
+  const RasterWs& ws = l.ws;
   const RasterDev d = make_dev(a);
   const int n = a->num_cams * a->P;
   A3D_CUDA_CHECK(cudaMemsetAsync(ws.keys_a, 0xFF, (size_t)max_rendered * 8, st));
-  A3D_CUDA_CHECK(cudaMemsetAsync(ws.ranges, 0, (size_t)total_tiles * 8, st));
+  A3D_CUDA_CHECK(cudaMemsetAsync(ws.ranges, 0, (size_t)l.total_tiles * 8, st));
   stamp(0, st);
   launch_preprocess(d, ws, radii, st);
   A3D_LAUNCH_CHECK();
@@ -330,16 +344,16 @@ extern "C" int a3d_raster_forward(const a3d_raster_args* a, float* color, float*
   size_t tb = ws.cub_bytes;
   A3D_CUDA_CHECK(cub::DeviceScan::InclusiveSum(ws.cub_temp, tb, ws.tiles, ws.offsets, n, st));
   launch_counts(ws, a->P, a->num_cams, max_rendered, st);
-  launch_duplicate(d, ws, gx, gx * gy, max_rendered, st);
+  launch_duplicate(d, ws, l.gx, l.gx * l.gy, max_rendered, st);
   A3D_LAUNCH_CHECK();
   stamp(2, st);
   tb = ws.cub_bytes;
   A3D_CUDA_CHECK(cub::DeviceRadixSort::SortPairs(ws.cub_temp, tb, ws.keys_a, ws.keys_b, ws.vals_a, ws.vals_b, (int)max_rendered, 0,
-                                                 end_bit, st));
+                                                 l.end_bit, st));
   stamp(3, st);
-  launch_ranges(ws, max_rendered, total_tiles, st);
+  launch_ranges(ws, max_rendered, l.total_tiles, st);
   stamp(4, st);
-  dim3 grid(gx, gy, a->num_cams), block(kTile, kTile);
+  dim3 grid(l.gx, l.gy, a->num_cams), block(kTile, kTile);
   raster_render_forward_kernel<<<grid, block, 0, st>>>(d, ws, color, depth, alpha);
   A3D_LAUNCH_CHECK();
   stamp(5, st);
@@ -351,18 +365,12 @@ extern "C" int a3d_raster_forward(const a3d_raster_args* a, float* color, float*
 
 // deterministic backward scratch: one record per pair slot, then the per-(camera, gaussian) opacity partials
 static size_t carve_det(void* base, const a3d_raster_args* a, long long cap, float** records, float** op_part) {
-  size_t off = 0;
-  auto take = [&](size_t bytes) {
-    off = (off + 255) & ~(size_t)255;
-    float* p = base ? reinterpret_cast<float*>(static_cast<char*>(base) + off) : nullptr;
-    off += bytes;
-    return p;
-  };
-  float* r = take((size_t)cap * kRecord * sizeof(float));
-  float* o = take((size_t)a->num_cams * a->P * sizeof(float));
+  Carve c{static_cast<char*>(base)};
+  float* r = c.take<float>((size_t)cap * kRecord);
+  float* o = c.take<float>((size_t)a->num_cams * a->P);
   if (records) *records = r;
   if (op_part) *op_part = o;
-  return (off + 255) & ~(size_t)255;
+  return c.bytes();
 }
 
 extern "C" size_t a3d_raster_backward_scratch_bytes(const a3d_raster_args* a, int64_t max_rendered) {
@@ -370,21 +378,16 @@ extern "C" size_t a3d_raster_backward_scratch_bytes(const a3d_raster_args* a, in
   return carve_det(nullptr, a, max_rendered, nullptr, nullptr);
 }
 
-extern "C" int a3d_raster_backward_ex(const a3d_raster_args* a, const float* dL_dcolor, const float* dL_ddepth, const float* dL_dalpha,
-                                      const float* alpha, const int32_t* radii, void* workspace, size_t workspace_bytes,
-                                      int64_t max_rendered, float* dL_dmeans3D, float* dL_dscales, float* dL_drotations,
-                                      float* dL_dopacity, float* dL_dcolors, float* dL_dshs, float* dL_dmeans2D, void* scratch,
-                                      size_t scratch_bytes, void* stream) {
+extern "C" int a3d_raster_backward(const a3d_raster_args* a, const float* dL_dcolor, const float* dL_ddepth, const float* dL_dalpha,
+                                   const int32_t* radii, void* workspace, size_t workspace_bytes, int64_t max_rendered,
+                                   float* dL_dmeans3D, float* dL_dscales, float* dL_drotations, float* dL_dopacity, float* dL_dcolors,
+                                   float* dL_dshs, float* dL_dmeans2D, void* scratch, size_t scratch_bytes, void* stream) {
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  (void)alpha;
   if (int r = check_args(a, max_rendered)) return r;
   if (!dL_dcolor || !radii || !workspace) return fail(A3D_EINVAL, "a3d_raster_backward: null input");
-  const int gx = (a->W + kTile - 1) / kTile, gy = (a->H + kTile - 1) / kTile;
-  const long long total_tiles = (long long)a->num_cams * gx * gy;
-  const size_t cub = cub_temp_bytes(a->num_cams * a->P, max_rendered, sort_bits(total_tiles));
-  RasterWs ws;
-  const size_t need = carve_workspace(workspace, a->P, a->H, a->W, a->num_cams, max_rendered, cub, &ws);
-  if (need > workspace_bytes) return fail(A3D_EINVAL, "a3d_raster_backward: workspace %zu < %zu bytes", workspace_bytes, need);
+  const RasterLayout l = raster_layout(workspace, a->P, a->H, a->W, a->num_cams, max_rendered);
+  if (l.bytes > workspace_bytes) return fail(A3D_EINVAL, "a3d_raster_backward: workspace %zu < %zu bytes", workspace_bytes, l.bytes);
+  const RasterWs& ws = l.ws;
   float *records = nullptr, *op_part = nullptr;
   if (a->deterministic) {
     const size_t det = carve_det(scratch, a, max_rendered, &records, &op_part);
@@ -396,7 +399,7 @@ extern "C" int a3d_raster_backward_ex(const a3d_raster_args* a, const float* dL_
   A3D_CUDA_CHECK(cudaMemsetAsync(ws.g_conic, 0, n * 12, st));
   A3D_CUDA_CHECK(cudaMemsetAsync(ws.g_depth, 0, n * 4, st));
   A3D_CUDA_CHECK(cudaMemsetAsync(ws.g_rgb, 0, n * 12, st));
-  dim3 grid(gx, gy, a->num_cams), block(kTile, kTile);
+  dim3 grid(l.gx, l.gy, a->num_cams), block(kTile, kTile);
   stamp(6, st);
   if (a->deterministic) {
     static bool attr = false;
@@ -423,22 +426,11 @@ extern "C" int a3d_raster_backward_ex(const a3d_raster_args* a, const float* dL_
   return A3D_OK;
 }
 
-extern "C" int a3d_raster_backward(const a3d_raster_args* a, const float* dL_dcolor, const float* dL_ddepth, const float* dL_dalpha,
-                                   const float* alpha, const int32_t* radii, void* workspace, size_t workspace_bytes,
-                                   int64_t max_rendered, float* dL_dmeans3D, float* dL_dscales, float* dL_drotations,
-                                   float* dL_dopacity, float* dL_dcolors, float* dL_dshs, float* dL_dmeans2D, void* stream) {
-  if (a && a->deterministic) return fail(A3D_EINVAL, "a3d_raster_backward: deterministic = 1 needs a3d_raster_backward_ex's scratch");
-  return a3d_raster_backward_ex(a, dL_dcolor, dL_ddepth, dL_dalpha, alpha, radii, workspace, workspace_bytes, max_rendered, dL_dmeans3D,
-                                dL_dscales, dL_drotations, dL_dopacity, dL_dcolors, dL_dshs, dL_dmeans2D, nullptr, 0, stream);
-}
-
 extern "C" int a3d_raster_binning_tap(const void* workspace, int P, int H, int W, int num_cams, int64_t max_rendered, int cam,
                                       uint64_t* keys_out, uint32_t* point_list_out, uint32_t* ranges_out, void* stream) {
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  const int gx = (W + kTile - 1) / kTile, gy = (H + kTile - 1) / kTile;
-  const size_t cub = cub_temp_bytes(num_cams * P, max_rendered, sort_bits((long long)num_cams * gx * gy));
-  RasterWs ws;
-  carve_workspace(const_cast<void*>(workspace), P, H, W, num_cams, max_rendered, cub, &ws);
+  const RasterLayout l = raster_layout(const_cast<void*>(workspace), P, H, W, num_cams, max_rendered);
+  const RasterWs& ws = l.ws;
   // raw copies of the global sorted tables; the host wrapper slices camera `cam` out of them using the counters
   (void)cam;
   if (keys_out) {   // external form of a key: (tile << 32) | depth bits (the upstream rasterizer's layout)
@@ -446,6 +438,6 @@ extern "C" int a3d_raster_binning_tap(const void* workspace, int P, int H, int W
     A3D_LAUNCH_CHECK();
   }
   if (point_list_out) A3D_CUDA_CHECK(cudaMemcpyAsync(point_list_out, ws.vals_b, (size_t)max_rendered * 4, cudaMemcpyDeviceToDevice, st));
-  if (ranges_out) A3D_CUDA_CHECK(cudaMemcpyAsync(ranges_out, ws.ranges, (size_t)num_cams * gx * gy * 8, cudaMemcpyDeviceToDevice, st));
+  if (ranges_out) A3D_CUDA_CHECK(cudaMemcpyAsync(ranges_out, ws.ranges, (size_t)l.total_tiles * 8, cudaMemcpyDeviceToDevice, st));
   return A3D_OK;
 }

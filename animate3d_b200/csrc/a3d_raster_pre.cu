@@ -24,6 +24,13 @@ __device__ __forceinline__ void sh_basis(int deg, float x, float y, float z, flo
   }
 }
 
+// unit direction from the camera centre to the gaussian mean m: the direction the SH colour is evaluated in
+__device__ __forceinline__ void view_dir(const float* m, const a3d_raster_cam& c, float& dx, float& dy, float& dz) {
+  dx = m[0] - c.campos[0]; dy = m[1] - c.campos[1]; dz = m[2] - c.campos[2];
+  const float n = sqrtf((dx * dx + dy * dy) + dz * dz);
+  dx /= n; dy /= n; dz /= n;
+}
+
 __global__ void raster_preprocess_kernel(RasterDev a, RasterWs ws, int32_t* __restrict__ radii) {
   const int idx = blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= a.num_cams * a.P) return;
@@ -46,10 +53,8 @@ __global__ void raster_preprocess_kernel(RasterDev a, RasterWs ws, int32_t* __re
   if (a.colors_precomp) {
     for (int ch = 0; ch < 3; ++ch) rgb[ch] = a.colors_precomp[3 * i + ch];
   } else {
-    float dx = a.means3D[3 * gi] - c.campos[0], dy = a.means3D[3 * gi + 1] - c.campos[1], dz = a.means3D[3 * gi + 2] - c.campos[2];
-    const float n = sqrtf((dx * dx + dy * dy) + dz * dz);
-    dx /= n; dy /= n; dz /= n;
-    float b[16];
+    float dx, dy, dz, b[16];
+    view_dir(a.means3D + 3 * gi, c, dx, dy, dz);
     sh_basis(a.sh_degree, dx, dy, dz, b);
     const int nb = (a.sh_degree + 1) * (a.sh_degree + 1);
     const float* sh = a.shs + (size_t)i * a.sh_coeffs * 3;
@@ -107,6 +112,32 @@ __global__ void raster_ranges_kernel(RasterWs ws, long long n, long long total_t
   if (idx == n - 1 || (ws.keys_b[idx + 1] >> 31) != tile) ws.ranges[tile].y = (uint32_t)(idx + 1);
 }
 
+// Per-(camera, gaussian) part of the preprocess backward, shared by both kernels, for a visible pair idx (camera cam, geometry
+// slot gi): the (dconic, dmean2D, ddepth) gradients pushed through the projection into dm / ds / dr, the dmeans2D write
+// (upstream convention: gradient w.r.t. NDC coordinates), and with sh_grad the SH basis of the view direction and the clamp
+// mask of the forward colours.  colour = clamp(sum_k basis_k(dir) * sh_k + 0.5) is linear in the coefficients; the dependence
+// of the basis on the view direction is not differentiated (Animate3D's features are frozen buffers, gaussian_4d.py:262-297).
+__device__ __forceinline__ void pair_backward(const RasterDev& a, const RasterWs& ws, int cam, size_t idx, size_t gi, float* dmeans2D,
+                                              bool sh_grad, float (&dm)[3], float (&ds)[3], float (&dr)[4], float (&b)[16],
+                                              uint32_t& clamped) {
+  const a3d_raster_cam& c = a.cams[cam];
+  const float gpx = ws.g_mean2d[2 * idx], gpy = ws.g_mean2d[2 * idx + 1];
+  preprocess_backward(a.means3D + 3 * gi, a.scales + 3 * gi, a.rotations + 4 * gi, a.scale_modifier, c.viewmatrix, c.projmatrix,
+                      c.tanfovx, c.tanfovy, a.H, a.W, ws.g_conic[3 * idx], ws.g_conic[3 * idx + 1], ws.g_conic[3 * idx + 2], gpx, gpy,
+                      ws.g_depth[idx], dm, ds, dr);
+  if (dmeans2D) {
+    dmeans2D[3 * idx] = gpx * 0.5f * (float)a.W;
+    dmeans2D[3 * idx + 1] = gpy * 0.5f * (float)a.H;
+    dmeans2D[3 * idx + 2] = 0.f;
+  }
+  if (sh_grad) {
+    float dx, dy, dz;
+    view_dir(a.means3D + 3 * gi, c, dx, dy, dz);
+    sh_basis(a.sh_degree, dx, dy, dz, b);
+    clamped = ws.clamped[idx];
+  }
+}
+
 // per-gaussian backward: (dconic, dmean2D, ddepth, drgb) of every camera -> means3D / scales / rotations / colors / SH
 __global__ void raster_preprocess_backward_kernel(RasterDev a, RasterWs ws, const int32_t* __restrict__ radii,
                                                   float* __restrict__ dmeans3D, float* __restrict__ dscales,
@@ -116,37 +147,20 @@ __global__ void raster_preprocess_backward_kernel(RasterDev a, RasterWs ws, cons
   if (idx >= a.num_cams * a.P) return;
   if (radii[idx] <= 0) return;
   const int cam = idx / a.P, i = idx % a.P;
-  const int g = a.per_cam_geometry ? cam : 0;
-  const size_t gi = (size_t)g * a.P + i;
-  const a3d_raster_cam& c = a.cams[cam];
-  const float gpx = ws.g_mean2d[2 * (size_t)idx], gpy = ws.g_mean2d[2 * (size_t)idx + 1];
-  float dm[3], ds[3], dr[4];
-  preprocess_backward(a.means3D + 3 * gi, a.scales + 3 * gi, a.rotations + 4 * gi, a.scale_modifier, c.viewmatrix, c.projmatrix,
-                      c.tanfovx, c.tanfovy, a.H, a.W, ws.g_conic[3 * (size_t)idx], ws.g_conic[3 * (size_t)idx + 1],
-                      ws.g_conic[3 * (size_t)idx + 2], gpx, gpy, ws.g_depth[idx], dm, ds, dr);
+  const size_t gi = (size_t)(a.per_cam_geometry ? cam : 0) * a.P + i;
+  float dm[3], ds[3], dr[4], b[16];
+  uint32_t cl = 0;
+  pair_backward(a, ws, cam, idx, gi, dmeans2D, !a.colors_precomp && dshs, dm, ds, dr, b, cl);
   for (int k = 0; k < 3; ++k) {
     if (dmeans3D) atomicAdd(dmeans3D + 3 * gi + k, dm[k]);
     if (dscales) atomicAdd(dscales + 3 * gi + k, ds[k]);
   }
   if (drots) for (int k = 0; k < 4; ++k) atomicAdd(drots + 4 * gi + k, dr[k]);
-  if (dmeans2D) {   // upstream convention: gradient w.r.t. NDC coordinates
-    dmeans2D[3 * (size_t)idx] = gpx * 0.5f * (float)a.W;
-    dmeans2D[3 * (size_t)idx + 1] = gpy * 0.5f * (float)a.H;
-    dmeans2D[3 * (size_t)idx + 2] = 0.f;
-  }
   const float* grgb = ws.g_rgb + 3 * (size_t)idx;
   if (a.colors_precomp) {
     if (dcolors) for (int ch = 0; ch < 3; ++ch) atomicAdd(dcolors + 3 * i + ch, grgb[ch]);
   } else if (dshs) {
-    // colour = clamp(sum_k basis_k(dir) * sh_k + 0.5): linear in the coefficients.  (The dependence of the basis on the
-    // view direction is not differentiated: Animate3D's features are frozen buffers, gaussian_4d.py:262-297.)
-    float dx = a.means3D[3 * gi] - c.campos[0], dy = a.means3D[3 * gi + 1] - c.campos[1], dz = a.means3D[3 * gi + 2] - c.campos[2];
-    const float n = sqrtf(dx * dx + dy * dy + dz * dz);
-    dx /= n; dy /= n; dz /= n;
-    float b[16];
-    sh_basis(a.sh_degree, dx, dy, dz, b);
     const int nb = (a.sh_degree + 1) * (a.sh_degree + 1);
-    const uint32_t cl = ws.clamped[idx];
     for (int ch = 0; ch < 3; ++ch) {
       if (cl & (1u << ch)) continue;
       for (int k = 0; k < nb; ++k) atomicAdd(dshs + ((size_t)i * a.sh_coeffs + k) * 3 + ch, b[k] * grgb[ch]);
@@ -197,14 +211,10 @@ __global__ void raster_preprocess_backward_det_kernel(RasterDev a, RasterWs ws, 
     const size_t idx = (size_t)cam * a.P + i;
     aop += op_part[idx];
     if (radii[idx] <= 0) continue;
-    const int g = a.per_cam_geometry ? cam : 0;
-    const size_t gi = (size_t)g * a.P + i;
-    const a3d_raster_cam& c = a.cams[cam];
-    const float gpx = ws.g_mean2d[2 * idx], gpy = ws.g_mean2d[2 * idx + 1];
-    float dm[3], ds[3], dr[4];
-    preprocess_backward(a.means3D + 3 * gi, a.scales + 3 * gi, a.rotations + 4 * gi, a.scale_modifier, c.viewmatrix, c.projmatrix,
-                        c.tanfovx, c.tanfovy, a.H, a.W, ws.g_conic[3 * idx], ws.g_conic[3 * idx + 1], ws.g_conic[3 * idx + 2], gpx, gpy,
-                        ws.g_depth[idx], dm, ds, dr);
+    const size_t gi = (size_t)(a.per_cam_geometry ? cam : 0) * a.P + i;
+    float dm[3], ds[3], dr[4], b[16];
+    uint32_t cl = 0;
+    pair_backward(a, ws, cam, idx, gi, dmeans2D, !a.colors_precomp && dshs, dm, ds, dr, b, cl);
     if (a.per_cam_geometry) {   // one camera per gradient entry: written directly
       for (int k = 0; k < 3; ++k) {
         if (dmeans3D) dmeans3D[3 * gi + k] += dm[k];
@@ -215,21 +225,10 @@ __global__ void raster_preprocess_backward_det_kernel(RasterDev a, RasterWs ws, 
       for (int k = 0; k < 3; ++k) { am[k] += dm[k]; as[k] += ds[k]; }
       for (int k = 0; k < 4; ++k) ar[k] += dr[k];
     }
-    if (dmeans2D) {
-      dmeans2D[3 * idx] = gpx * 0.5f * (float)a.W;
-      dmeans2D[3 * idx + 1] = gpy * 0.5f * (float)a.H;
-      dmeans2D[3 * idx + 2] = 0.f;
-    }
     const float* grgb = ws.g_rgb + 3 * idx;
     if (a.colors_precomp) {
       for (int ch = 0; ch < 3; ++ch) acol[ch] += grgb[ch];
     } else if (dshs) {
-      float dx = a.means3D[3 * gi] - c.campos[0], dy = a.means3D[3 * gi + 1] - c.campos[1], dz = a.means3D[3 * gi + 2] - c.campos[2];
-      const float n = sqrtf(dx * dx + dy * dy + dz * dz);
-      dx /= n; dy /= n; dz /= n;
-      float b[16];
-      sh_basis(a.sh_degree, dx, dy, dz, b);
-      const uint32_t cl = ws.clamped[idx];
 #pragma unroll
       for (int k = 0; k < 16; ++k)
         if (k < nb)

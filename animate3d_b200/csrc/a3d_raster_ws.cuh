@@ -4,6 +4,7 @@
 #include <stdint.h>
 
 #include "../../include/a3d.h"
+#include "a3d_carve.h"
 #include "a3d_raster_math.h"
 
 namespace a3d {
@@ -43,40 +44,34 @@ struct RasterWs {
 
 // Carves `base` (may be null for a size query) and returns the bytes needed.
 inline size_t carve_workspace(void* base, int P, int H, int W, int cams, long long cap, size_t cub_bytes, RasterWs* ws) {
-  size_t off = 0;
-  auto take = [&](size_t bytes) {
-    off = (off + 255) & ~(size_t)255;
-    void* p = base ? static_cast<char*>(base) + off : nullptr;
-    off += bytes;
-    return p;
-  };
+  Carve c{static_cast<char*>(base)};
   const size_t n = (size_t)cams * P;
   const int gx = (W + kTile - 1) / kTile, gy = (H + kTile - 1) / kTile;
   RasterWs w;
-  w.depth = (float*)take(n * 4);
-  w.xy = (float2*)take(n * 8);
-  w.conic_opac = (float4*)take(n * 16);
-  w.rgb_depth = (float4*)take(n * 16);
-  w.rect = (int4*)take(n * 16);
-  w.tiles = (uint32_t*)take(n * 4);
-  w.offsets = (uint32_t*)take(n * 4);
-  w.clamped = (uint8_t*)take(n);
-  w.keys_a = (uint64_t*)take((size_t)cap * 8);
-  w.keys_b = (uint64_t*)take((size_t)cap * 8);
-  w.vals_a = (uint32_t*)take((size_t)cap * 4);
-  w.vals_b = (uint32_t*)take((size_t)cap * 4);
-  w.ranges = (uint2*)take((size_t)cams * gx * gy * 8);
-  w.n_contrib = (uint32_t*)take((size_t)cams * H * W * 4);
-  w.final_T = (float*)take((size_t)cams * H * W * 4);
-  w.counters = (long long*)take((size_t)(cams + 2) * 8);
-  w.g_mean2d = (float*)take(n * 8);
-  w.g_conic = (float*)take(n * 12);
-  w.g_depth = (float*)take(n * 4);
-  w.g_rgb = (float*)take(n * 12);
-  w.cub_temp = take(cub_bytes);
+  w.depth = c.take<float>(n);
+  w.xy = c.take<float2>(n);
+  w.conic_opac = c.take<float4>(n);
+  w.rgb_depth = c.take<float4>(n);
+  w.rect = c.take<int4>(n);
+  w.tiles = c.take<uint32_t>(n);
+  w.offsets = c.take<uint32_t>(n);
+  w.clamped = c.take<uint8_t>(n);
+  w.keys_a = c.take<uint64_t>(cap);
+  w.keys_b = c.take<uint64_t>(cap);
+  w.vals_a = c.take<uint32_t>(cap);
+  w.vals_b = c.take<uint32_t>(cap);
+  w.ranges = c.take<uint2>((size_t)cams * gx * gy);
+  w.n_contrib = c.take<uint32_t>((size_t)cams * H * W);
+  w.final_T = c.take<float>((size_t)cams * H * W);
+  w.counters = c.take<long long>(cams + 2);
+  w.g_mean2d = c.take<float>(2 * n);
+  w.g_conic = c.take<float>(3 * n);
+  w.g_depth = c.take<float>(n);
+  w.g_rgb = c.take<float>(3 * n);
+  w.cub_temp = c.take<char>(cub_bytes);
   w.cub_bytes = cub_bytes;
   if (ws) *ws = w;
-  return (off + 255) & ~(size_t)255;
+  return c.bytes();
 }
 
 void launch_preprocess(const RasterDev& a, const RasterWs& ws, int32_t* radii, cudaStream_t st);

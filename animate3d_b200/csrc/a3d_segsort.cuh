@@ -3,6 +3,7 @@
 #pragma once
 #include <cub/cub.cuh>
 
+#include "a3d_carve.h"
 #include "a3d_host.cuh"
 
 namespace a3d {
@@ -39,19 +40,5 @@ inline int seg_sort(const uint32_t* keys_in, const uint32_t* vals_in, uint32_t* 
   A3D_LAUNCH_CHECK();
   return A3D_OK;
 }
-
-// Bump allocator over caller-owned scratch (base may be null for a size query); 256-byte aligned pieces.
-struct Carve {
-  char* base;
-  size_t off = 0;
-  template <class T>
-  T* take(size_t count) {
-    off = (off + 255) & ~(size_t)255;
-    T* p = base ? reinterpret_cast<T*>(base + off) : nullptr;
-    off += count * sizeof(T);
-    return p;
-  }
-  size_t bytes() const { return (off + 255) & ~(size_t)255; }
-};
 
 }  // namespace a3d

@@ -61,12 +61,12 @@ def _plane_grad_out(scratch: torch.Tensor, plane: torch.Tensor) -> torch.Tensor:
 
 
 def _backward(lib, a, g_means, g_scales, g_rots, device):
-    """a3d_deform_backward_ex; with torch's deterministic flag set, the fixed-order path and its scratch."""
+    """a3d_deform_backward; with torch's deterministic flag set, the fixed-order path and its scratch."""
     a.deterministic = L.deterministic()
     nbytes = lib.a3d_deform_backward_scratch_bytes(C.byref(a))
     scratch = L.scratch(nbytes, device)
-    L.check(lib.a3d_deform_backward_ex(C.byref(a), C.c_void_p(L.ptr(g_means)), C.c_void_p(L.ptr(g_scales)), C.c_void_p(L.ptr(g_rots)),
-                                       C.c_void_p(L.ptr(scratch)), C.c_size_t(nbytes), L.stream_ptr()))
+    L.check(lib.a3d_deform_backward(C.byref(a), C.c_void_p(L.ptr(g_means)), C.c_void_p(L.ptr(g_scales)), C.c_void_p(L.ptr(g_rots)),
+                                    C.c_void_p(L.ptr(scratch)), C.c_size_t(nbytes), L.stream_ptr()))
 
 
 class _FeatMean(torch.autograd.Function):

@@ -99,7 +99,7 @@ class _RasterizeBatch(torch.autograd.Function):
         global last_num_rendered
         last_num_rendered = total
         _cap_hint[key] = max(int(total * 1.08) + 1024, 1 << 16)   # the radix sort runs over the capacity: keep the slack small
-        ctx.save_for_backward(means3D, scales, rotations, opacities, shs, colors_precomp, cams_t, radii, alpha, ws)
+        ctx.save_for_backward(means3D, scales, rotations, opacities, shs, colors_precomp, cams_t, radii, ws)
         ctx.meta = (meta, cap, nbytes, P, ncam)
         ctx.m2_shape = None if means2D is None else tuple(means2D.shape)
         ctx.num_rendered = counts[:ncam].clone()
@@ -109,7 +109,7 @@ class _RasterizeBatch(torch.autograd.Function):
     @staticmethod
     def backward(ctx, g_color, g_radii, g_depth, g_alpha):
         lib = L.load()
-        means3D, scales, rotations, opacities, shs, colors_precomp, cams_t, radii, alpha, ws = ctx.saved_tensors
+        means3D, scales, rotations, opacities, shs, colors_precomp, cams_t, radii, ws = ctx.saved_tensors
         (H, W, sh_degree, per_cam, scale_modifier, bg), cap, nbytes, P, ncam = ctx.meta
         dev = means3D.device
         g_color = g_color.contiguous().float()
@@ -127,12 +127,12 @@ class _RasterizeBatch(torch.autograd.Function):
         scratch = L.scratch(sbytes, dev)
         global last_backward_scratch_bytes
         last_backward_scratch_bytes = sbytes
-        L.check(lib.a3d_raster_backward_ex(C.byref(args), C.c_void_p(g_color.data_ptr()), C.c_void_p(L.ptr(g_depth)),
-                                           C.c_void_p(L.ptr(g_alpha)), C.c_void_p(alpha.data_ptr()), C.c_void_p(radii.data_ptr()),
-                                           C.c_void_p(ws.data_ptr()), C.c_size_t(nbytes), C.c_int64(cap), C.c_void_p(dm.data_ptr()),
-                                           C.c_void_p(ds.data_ptr()), C.c_void_p(dr.data_ptr()), C.c_void_p(do.data_ptr()),
-                                           C.c_void_p(L.ptr(dc)), C.c_void_p(L.ptr(dsh)), C.c_void_p(dm2.data_ptr()),
-                                           C.c_void_p(L.ptr(scratch)), C.c_size_t(sbytes), L.stream_ptr()))
+        L.check(lib.a3d_raster_backward(C.byref(args), C.c_void_p(g_color.data_ptr()), C.c_void_p(L.ptr(g_depth)),
+                                        C.c_void_p(L.ptr(g_alpha)), C.c_void_p(radii.data_ptr()), C.c_void_p(ws.data_ptr()),
+                                        C.c_size_t(nbytes), C.c_int64(cap), C.c_void_p(dm.data_ptr()), C.c_void_p(ds.data_ptr()),
+                                        C.c_void_p(dr.data_ptr()), C.c_void_p(do.data_ptr()), C.c_void_p(L.ptr(dc)),
+                                        C.c_void_p(L.ptr(dsh)), C.c_void_p(dm2.data_ptr()), C.c_void_p(L.ptr(scratch)),
+                                        C.c_size_t(sbytes), L.stream_ptr()))
         g_m2 = None if ctx.m2_shape is None else dm2.reshape(ctx.m2_shape)   # `viewspace_points` gradient, NDC units
         return dm, g_m2, ds, dr, do, dsh, dc, None, None
 

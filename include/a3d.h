@@ -200,7 +200,7 @@ typedef struct a3d_raster_args {
   float scale_modifier;
   float bg[3];
   int deterministic;         /* 1: the backward sums every gradient in a fixed order (bit-reproducible; needs the scratch of
-                                a3d_raster_backward_ex); 0: float atomics.  The forward is deterministic either way. */
+                                a3d_raster_backward_scratch_bytes); 0: float atomics.  The forward is deterministic either way. */
 } a3d_raster_args;
 
 /* workspace bytes for a forward with at most max_rendered (tile,gaussian) pairs per camera */
@@ -210,28 +210,22 @@ size_t a3d_raster_workspace_bytes(int P, int H, int W, int num_cams, int64_t max
 int a3d_raster_forward(const a3d_raster_args* args, float* color, float* depth, float* alpha, int32_t* radii,
                        void* workspace, size_t workspace_bytes, int64_t max_rendered, int64_t* num_rendered_host,
                        void* stream);
-/* backward: grads w.r.t. means3D/scales/rotations ([cams or 1][P,*], accumulated over cameras when geometry is shared),
- * opacities [P,1], colors/shs, means2D [cams,P,3]. Needs the workspace of the matching forward untouched. */
-int a3d_raster_backward(const a3d_raster_args* args, const float* dL_dcolor, const float* dL_ddepth,
-                        const float* dL_dalpha, const float* alpha, const int32_t* radii, void* workspace,
-                        size_t workspace_bytes, int64_t max_rendered, float* dL_dmeans3D, float* dL_dscales,
-                        float* dL_drotations, float* dL_dopacity, float* dL_dcolors, float* dL_dshs,
-                        float* dL_dmeans2D, void* stream);
-/* Scratch bytes a3d_raster_backward_ex needs: 0 when args->deterministic is 0, else 40 B per (tile, gaussian) pair slot of
+/* Scratch bytes a3d_raster_backward needs: 0 when args->deterministic is 0, else 40 B per (tile, gaussian) pair slot of
  * max_rendered plus 4 B per (camera, gaussian). */
 size_t a3d_raster_backward_scratch_bytes(const a3d_raster_args* args, int64_t max_rendered);
-/* a3d_raster_backward with caller-owned scratch (scratch may be NULL when the size query returned 0).  With
- * args->deterministic set (torch.use_deterministic_algorithms of the caller), the render backward reduces the 8 warp
- * partials of a list entry in warp order and stores one 10-float record per (camera, tile, gaussian) pair in the pair's
- * pre-sort slot; a per-(camera, gaussian) kernel sums its slots in slot (= tile) order, and a per-gaussian kernel pushes
- * every camera's gradients through the projection, summing cameras in camera order.  Same reference interface as
- * a3d_raster_backward (rasterize_gaussians_backward, which accumulates with float atomics).  a3d_raster_backward itself
- * rejects deterministic = 1. */
-int a3d_raster_backward_ex(const a3d_raster_args* args, const float* dL_dcolor, const float* dL_ddepth,
-                           const float* dL_dalpha, const float* alpha, const int32_t* radii, void* workspace,
-                           size_t workspace_bytes, int64_t max_rendered, float* dL_dmeans3D, float* dL_dscales,
-                           float* dL_drotations, float* dL_dopacity, float* dL_dcolors, float* dL_dshs,
-                           float* dL_dmeans2D, void* scratch, size_t scratch_bytes, void* stream);
+/* backward: grads w.r.t. means3D/scales/rotations ([cams or 1][P,*], accumulated over cameras when geometry is shared),
+ * opacities [P,1], colors/shs, means2D [cams,P,3]. Needs the workspace of the matching forward untouched, and caller-owned
+ * scratch of a3d_raster_backward_scratch_bytes (NULL when that returned 0).  With args->deterministic 0 the gradients are
+ * accumulated with float atomics, like rasterize_gaussians_backward.  With args->deterministic set
+ * (torch.use_deterministic_algorithms of the caller), the render backward reduces the 8 warp partials of a list entry in
+ * warp order and stores one 10-float record per (camera, tile, gaussian) pair in the pair's pre-sort slot; a
+ * per-(camera, gaussian) kernel sums its slots in slot (= tile) order, and a per-gaussian kernel pushes every camera's
+ * gradients through the projection, summing cameras in camera order. */
+int a3d_raster_backward(const a3d_raster_args* args, const float* dL_dcolor, const float* dL_ddepth,
+                        const float* dL_dalpha, const int32_t* radii, void* workspace, size_t workspace_bytes,
+                        int64_t max_rendered, float* dL_dmeans3D, float* dL_dscales, float* dL_drotations,
+                        float* dL_dopacity, float* dL_dcolors, float* dL_dshs, float* dL_dmeans2D, void* scratch,
+                        size_t scratch_bytes, void* stream);
 /* debug/parity taps of the binning stage for one camera: sorted keys [n] uint64, point_list [n] uint32, ranges [tiles] uint2 */
 int a3d_raster_binning_tap(const void* workspace, int P, int H, int W, int num_cams, int64_t max_rendered, int cam,
                            uint64_t* keys_out, uint32_t* point_list_out, uint32_t* ranges_out, void* stream);
@@ -265,7 +259,7 @@ typedef struct a3d_deform_args {
   const float* rot_base;      /* [T,P,4] per-frame base quaternions, replace `rotation` (forward and backward) */
   float* grad_rot_base;       /* backward: receives dL/d rot_base, [T,P,4] */
   const float* grad_featmean; /* backward: dL/d (per-frame mean feature), [T, num_scales*channels]; folded into grad_planes */
-  int deterministic;          /* backward: 1 = fixed summation order (needs the scratch of a3d_deform_backward_ex), 0 = atomics */
+  int deterministic;          /* backward: 1 = fixed summation order (needs the scratch of a3d_deform_backward_scratch_bytes), 0 = atomics */
 } a3d_deform_args;
 
 int a3d_deform_forward(const a3d_deform_args* args, float* means, float* scales, float* rotations, void* stream);
@@ -273,44 +267,41 @@ int a3d_deform_forward(const a3d_deform_args* args, float* means, float* scales,
  * featmean [T, num_scales*channels].  Always summed in a fixed order (a cluster of 8 CTAs per frame, reduced through
  * distributed shared memory in rank order), so it is bit-reproducible and needs no scratch. */
 int a3d_deform_featmean(const a3d_deform_args* args, float* featmean, void* stream);
-/* Accumulates into args->grad_w1 / grad_w2 ([out, in] like the weights) and args->grad_planes.  grad_planes[i] is a
- * CHANNEL-LAST scratch [plane_h[i], plane_w[i], channels] (zero it first; 16-byte aligned): the 16 channels of a texel are
- * written with vector reductions; transpose it into the [1, channels, H, W] parameter gradient afterwards. */
-int a3d_deform_backward(const a3d_deform_args* args, const float* dL_dmeans, const float* dL_dscales, const float* dL_drotations,
-                        void* stream);
-/* Scratch bytes a3d_deform_backward_ex needs: 0 when args->deterministic is 0.  Otherwise 768 B per (frame, gaussian) for
+/* Scratch bytes a3d_deform_backward needs: 0 when args->deterministic is 0.  Otherwise 768 B per (frame, gaussian) for
  * the stored upstream plane factors (0.61 GB at T = 16, P = 50 000), 16 B per (frame, gaussian) of sort buffers and the
  * per-CTA weight-gradient partials. */
 size_t a3d_deform_backward_scratch_bytes(const a3d_deform_args* args);
-/* a3d_deform_backward with caller-owned scratch (NULL when the size query returned 0); same reference interface (the autograd
- * backward of gaussian_4d.py:450-548, whose grid_sample backward scatters with float atomics).  With args->deterministic set:
- * MLP weight gradients are per-CTA partials reduced in CTA order; plane gradients are a gather: per plane, the (frame,
- * gaussian) points are stably radix-sorted by their lower-left cell, and every texel sums the stored factors (d loss / d
- * feature x the other planes' samples, grad_featmean folded in) of the points of its <= 4 adjacent cells in sorted order. */
-int a3d_deform_backward_ex(const a3d_deform_args* args, const float* dL_dmeans, const float* dL_dscales,
-                           const float* dL_drotations, void* scratch, size_t scratch_bytes, void* stream);
+/* The autograd backward of gaussian_4d.py:450-548.  Accumulates into args->grad_w1 / grad_w2 ([out, in] like the weights)
+ * and args->grad_planes.  grad_planes[i] is a CHANNEL-LAST scratch [plane_h[i], plane_w[i], channels] (zero it first;
+ * 16-byte aligned): transpose it into the [1, channels, H, W] parameter gradient afterwards.  scratch: caller-owned, of
+ * a3d_deform_backward_scratch_bytes (NULL when that returned 0).  With args->deterministic 0 the texel gradients are written
+ * with vector float atomics, like the reference's grid_sample backward.  With args->deterministic set: MLP weight gradients
+ * are per-CTA partials reduced in CTA order; plane gradients are a gather: per plane, the (frame, gaussian) points are stably
+ * radix-sorted by their lower-left cell, and every texel sums the stored factors (d loss / d feature x the other planes'
+ * samples, grad_featmean folded in) of the points of its <= 4 adjacent cells in sorted order. */
+int a3d_deform_backward(const a3d_deform_args* args, const float* dL_dmeans, const float* dL_dscales, const float* dL_drotations,
+                        void* scratch, size_t scratch_bytes, void* stream);
 
 /* ---------------------------------------------------------------- ARAP regulariser (SURVEY 8f-3) -------------- */
 /* K nearest neighbours of every point among the same points, self excluded, squared distances ascending, ties by index:
  * pytorch3d.ops.knn_points(p, p, K=K+1)[..., 1:] as used by cal_connectivity_from_points
  * (custom/threestudio-animate3d/systems/util.py:79-82).  nbr [n,K] int32, dist2 [n,K]; K <= 12. */
 int a3d_knn_graph(const float* points, int n, int K, int32_t* nbr, float* dist2, void* stream);
-/* cal_arap_error (util.py:183-215) with estimate_rotation (138-173) fused, all frames in one launch:
+/* cal_arap_error (util.py:183-215) with estimate_rotation (138-173) fused, all frames at once:
  *   err = sum_{t>=1} sum_{i in sample} sum_n w[i,n] | e_in(t) - R_i(t) e_in(0) |^2,   e_in(t) = x_t[i] - x_t[nbr[i,n]],
  * R_i(t) = the weighted Procrustes rotation of the node's frame-0 edges onto its frame-t edges (no gradient through R).
  * nodes [Nt,Nv,3]; nbr [Nv,K] (-1 = no edge); weight [Nv,K] or NULL (1 on existing edges, the reference's call);
- * sample [Ns] node indices or NULL (all nodes).  err: device scalar; grad [Nt,Nv,3] = d err / d nodes or NULL.  Both are
- * zeroed here.  Checked on the CPU (tests/test_arap_cpu.py) and on the GPU against the reference goldens (tests/test_arap_gpu.py). */
+ * sample [Ns] node indices or NULL (all nodes).  err: device scalar; grad [Nt,Nv,3] = d err / d nodes or NULL; both are
+ * overwritten.  scratch: caller-owned, of a3d_arap_scratch_bytes (NULL when that returned 0).  With deterministic 0 one
+ * kernel accumulates energy and gradient with float atomics.  With deterministic 1 every sum runs in a fixed order: the
+ * energy from per-(frame, sample) partials reduced by one CTA; the gradient from per-(frame, sample, edge) 3-vector records
+ * gathered per node after a stable sort of the (target node, record) pairs, so repeated samples add in sample order and the
+ * frame-0 gradient adds frames in order.  Checked on the CPU (tests/test_arap_cpu.py) and on the GPU against the reference
+ * goldens (tests/test_arap_gpu.py). */
 int a3d_arap(const float* nodes, int Nt, int Nv, const int32_t* nbr, int K, const float* weight, const int32_t* sample, int Ns,
-             float* err, float* grad, void* stream);
-/* Scratch bytes of a3d_arap_deterministic for the same sizes (Ns of a NULL sample = Nv). */
-size_t a3d_arap_deterministic_scratch_bytes(int Nt, int Nv, int K, int Ns);
-/* a3d_arap (cal_arap_error, util.py:183-215) with every sum in a fixed order: the energy from per-(frame, sample) partials
- * reduced by one CTA; the gradient from per-(frame, sample, edge) 3-vector records gathered per node after a stable sort of
- * the (target node, record) pairs, so repeated samples add in sample order and the frame-0 gradient adds frames in order. */
-int a3d_arap_deterministic(const float* nodes, int Nt, int Nv, const int32_t* nbr, int K, const float* weight,
-                           const int32_t* sample, int Ns, float* err, float* grad, void* scratch, size_t scratch_bytes,
-                           void* stream);
+             int deterministic, float* err, float* grad, void* scratch, size_t scratch_bytes, void* stream);
+/* Scratch bytes a3d_arap needs for the same sizes (Ns of a NULL sample = Nv): 0 when deterministic is 0. */
+size_t a3d_arap_scratch_bytes(int Nt, int Nv, int K, int Ns, int deterministic);
 
 /* debug hook: a device uint64 counter the tensor-core attention kernel bumps once per (warp, key step) that takes the
    lazy-rescale branch of the single-pass softmax (NULL = off; tests use it to prove adversarial inputs reach that branch). */

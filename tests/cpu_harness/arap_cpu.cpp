@@ -1,5 +1,5 @@
-// CPU harness (TEST INFRASTRUCTURE) around animate3d_b200/csrc/a3d_arap_math.h: the exact __host__ __device__ arithmetic of
-// the ARAP CUDA kernel, driven serially so it can be checked against the reference goldens without a GPU.
+// CPU harness (TEST INFRASTRUCTURE) around animate3d_b200/csrc/a3d_arap_math.h: the exact __host__ __device__ edge gather and
+// arithmetic of the ARAP CUDA kernels, driven serially so they can be checked against the reference goldens without a GPU.
 // Build: g++ -O1 -shared -fPIC arap_cpu.cpp -o arap_cpu.so   (done by tests/test_arap_cpu.py)
 #include "../../animate3d_b200/csrc/a3d_arap_math.h"
 
@@ -7,7 +7,7 @@ using namespace a3d;
 
 extern "C" {
 
-// nodes [Nt,Nv,3]; nbr [Nv,K] (-1 = absent); weight [Nv,K]; sample [Ns] node indices.  grad [Nt,Nv,3] must be zeroed.
+// nodes [Nt,Nv,3]; nbr [Nv,K] (-1 = absent); weight [Nv,K] or NULL (1 on existing edges); sample [Ns] node indices.  grad [Nt,Nv,3] must be zeroed.
 double arap_cpu(const float* nodes, int Nt, int Nv, const int* nbr, int K, const float* weight, const int* sample, int Ns,
                 float* grad) {
   double total = 0.0;
@@ -16,15 +16,7 @@ double arap_cpu(const float* nodes, int Nt, int Nv, const int* nbr, int K, const
       const int i = sample[si];
       float e0[kArapMaxK][3], et[kArapMaxK][3], g0[kArapMaxK][3], gt[kArapMaxK][3], w[kArapMaxK];
       bool valid[kArapMaxK];
-      for (int n = 0; n < K; ++n) {
-        const int j = nbr[i * K + n];
-        valid[n] = j >= 0;
-        w[n] = weight[i * K + n];
-        for (int c = 0; c < 3; ++c) {
-          e0[n][c] = valid[n] ? nodes[(0 * Nv + i) * 3 + c] - nodes[(0 * Nv + j) * 3 + c] : 0.f;
-          et[n][c] = valid[n] ? nodes[((long)t * Nv + i) * 3 + c] - nodes[((long)t * Nv + j) * 3 + c] : 0.f;
-        }
-      }
+      arap_gather(nodes, Nv, nbr, K, weight, i, t, e0, et, w, valid);
       total += arap_node(K, e0, et, valid, w, gt, g0);
       for (int n = 0; n < K; ++n) {
         if (!valid[n]) continue;

@@ -27,7 +27,7 @@ def test_library_exports_every_declared_symbol():
     lib = _lib.load(require_gpu=False)
     missing = [s for s in declared_symbols() if not hasattr(lib, s)]
     assert not missing, f"declared in include/a3d.h but not exported by liba3d.so: {missing}"
-    assert lib.a3d_version() == 100
+    assert lib.a3d_version() == 101
 
 
 def test_hot_path_fails_loudly_without_gpu():

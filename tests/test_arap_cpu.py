@@ -1,6 +1,7 @@
 """The ARAP arithmetic shared with the CUDA kernel (animate3d_b200/csrc/a3d_arap_math.h), driven serially on the CPU through
 tests/cpu_harness/arap_cpu.cpp, against the reference goldens (ref_arap.pt: outputs of systems/util.py's own functions) and the
-oracle.  CPU-only; the GPU wrapper (a3d_arap.cu) adds indexing and atomics around exactly this code."""
+oracle.  CPU-only; the harness runs the kernels' own edge gather (arap_gather) and arap_node, and the GPU wrapper (a3d_arap.cu)
+adds only the sample indexing and the gradient scatter around them."""
 import ctypes as C
 import os
 import subprocess
