@@ -1,7 +1,8 @@
 """nn.Module surface of the MV motion UNet (SURVEY 8b "UNet module" and "diffusers attention-processor protocol").
 
-The engine never executes these modules: it repacks their parameters into fused fp16 operands (`unet.py::_prepare`).  They
-exist so that code written against the reference keeps working unchanged:
+The engine never executes these modules: it repacks their parameters into fused fp16 operands (`unet.py::_prepare`, and
+`processor_exec.pack_*` for the attention processors).  They exist so that code written against the reference keeps working
+unchanged:
 
   * `state_dict()` / `load_state_dict()` with the reference's key names (diffusers 0.28 naming, processors' parameters under
     `<attn>.processor.*`), the 726-missing rule of inference.py:219-223
@@ -64,9 +65,9 @@ class _Processor(Node):
         raise NotImplementedError
 
     def __call__(self, attn, hidden_states, encoder_hidden_states=None, attention_mask=None, temb=None, *args, **kwargs):
-        """diffusers attention-processor protocol (attention_processor.py:39-48, 169-178, 325-334, 541-550).  Inside the engine
-        the processor's arithmetic is fused into `MVUNetMotionModel.forward`; called stand-alone it runs the same kernels
-        through `animate3d_b200.processor_exec`."""
+        """diffusers attention-processor protocol (attention_processor.py:39-48, 169-178, 325-334, 541-550).  Runs the packer and
+        launch stages of `animate3d_b200.processor_exec` that `MVUNetMotionModel.forward` runs for every attention layer, on
+        fresh tensors instead of the UNet's activation arena."""
         from . import processor_exec
         return processor_exec.run(self, attn, hidden_states, encoder_hidden_states, attention_mask, temb, **kwargs)
 

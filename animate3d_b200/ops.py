@@ -10,6 +10,15 @@ from . import _lib as L
 
 HALF = torch.float16
 
+launches = 0     # kernels enqueued through these wrappers since import; a forward's count is the change over it
+
+
+def _enqueued(rc: int, kernels: int = 1) -> None:
+    """Raise on an error code, else count the kernels the entry point enqueued."""
+    global launches
+    L.check(rc)
+    launches += kernels
+
 
 def _chk16(*ts):
     for t in ts:
@@ -47,7 +56,7 @@ def gemm(A: torch.Tensor, B: torch.Tensor, out: torch.Tensor, *, M: int, N: int,
     a.geglu, a.out_f32 = int(geglu), int(out_f32)
     a.perm_a, a.perm_b = perm
     a.impl = impl
-    L.check(lib.a3d_gemm(C.byref(a), L.stream_ptr()))
+    _enqueued(lib.a3d_gemm(C.byref(a), L.stream_ptr()))
     return out
 
 
@@ -71,14 +80,14 @@ def attention(q: L.View5, k: L.View5, v: L.View5, out: torch.Tensor, ostrides, *
     a.heads, a.d, a.scale = heads, d, scale
     a.kv_div, a.kv_i3_zero = kv_div, int(kv_i3_zero)
     a.accumulate, a.out_scale, a.impl = int(accumulate), out_scale, impl
-    L.check(lib.a3d_attention(C.byref(a), L.stream_ptr()))
+    _enqueued(lib.a3d_attention(C.byref(a), L.stream_ptr()))
 
 
 def temporal_attn(qkv: torch.Tensor, out: torch.Tensor, pixels: int, frames: int, heads: int, d: int, scale: float,
                   ldo: int = 0, out_col_offset: int = 0):
     """out rows have stride `ldo` halves (0 = heads*d) and start at column `out_col_offset` of `out`."""
     lib = L.load()
-    L.check(lib.a3d_temporal_attn(C.c_void_p(qkv.data_ptr()), C.c_void_p(out.data_ptr() + 2 * out_col_offset), C.c_int64(pixels),
+    _enqueued(lib.a3d_temporal_attn(C.c_void_p(qkv.data_ptr()), C.c_void_p(out.data_ptr() + 2 * out_col_offset), C.c_int64(pixels),
                                   frames, heads, d, C.c_float(scale), C.c_int64(ldo), L.stream_ptr()))
 
 
@@ -91,77 +100,77 @@ def group_norm_ws_floats(samples: int, rows_per_sample: int, c: int, groups: int
 def group_norm(x1, c1, x2, c2, gamma, beta, y, samples, rows_per_sample, groups, eps, silu, ws_stats, perm=(0, 0)):
     lib = L.load()
     assert ws_stats.numel() >= group_norm_ws_floats(samples, rows_per_sample, c1 + (c2 if x2 is not None else 0), groups)
-    L.check(lib.a3d_group_norm(C.c_void_p(x1.data_ptr()), c1, C.c_void_p(L.ptr(x2)), c2, C.c_void_p(gamma.data_ptr()),
+    _enqueued(lib.a3d_group_norm(C.c_void_p(x1.data_ptr()), c1, C.c_void_p(L.ptr(x2)), c2, C.c_void_p(gamma.data_ptr()),
                                C.c_void_p(beta.data_ptr()), C.c_void_p(y.data_ptr()), C.c_int64(samples),
                                C.c_int64(rows_per_sample), groups, C.c_float(eps), int(silu), C.c_int64(perm[0]),
-                               C.c_int64(perm[1]), C.c_void_p(ws_stats.data_ptr()), L.stream_ptr()))
+                               C.c_int64(perm[1]), C.c_void_p(ws_stats.data_ptr()), L.stream_ptr()), 3)
     return y
 
 
 def group_norm_backward(x, c, gamma, beta, fwd_stats, dy, dx, samples, rows_per_sample, groups, silu, ws):
     lib = L.load()
-    L.check(lib.a3d_group_norm_backward(C.c_void_p(x.data_ptr()), c, C.c_void_p(gamma.data_ptr()), C.c_void_p(beta.data_ptr()),
+    _enqueued(lib.a3d_group_norm_backward(C.c_void_p(x.data_ptr()), c, C.c_void_p(gamma.data_ptr()), C.c_void_p(beta.data_ptr()),
                                         C.c_void_p(fwd_stats.data_ptr()), C.c_void_p(dy.data_ptr()), C.c_void_p(dx.data_ptr()),
                                         C.c_int64(samples), C.c_int64(rows_per_sample), groups, int(silu), C.c_void_p(ws.data_ptr()),
-                                        L.stream_ptr()))
+                                        L.stream_ptr()), 3)
     return dx
 
 
 def layer_norm(x, gamma, beta, y, rows, c, eps=1e-5):
     lib = L.load()
-    L.check(lib.a3d_layer_norm(C.c_void_p(x.data_ptr()), C.c_void_p(gamma.data_ptr()), C.c_void_p(beta.data_ptr()),
+    _enqueued(lib.a3d_layer_norm(C.c_void_p(x.data_ptr()), C.c_void_p(gamma.data_ptr()), C.c_void_p(beta.data_ptr()),
                                C.c_void_p(y.data_ptr()), C.c_int64(rows), c, C.c_float(eps), L.stream_ptr()))
     return y
 
 
 def upsample2x(x, y, n, h, w, c):
     lib = L.load()
-    L.check(lib.a3d_upsample2x(C.c_void_p(x.data_ptr()), C.c_void_p(y.data_ptr()), C.c_int64(n), h, w, c, L.stream_ptr()))
+    _enqueued(lib.a3d_upsample2x(C.c_void_p(x.data_ptr()), C.c_void_p(y.data_ptr()), C.c_int64(n), h, w, c, L.stream_ptr()))
     return y
 
 
 def silu_rows(x, y, rows, c, rep):
     lib = L.load()
-    L.check(lib.a3d_silu_rows(C.c_void_p(x.data_ptr()), C.c_void_p(y.data_ptr()), C.c_int64(rows), c, rep, L.stream_ptr()))
+    _enqueued(lib.a3d_silu_rows(C.c_void_p(x.data_ptr()), C.c_void_p(y.data_ptr()), C.c_int64(rows), c, rep, L.stream_ptr()))
     return y
 
 
 def conv_in(sample, w, b, y, bn, cin, f, h, wd, cout):
     lib = L.load()
-    L.check(lib.a3d_conv_in(C.c_void_p(sample.data_ptr()), C.c_void_p(w.data_ptr()), C.c_void_p(b.data_ptr()),
+    _enqueued(lib.a3d_conv_in(C.c_void_p(sample.data_ptr()), C.c_void_p(w.data_ptr()), C.c_void_p(b.data_ptr()),
                             C.c_void_p(y.data_ptr()), bn, cin, f, h, wd, cout, L.stream_ptr()))
     return y
 
 
 def conv_out(x, w, b, y, bn, cin, f, h, wd, cout):
     lib = L.load()
-    L.check(lib.a3d_conv_out(C.c_void_p(x.data_ptr()), C.c_void_p(w.data_ptr()), C.c_void_p(b.data_ptr()),
+    _enqueued(lib.a3d_conv_out(C.c_void_p(x.data_ptr()), C.c_void_p(w.data_ptr()), C.c_void_p(b.data_ptr()),
                              C.c_void_p(y.data_ptr()), bn, cin, f, h, wd, cout, L.stream_ptr()))
     return y
 
 
 def timestep_proj(t, out, rows, half):
     lib = L.load()
-    L.check(lib.a3d_timestep_proj(C.c_void_p(t.data_ptr()), C.c_void_p(out.data_ptr()), rows, half, L.stream_ptr()))
+    _enqueued(lib.a3d_timestep_proj(C.c_void_p(t.data_ptr()), C.c_void_p(out.data_ptr()), rows, half, L.stream_ptr()))
     return out
 
 
 def linear_f32(x, w, b, y, m, n, k, act_in=0, accumulate=False):
     lib = L.load()
-    L.check(lib.a3d_linear_f32(C.c_void_p(x.data_ptr()), C.c_void_p(w.data_ptr()), C.c_void_p(L.ptr(b)),
+    _enqueued(lib.a3d_linear_f32(C.c_void_p(x.data_ptr()), C.c_void_p(w.data_ptr()), C.c_void_p(L.ptr(b)),
                                C.c_void_p(y.data_ptr()), m, n, k, act_in, int(accumulate), L.stream_ptr()))
     return y
 
 
 def cast_f32_f16(x, y):
     lib = L.load()
-    L.check(lib.a3d_cast_f32_f16(C.c_void_p(x.data_ptr()), C.c_void_p(y.data_ptr()), C.c_int64(x.numel()), L.stream_ptr()))
+    _enqueued(lib.a3d_cast_f32_f16(C.c_void_p(x.data_ptr()), C.c_void_p(y.data_ptr()), C.c_int64(x.numel()), L.stream_ptr()))
     return y
 
 
 def ddim_cfg_step(latents, noise_pred, first_frame, bn, c, f, hw, guidance, alpha_t, alpha_prev, uncond_first=True):
     lib = L.load()
-    L.check(lib.a3d_ddim_cfg_step(C.c_void_p(latents.data_ptr()), C.c_void_p(noise_pred.data_ptr()),
+    _enqueued(lib.a3d_ddim_cfg_step(C.c_void_p(latents.data_ptr()), C.c_void_p(noise_pred.data_ptr()),
                                   C.c_void_p(L.ptr(first_frame)), bn, c, f, hw, C.c_float(guidance), C.c_float(alpha_t),
                                   C.c_float(alpha_prev), int(uncond_first), L.stream_ptr()))
     return latents

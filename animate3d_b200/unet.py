@@ -20,61 +20,22 @@ Torch is used for device memory and the stream only; there is no fallback path.
 """
 from __future__ import annotations
 
-import math
 from dataclasses import dataclass
-from typing import Dict, List, Optional, Tuple
+from typing import Dict, List, Optional
 
 import torch
 
 from . import _lib as L
 from . import ops
+from . import processor_exec as P
 from .modules import attn_processors_of, build_tree
-from .unet_config import UNetConfig, key_plan, sinusoidal_pe, up_plan
-
-HALF = torch.float16
+from .processor_exec import HALF, _Lin, linear
+from .unet_config import UNetConfig, key_plan, up_plan
 
 
 @dataclass
 class UNet3DConditionOutput:
     sample: torch.Tensor
-
-
-def _sine_pos_enc_2d(num_feats: int, h: int, w: int, temperature=10000, scale=2 * math.pi, eps=1e-6) -> torch.Tensor:
-    """[h*w, 2*num_feats] table of SinePositionalEncoding2D(num_feats, normalize=True) (animatediff/models/embeddings.py:58-96)."""
-    y = torch.arange(1, h + 1, dtype=torch.float32)[:, None].expand(h, w)
-    x = torch.arange(1, w + 1, dtype=torch.float32)[None, :].expand(h, w)
-    y = y / (y[-1:, :] + eps) * scale
-    x = x / (x[:, -1:] + eps) * scale
-    dim_t = torch.arange(num_feats, dtype=torch.float32)
-    dim_t = temperature ** (2 * (dim_t // 2) / num_feats)
-    px = x[:, :, None] / dim_t
-    py = y[:, :, None] / dim_t
-    px = torch.stack((px[:, :, 0::2].sin(), px[:, :, 1::2].cos()), dim=3).reshape(h, w, -1)
-    py = torch.stack((py[:, :, 0::2].sin(), py[:, :, 1::2].cos()), dim=3).reshape(h, w, -1)
-    return torch.cat((py, px), dim=2).reshape(h * w, -1)
-
-
-def _dqk(d):
-    return (d + 15) // 16 * 16
-
-
-def _dv(d):
-    return (d + 1 + 15) // 16 * 16
-
-
-def _pad_heads(w: torch.Tensor, heads: int, d: int, dp: int) -> torch.Tensor:
-    """[heads*d, K] -> [heads*dp, K] with zero rows after each head's d rows."""
-    k = w.shape[1]
-    out = torch.zeros(heads, dp, k, dtype=w.dtype, device=w.device)
-    out[:, :d] = w.reshape(heads, d, k)
-    return out.reshape(heads * dp, k)
-
-
-def _ones_bias(heads: int, d: int, dv: int, offset: int, total: int, device) -> torch.Tensor:
-    b = torch.zeros(total, dtype=torch.float32, device=device)
-    idx = offset + torch.arange(heads, device=device) * dv + d
-    b[idx] = 1.0
-    return b
 
 
 def _geglu_interleave(w: torch.Tensor) -> torch.Tensor:
@@ -83,23 +44,6 @@ def _geglu_interleave(w: torch.Tensor) -> torch.Tensor:
     u, g = w[:half], w[half:]
     rest = w.shape[1:]
     return torch.stack([u.reshape(half // 32, 32, *rest), g.reshape(half // 32, 32, *rest)], dim=1).reshape(w.shape)
-
-
-class _Lin:
-    """fp16 weight [N, K] + fp32 bias on device."""
-    __slots__ = ("w", "b", "n", "k")
-
-    def __init__(self, w: torch.Tensor, b: Optional[torch.Tensor], device):
-        self.w = w.to(device=device, dtype=HALF).contiguous()
-        self.b = None if b is None else b.to(device=device, dtype=torch.float32).contiguous()
-        self.n, self.k = self.w.shape
-
-    def rows(self, a: int, b: int) -> "_Lin":
-        """Row slice [a, b) of the weight (and bias) without copying -- used to split a fused projection."""
-        o = object.__new__(_Lin)
-        o.w, o.b = self.w[a:b], None if self.b is None else self.b[a:b]
-        o.n, o.k = b - a, self.k
-        return o
 
 
 class MVUNetMotionModel(torch.nn.Module):
@@ -133,9 +77,7 @@ class MVUNetMotionModel(torch.nn.Module):
         # View-sharded forwards run eagerly: capturing the asynchronous NCCL all-gathers of torch 2.11 / NCCL 2.28 in a CUDA graph
         # deadlocks on this stack; the kernels between two gathers are long enough for the launch stream to stay ahead.
         self.use_cuda_graph = view_group is None
-        self.gemm_impl = L.IMPL_AUTO
-        self.attn_impl = L.IMPL_AUTO
-        self.launches = 0            # kernel launches issued by the last eager run (bench's gpu_launches claim)
+        self.launches_per_forward = 0   # kernels enqueued by the last eager run (bench's gpu_launches claim)
         self.collectives = 0         # view-sharded mode: K|V all-gathers issued by the last eager run and their payload
         self.collective_bytes = 0
         self.comm_enabled = True     # False = skip the all-gathers (timing only: measures the compute of the sharded forward)
@@ -311,7 +253,6 @@ class MVUNetMotionModel(torch.nn.Module):
             raise KeyError(f"cannot run: {len(miss)} weights missing, e.g. {miss[:3]}")
         sd = {k: v.detach() for k, v in torch.nn.Module.state_dict(self).items()}
         W: Dict[str, object] = {}
-        heads = cfg.num_attention_heads
         f32 = lambda k: sd[k].to(dev, torch.float32).contiguous()
 
         def conv3(p):
@@ -350,66 +291,33 @@ class MVUNetMotionModel(torch.nn.Module):
         self._kv_off = 0
 
         def transformer2d(p, c):
-            d = c // heads
-            dqk, dv = _dqk(d), _dv(d)
             tb = f"{p}.transformer_blocks.0"
-            t = {"c": c, "d": d, "norm": (f32(f"{p}.norm.weight"), f32(f"{p}.norm.bias")),
-                 "proj_in": conv1(f"{p}.proj_in"), "proj_out": conv1(f"{p}.proj_out")}
+            node = self.get_submodule(tb)
+            t = {"c": c, "norm": (f32(f"{p}.norm.weight"), f32(f"{p}.norm.bias")),
+                 "proj_in": conv1(f"{p}.proj_in"), "proj_out": conv1(f"{p}.proj_out"),
+                 "attn1": P.pack_mv_i2v(node.attn1.processor, node.attn1, dev),
+                 "attn2": P.pack_ip_adapter(node.attn2.processor, node.attn2, dev)}
             for i in (1, 2, 3):
                 t[f"ln{i}"] = (f32(f"{tb}.norm{i}.weight"), f32(f"{tb}.norm{i}.bias"))
-            a1 = f"{tb}.attn1"
-            wq = _pad_heads(sd[f"{a1}.to_q.weight"], heads, d, dqk)
-            wqi = _pad_heads(sd[f"{a1}.processor.to_q_i2v.weight"], heads, d, dqk)
-            wk = _pad_heads(sd[f"{a1}.to_k.weight"], heads, d, dqk)
-            wv = _pad_heads(sd[f"{a1}.to_v.weight"], heads, d, dv)
-            wqkv = torch.cat([wq, wqi, wk, wv], 0)
-            t["qkv"] = _Lin(wqkv, _ones_bias(heads, d, dv, 3 * heads * dqk, wqkv.shape[0], "cpu"), dev)
-            # to_out(O1 + to_out_i2v(O2)) (attention_processor.py:423-431) is ONE GEMM over [O1 | O2] with K = 2C:
-            #   [O1 | O2] [W_out | W_out W_i2v]^T + (b_out + W_out b_i2v)   -- products formed in fp32, rounded to fp16 once
-            w_out, b_out = sd[f"{a1}.to_out.0.weight"].float(), sd[f"{a1}.to_out.0.bias"].float()
-            w_i2v, b_i2v = sd[f"{a1}.processor.to_out_i2v.weight"].float(), sd[f"{a1}.processor.to_out_i2v.bias"].float()
-            t["out1"] = _Lin(torch.cat([w_out, w_out @ w_i2v], 1), b_out + w_out @ b_i2v, dev)
-            a2 = f"{tb}.attn2"
-            t["q2"] = _Lin(_pad_heads(sd[f"{a2}.to_q.weight"], heads, d, dqk), None, dev)
-            t["out2"] = lin(f"{a2}.to_out.0")
-            # text / ip K,V projections of all spatial transformers are two GEMMs (one per token source)
-            wkv = torch.cat([_pad_heads(sd[f"{a2}.to_k.weight"], heads, d, dqk), _pad_heads(sd[f"{a2}.to_v.weight"], heads, d, dv)], 0)
-            wip = torch.cat([_pad_heads(sd[f"{a2}.processor.to_k_ip.0.weight"], heads, d, dqk),
-                             _pad_heads(sd[f"{a2}.processor.to_v_ip.0.weight"], heads, d, dv)], 0)
-            ob = _ones_bias(heads, d, dv, heads * dqk, wkv.shape[0], "cpu")
+            # text / ip K,V projections of all spatial transformers are two GEMMs (one per token source): the layers' packed
+            # operands side by side, this layer's at column kv_off
+            kv, ip = t["attn2"].pop("kv"), t["attn2"].pop("ip")
             t["kv_off"] = self._kv_off
-            self._kv_off += wkv.shape[0]
-            kv_w.append(wkv); kv_b.append(ob); ip_w.append(wip); ip_b.append(ob)
+            self._kv_off += kv.n
+            kv_w.append(kv.w); kv_b.append(kv.b); ip_w.append(ip.w); ip_b.append(ip.b)
             t["ff1"] = _Lin(_geglu_interleave(sd[f"{tb}.ff.net.0.proj.weight"]), _geglu_interleave(sd[f"{tb}.ff.net.0.proj.bias"]), dev)
             t["ff2"] = lin(f"{tb}.ff.net.2")
             return t
 
-        def motion(p, c, fs):
-            d = c // cfg.motion_num_attention_heads
-            dqk, dv = _dqk(d), _dv(d)
+        def motion(p, c):
             tb = f"{p}.transformer_blocks.0"
-            m = {"c": c, "d": d, "fs": fs, "norm": (f32(f"{p}.norm.weight"), f32(f"{p}.norm.bias")),
+            node = self.get_submodule(tb)
+            m = {"c": c, "norm": (f32(f"{p}.norm.weight"), f32(f"{p}.norm.bias")),
                  "proj_in": lin(f"{p}.proj_in"), "proj_out": lin(f"{p}.proj_out")}
             for i in (1, 2, 3):
                 m[f"ln{i}"] = (f32(f"{tb}.norm{i}.weight"), f32(f"{tb}.norm{i}.bias"))
-            pos2d = _sine_pos_enc_2d(c // 2, fs, fs).to(sd[f"{p}.norm.weight"].device)      # [hw, c]
             for a in ("attn1", "attn2"):
-                ap, pp = f"{tb}.{a}", f"{tb}.{a}.processor"
-                wt = torch.cat([sd[f"{ap}.to_q.weight"], sd[f"{ap}.to_k.weight"], sd[f"{ap}.to_v.weight"]], 0)   # [3c, c]
-                pe = sd[f"{pp}.time_pos_embed.pe"][0]                                                             # [32, c]
-                wsp = torch.cat([_pad_heads(sd[f"{pp}.to_q_sp.weight"], heads, d, dqk),
-                                 _pad_heads(sd[f"{pp}.to_k_sp.weight"], heads, d, dqk),
-                                 _pad_heads(sd[f"{pp}.to_v_sp.weight"], heads, d, dv)], 0)
-                # AlphaBlender (attention_processor.py:700-713): alpha * to_out_sp(S) + (1 - alpha) * to_out(T) is ONE GEMM over
-                # [S | T] with K = 2C: weights [alpha W_sp | (1 - alpha) W_t], bias alpha b_sp + (1 - alpha) b_t (alpha is a
-                # tensor all the way: a mix_factor whose sigmoid underflows to exactly 0 or 1 stays exact)
-                alpha = torch.sigmoid(sd[f"{pp}.alpha_blender.mix_factor"].float()).reshape(())
-                w_sp, b_sp = sd[f"{pp}.to_out_sp.weight"].float(), sd[f"{pp}.to_out_sp.bias"].float()
-                w_t, b_t = sd[f"{ap}.to_out.0.weight"].float(), sd[f"{ap}.to_out.0.bias"].float()
-                m[a] = {"t_qkv": _Lin(wt, None, dev), "t_table": (pe @ wt.t()).to(dev).contiguous(),          # [32, 3c]
-                        "s_qkv": _Lin(wsp, _ones_bias(heads, d, dv, 2 * heads * dqk, wsp.shape[0], "cpu"), dev),
-                        "s_table": (pos2d @ wsp.t()).to(dev).contiguous(),                                      # [hw, Nsp]
-                        "out": _Lin(torch.cat([alpha * w_sp, (1 - alpha) * w_t], 1), alpha * b_sp + (1 - alpha) * b_t, dev)}
+                m[a] = P.pack_spatiotemporal(getattr(node, a).processor, getattr(node, a), dev)
             m["ff1"] = _Lin(_geglu_interleave(sd[f"{tb}.ff.net.0.proj.weight"]), _geglu_interleave(sd[f"{tb}.ff.net.0.proj.bias"]), dev)
             m["ff2"] = lin(f"{tb}.ff.net.2")
             return m
@@ -431,13 +339,13 @@ class MVUNetMotionModel(torch.nn.Module):
                 lay = {"res": resnet(f"down_blocks.{i}.resnets.{j}", cin if j == 0 else cout, 0)}
                 if cfg.down_has_attn[i]:
                     lay["attn"] = transformer2d(f"down_blocks.{i}.attentions.{j}", cout)
-                lay["motion"] = motion(f"down_blocks.{i}.motion_modules.{j}", cout, cfg.feature_size(i))
+                lay["motion"] = motion(f"down_blocks.{i}.motion_modules.{j}", cout)
                 layers.append(lay)
             down.append({"layers": layers, "down": conv3(f"down_blocks.{i}.downsamplers.0.conv") if i != len(ch) - 1 else None})
         W["down"] = down
         c = ch[-1]
         W["mid"] = {"res0": resnet("mid_block.resnets.0", c, 0), "attn": transformer2d("mid_block.attentions.0", c),
-                    "motion": motion("mid_block.motion_modules.0", c, cfg.feature_size(len(ch) - 1)),
+                    "motion": motion("mid_block.motion_modules.0", c),
                     "res1": resnet("mid_block.resnets.1", c, 0)}
         up = []
         skips = []
@@ -451,7 +359,7 @@ class MVUNetMotionModel(torch.nn.Module):
                 lay = {"res": resnet(f"up_blocks.{i}.resnets.{j}", cin - c2, c2)}
                 if has_attn:
                     lay["attn"] = transformer2d(f"up_blocks.{i}.attentions.{j}", cout)
-                lay["motion"] = motion(f"up_blocks.{i}.motion_modules.{j}", cout, cfg.feature_size(len(ch) - 1 - i))
+                lay["motion"] = motion(f"up_blocks.{i}.motion_modules.{j}", cout)
                 layers.append(lay)
             up.append({"layers": layers, "up": conv3(f"up_blocks.{i}.upsamplers.0.conv") if has_up else None, "cout": cout})
         W["up"] = up
@@ -481,18 +389,12 @@ class MVUNetMotionModel(torch.nn.Module):
         return t[:numel].view(*shape)
 
     # ------------------------------------------------------------------------------------------------ building blocks
-    def _gemm(self, A, lin: _Lin, out, M, **kw):
-        self.launches += 1
-        return ops.gemm(A, lin.w, out, M=M, N=lin.n, K=lin.k, bias=kw.pop("bias", lin.b), impl=self.gemm_impl, **kw)
-
     def _gn(self, x1, c1, x2, c2, gb, y, samples, rps, eps, silu, perm=(0, 0)):
-        self.launches += 3
         ws = self._buf("gn_stats", (ops.group_norm_ws_floats(samples, rps, c1 + (c2 if x2 is not None else 0),
                                                              self.cfg.norm_num_groups),), torch.float32)
         return ops.group_norm(x1, c1, x2, c2, gb[0], gb[1], y, samples, rps, self.cfg.norm_num_groups, eps, silu, ws, perm)
 
     def _ln(self, x, gb, y, rows, c):
-        self.launches += 1
         return ops.layer_norm(x, gb[0], gb[1], y, rows, c, 1e-5)
 
     def _resnet(self, r, x, skip, out, n_img, h, w, lvl):
@@ -506,31 +408,27 @@ class MVUNetMotionModel(torch.nn.Module):
         self._gn(x, c1, skip, c2, r["norm1"], gin, n_img, h * w, self.cfg.norm_eps, 1)
         h1 = self._buf(f"h1_{lvl}", (M, cout))
         temb = self._temb_table
-        self._gemm(gin, r["conv1"], h1, M, conv=(n_img, h, w, cin, 1), rowbias=temb[:, r["temb_off"]:], rb_div=h * w,
-                   rb_mod=1 << 40)
+        linear(gin, r["conv1"], h1, M, conv=(n_img, h, w, cin, 1), rowbias=temb[:, r["temb_off"]:], rb_div=h * w,
+               rb_mod=1 << 40)
         gout = g.view(-1)[: M * cout].view(M, cout)
         self._gn(h1, cout, None, 0, r["norm2"], gout, n_img, h * w, self.cfg.norm_eps, 1)
         if "sc_a" in r:
             sc = self._buf(f"sc{lvl}", (M, cout))
-            self._gemm(x, r["sc_a"], sc, M)
+            linear(x, r["sc_a"], sc, M)
             if r["sc_b"] is not None:
-                self._gemm(skip, r["sc_b"], sc, M, R2=sc, ldr2=cout)
+                linear(skip, r["sc_b"], sc, M, R2=sc, ldr2=cout)
             res = sc
         else:
             res = x
-        self._gemm(gout, r["conv2"], out, M, conv=(n_img, h, w, cout, 1), R2=res, ldr2=cout)
+        linear(gout, r["conv2"], out, M, conv=(n_img, h, w, cout, 1), R2=res, ldr2=cout)
         return out
 
     def _ff(self, t, ln_gb, ff1, ff2, M, c, lvl):
         ln = self._buf(f"ln{lvl}", (M, c))
         self._ln(t, ln_gb, ln, M, c)
         mid = self._buf(f"ff{lvl}", (M, 4 * c))
-        self._gemm(ln, ff1, mid, M, geglu=True)
-        self._gemm(mid, ff2, t, M, R2=t, ldr2=c)
-
-    def _attn(self, q, k, v, out, ostr, d, **kw):
-        self.launches += 1
-        ops.attention(q, k, v, out, ostr, heads=self.cfg.num_attention_heads, d=d, scale=d ** -0.5, impl=self.attn_impl, **kw)
+        linear(ln, ff1, mid, M, geglu=True)
+        linear(mid, ff2, t, M, R2=t, ldr2=c)
 
     def _kv_gather_start(self, ln, lin, n_q, M, lvl, table, rb_div, rb_mod):
         """View-parallel projection, first half: the K|V rows of the fused [q.. | k | v] projection are computed FIRST and their
@@ -543,138 +441,95 @@ class MVUNetMotionModel(torch.nn.Module):
         kv_loc = self._buf(f"kvloc{lvl}", (M, n_kv))
         kv_all = self._buf(f"kvall{lvl}", (V, M, n_kv))
         rb = {} if table is None else {"rb_div": rb_div, "rb_mod": rb_mod}
-        self._gemm(ln, lin.rows(n_q, lin.n), kv_loc, M, rowbias=None if table is None else table[:, n_q:], **rb)
+        linear(ln, lin.rows(n_q, lin.n), kv_loc, M, rowbias=None if table is None else table[:, n_q:], **rb)
         work = None
         if self.comm_enabled:
             work = dist.all_gather_into_tensor(kv_all.view(-1), kv_loc.view(-1), group=self.view_group, async_op=True)
             self.collectives += 1
             self.collective_bytes += kv_loc.numel() * 2 * (V - 1)
-        return work, kv_all, n_kv
+        return work, kv_all
 
     def _q_project(self, ln, lin, n_q, M, lvl, table, rb_div, rb_mod):
         qb = self._buf(f"qkv{lvl}", (M, n_q))
         rb = {} if table is None else {"rb_div": rb_div, "rb_mod": rb_mod}
-        self._gemm(ln, lin.rows(0, n_q), qb, M, rowbias=None if table is None else table[:, :n_q], **rb)
+        linear(ln, lin.rows(0, n_q), qb, M, rowbias=None if table is None else table[:, :n_q], **rb)
         return qb
 
-    def _kv_gather_finish(self, token, qb, n_q, hq, q_strides, kv_strides, hw, F, B):
-        work, kv_all, n_kv = token
+    def _kv_gather_finish(self, token, p, qb, hw, F, B):
+        """-> the processor's views over the local queries and the K|V gathered from every view."""
+        work, kv_all = token
         if work is not None:
             work.wait()            # the compute stream waits for the gathered K|V (no host sync)
-        V = self.view_world
-        ext_q, ext_k = (hw, 1, F, B), (hw, V, F, B)
-        vq = ops.view5(qb, 0, n_q, q_strides(n_q), ext_q)
-        vq2 = ops.view5(qb, hq, n_q - hq, q_strides(n_q), ext_q) if n_q > hq else None
-        vk = ops.view5(kv_all, 0, n_kv, kv_strides(n_kv), ext_k)
-        vv = ops.view5(kv_all, hq, n_kv - hq, kv_strides(n_kv), ext_k)
-        return vq, vq2, vk, vv
+        return P.qkv_views(p, qb, kv_all, hw, F, B, 1, kv_view_rows=qb.shape[0])
 
     def _transformer2d(self, t, x, n_img, h, w, lvl, B, Nv, F):
         """Transformer2DModel + BasicTransformerBlock with the MVDreamI2V (attn1) and IPAdapter (attn2) processors."""
-        cfg = self.cfg
-        heads = cfg.num_attention_heads
-        c, d = t["c"], t["d"]
-        dqk, dv = _dqk(d), _dv(d)
+        a1, a2 = t["attn1"], t["attn2"]
+        c = t["c"]
         hw = h * w
         M = n_img * hw
         g = self._buf(f"gn{lvl}", (M, c))
         self._gn(x, c, None, 0, t["norm"], g, n_img, hw, 1e-6, 0)
         tok = self._buf(f"tok{lvl}", (M, c))
-        self._gemm(g, t["proj_in"], tok, M)
+        linear(g, t["proj_in"], tok, M)
         ln = self._buf(f"ln{lvl}", (M, c))
         # ---- attn1: cross-view self attention over the Nv views of a frame + I2V attention against frame 0
         self._ln(tok, t["ln1"], ln, M, c)
-        nq = t["qkv"].n
-        qkv = self._buf(f"qkv{lvl}", (M, nq))
-        hq = heads * dqk
-        ostr = (c, F * hw * c, hw * c, Nv * F * hw * c)
+        qkv = self._buf(f"qkv{lvl}", (M, a1["qkv"].n))
         if self.view_group is None:
-            self._gemm(ln, t["qkv"], qkv, M)
-            st = (nq, F * hw * nq, hw * nq, Nv * F * hw * nq)           # rows ordered (b n f p)
-            ext = (hw, Nv, F, B)
-            vq = ops.view5(qkv, 0, nq, st, ext)
-            vqi = ops.view5(qkv, hq, nq - hq, st, ext)
-            vk = ops.view5(qkv, 2 * hq, nq - 2 * hq, st, ext)
-            vv = ops.view5(qkv, 3 * hq, nq - 3 * hq, st, ext)
+            linear(ln, a1["qkv"], qkv, M)
+            views = P.qkv_views(a1, qkv, qkv, hw, F, B, Nv)
         else:
             # views span ranks: local rows are (b f p) of ONE view; K|V of every view are all-gathered while the two query
             # projections run
-            tok_kv = self._kv_gather_start(ln, t["qkv"], 2 * hq, M, lvl, None, 0, 0)
-            qb = self._q_project(ln, t["qkv"], 2 * hq, M, lvl, None, 0, 0)
-            vq, vqi, vk, vv = self._kv_gather_finish(tok_kv, qb, 2 * hq, hq, (lambda n_: (n_, F * hw * n_, hw * n_, F * hw * n_)),
-                                                     (lambda n_: (n_, M * n_, hw * n_, F * hw * n_)), hw, F, B)
+            tok_kv = self._kv_gather_start(ln, a1["qkv"], 2 * a1["hq"], M, lvl, None, 0, 0)
+            qb = self._q_project(ln, a1["qkv"], 2 * a1["hq"], M, lvl, None, 0, 0)
+            views = self._kv_gather_finish(tok_kv, a1, qb, hw, F, B)
         o12 = self._buf(f"ao{lvl}", (M, 2 * c))                                  # [O1 | O2], rows of 2C
-        ostr12 = tuple(2 * s_ for s_ in ostr)
-        self._attn(vq, vk, vv, o12, ostr12, d)
-        self._attn(vqi, vk, vv, o12, ostr12, d, kv_i3_zero=True, out_col_offset=c)
-        self._gemm(o12, t["out1"], tok, M, R2=tok, ldr2=c)                       # to_out(O1 + to_out_i2v(O2)) + residual
+        P.mv_i2v_attend(a1, views, o12, tok, residual=tok)
         # ---- attn2: text (77) + image (4) cross attention, K/V shared by the F frames of a view
         self._ln(tok, t["ln2"], ln, M, c)
-        q2 = qkv.view(-1)[: M * hq].view(M, hq)
-        self._gemm(ln, t["q2"], q2, M)
-        vq2 = ops.view5(q2, 0, hq, (hq, hw * hq, hw * hq, F * hw * hq), (hw, 1, F, B * Nv))
-        ostr2 = (c, hw * c, hw * c, F * hw * c)
+        q2 = qkv.view(-1)[: M * a2["hq"]].view(M, a2["hq"])
+        linear(ln, a2["q"], q2, M)
         o1 = o12.view(-1)[: M * c].view(M, c)
-        for kvbuf, lk, accumulate, sc in ((self._kv_text, self._n_text, False, 1.0), (self._kv_ip, cfg.ip_num_tokens, True, cfg.ip_scale)):
-            ld = kvbuf.shape[1]
-            off = t["kv_off"]
-            stk = (ld, lk * ld, lk * ld, lk * ld)
-            vk2 = ops.view5(kvbuf, off, ld - off, stk, (lk, 1, 1, B * Nv))
-            vv2 = ops.view5(kvbuf, off + hq, ld - off - hq, stk, (lk, 1, 1, B * Nv))
-            self._attn(vq2, vk2, vv2, o1, ostr2, d, kv_div=F, accumulate=accumulate, out_scale=sc)
-        self._gemm(o1, t["out2"], tok, M, R2=tok, ldr2=c)
+        for kv, image in ((self._kv_text, False), (self._kv_ip, True)):
+            P.ip_adapter_attend(a2, q2, kv, t["kv_off"], o1, hw, F, image)
+        linear(o1, a2["out"], tok, M, residual=tok)
         # ---- feed forward
         self._ff(tok, t["ln3"], t["ff1"], t["ff2"], M, c, lvl)
-        self._gemm(tok, t["proj_out"], x, M, R2=x, ldr2=c)
+        linear(tok, t["proj_out"], x, M, R2=x, ldr2=c)
         return x
 
     def _motion(self, m, x, n_img, h, w, lvl, B, Nv, F):
         """TransformerTemporalModel with the SpatioTemporalI2V processor on attn1 and attn2 (released configuration)."""
-        cfg = self.cfg
-        heads = cfg.motion_num_attention_heads
-        c, d = m["c"], m["d"]
-        dqk, dv = _dqk(d), _dv(d)
+        c = m["c"]
         hw = h * w
         M = n_img * hw
         g = self._buf(f"gn{lvl}", (M, c))
         # GroupNorm statistics pooled over the F frames of a sample; rows re-ordered (bn f p) -> (bn p f) on the way out
         self._gn(x, c, None, 0, m["norm"], g, B * Nv, F * hw, 1e-6, 0, perm=(F, hw))
         tok = self._buf(f"tok{lvl}", (M, c))
-        self._gemm(g, m["proj_in"], tok, M)
+        linear(g, m["proj_in"], tok, M)
         ln = self._buf(f"ln{lvl}", (M, c))
         tq = self._buf(f"tqkv{lvl}", (M, 3 * c))
         st2 = self._buf(f"ao{lvl}", (M, 2 * c))                                  # [S | T]: cross-view branch | temporal branch
-        hq = heads * dqk
         for a, lnk in (("attn1", "ln1"), ("attn2", "ln2")):
             p = m[a]
             self._ln(tok, m[lnk], ln, M, c)
-            ns = p["s_qkv"].n
             if self.view_group is not None:
                 # spatial (cross-view) K|V first: their all-gather overlaps the query projection and the WHOLE temporal branch
-                tok_kv = self._kv_gather_start(ln, p["s_qkv"], hq, M, lvl, p["s_table"], F, hw)
-                qb = self._q_project(ln, p["s_qkv"], hq, M, lvl, p["s_table"], F, hw)
-            # temporal branch: (x + pe_t) W == x W + table[f]
-            self._gemm(ln, p["t_qkv"], tq, M, rowbias=p["t_table"], rb_div=1, rb_mod=F)
-            self.launches += 1
-            ops.temporal_attn(tq, st2, M // F, F, heads, d, d ** -0.5, ldo=2 * c, out_col_offset=c)
-            # spatial (cross-view) branch: (x + pos2d) W == x W + table[p]
+                tok_kv = self._kv_gather_start(ln, p["s_qkv"], p["hq"], M, lvl, p["s_table"], F, hw)
+                qb = self._q_project(ln, p["s_qkv"], p["hq"], M, lvl, p["s_table"], F, hw)
+            P.spatiotemporal_temporal(p, ln, tq, st2, F)
             if self.view_group is None:
-                sq = self._buf(f"qkv{lvl}", (M, ns))
-                self._gemm(ln, p["s_qkv"], sq, M, rowbias=p["s_table"], rb_div=F, rb_mod=hw)
-                st = (F * ns, hw * F * ns, ns, Nv * hw * F * ns)            # rows ordered (b n p f)
-                ext = (hw, Nv, F, B)
-                vq = ops.view5(sq, 0, ns, st, ext)
-                vk = ops.view5(sq, hq, ns - hq, st, ext)
-                vv = ops.view5(sq, 2 * hq, ns - 2 * hq, st, ext)
+                views = P.spatiotemporal_project(p, ln, self._buf(f"qkv{lvl}", (M, p["s_qkv"].n)), hw, F, B, Nv)
             else:
-                vq, _, vk, vv = self._kv_gather_finish(tok_kv, qb, hq, hq, (lambda n_: (F * n_, hw * F * n_, n_, hw * F * n_)),
-                                                       (lambda n_: (F * n_, M * n_, n_, hw * F * n_)), hw, F, B)
-            self._attn(vq, vk, vv, st2, (2 * F * c, 2 * hw * F * c, 2 * c, 2 * Nv * hw * F * c), d)
-            # AlphaBlender of both branches' output projections + the block residual: one GEMM, K = 2C
-            self._gemm(st2, p["out"], tok, M, R2=tok, ldr2=c)
+                views = self._kv_gather_finish(tok_kv, p, qb, hw, F, B)
+            # cross-view attention, then the AlphaBlender of both branches' output projections + the block residual
+            P.spatiotemporal_attend(p, views, st2, tok, residual=tok)
         self._ff(tok, m["ln3"], m["ff1"], m["ff2"], M, c, lvl)
         # proj_out, rows back to (bn f p), + residual
-        self._gemm(tok, m["proj_out"], x, M, perm=(hw, F), R2=x, ldr2=c)
+        linear(tok, m["proj_out"], x, M, perm=(hw, F), R2=x, ldr2=c)
         return x
 
     # ------------------------------------------------------------------------------------------------ forward
@@ -697,7 +552,6 @@ class MVUNetMotionModel(torch.nn.Module):
         c1 = self._buf("c1", (BN, cfg.time_embed_dim), torch.float32)
         ops.linear_f32(st["camera"], ce[0], ce[1], c1, BN, cfg.time_embed_dim, cfg.camera_embedding_dim)
         ops.linear_f32(c1, ce[2], ce[3], emb, BN, cfg.time_embed_dim, cfg.time_embed_dim, act_in=1, accumulate=True)
-        self.launches += 5
         semb = self._buf("semb", (N, cfg.time_embed_dim))
         if cond_zero:
             # frame-0 rows use the t=0 embedding (unet_motion_mv_model.py:732-752); rare path, assembled with torch indexing
@@ -714,14 +568,14 @@ class MVUNetMotionModel(torch.nn.Module):
         else:
             ops.silu_rows(emb, semb, N, cfg.time_embed_dim, F)
         self._temb_table = self._buf("temb_table", (N, W["temb"].n), torch.float32)
-        self._gemm(semb, W["temb"], self._temb_table, N, out_f32=True)
+        linear(semb, W["temb"], self._temb_table, N, out_f32=True)
         # ---- text / ip tokens -> K,V of all 16 spatial transformers (once per view, not per frame)
         n_text = st["text"].shape[1]
         self._n_text = n_text
         text16 = self._buf("text16", (BN * n_text, cfg.cross_attention_dim))
         ops.cast_f32_f16(st["text"], text16)
         self._kv_text = self._buf("kv_text", (BN * n_text, W["kv_text"].n))
-        self._gemm(text16, W["kv_text"], self._kv_text, BN * n_text)
+        linear(text16, W["kv_text"], self._kv_text, BN * n_text)
         ipw = W["ip_proj"]
         ipt = self._buf("ipt", (BN, cfg.ip_num_tokens * cfg.cross_attention_dim), torch.float32)
         ops.linear_f32(st["image_embeds"], ipw[0], ipw[1], ipt, BN, cfg.ip_num_tokens * cfg.cross_attention_dim, cfg.ip_image_embed_dim)
@@ -730,15 +584,13 @@ class MVUNetMotionModel(torch.nn.Module):
         ipn = self._buf("ipn", (BN * cfg.ip_num_tokens, cfg.cross_attention_dim))
         ops.layer_norm(ip16, ipw[2], ipw[3], ipn, BN * cfg.ip_num_tokens, cfg.cross_attention_dim, 1e-5)
         self._kv_ip = self._buf("kv_ip", (BN * cfg.ip_num_tokens, W["kv_ip"].n))
-        self._gemm(ipn, W["kv_ip"], self._kv_ip, BN * cfg.ip_num_tokens)
-        self.launches += 5
+        linear(ipn, W["kv_ip"], self._kv_ip, BN * cfg.ip_num_tokens)
         # ---- conv_in (+ layout change of line 767)
         hs = [h0 >> i for i in range(len(ch))]
         ws = [w0 >> i for i in range(len(ch))]
         skips = []
         x = self._buf("skip0", (N * hs[0] * ws[0], ch[0]))
         ops.conv_in(st["sample"], W["conv_in"][0], W["conv_in"][1], x, BN, cfg.in_channels, F, hs[0], ws[0], ch[0])
-        self.launches += 1
         skips.append(x)
         si = 1
         for i, blk in enumerate(W["down"]):
@@ -754,7 +606,7 @@ class MVUNetMotionModel(torch.nn.Module):
             if blk["down"] is not None:
                 c = blk["down"].n
                 out = self._buf(f"skip{si}", (N * hs[i + 1] * ws[i + 1], c)); si += 1
-                self._gemm(x, blk["down"], out, N * hs[i + 1] * ws[i + 1], conv=(N, h, w, c, 2))
+                linear(x, blk["down"], out, N * hs[i + 1] * ws[i + 1], conv=(N, h, w, c, 2))
                 x = out
                 skips.append(x)
         lv = len(ch) - 1
@@ -782,16 +634,14 @@ class MVUNetMotionModel(torch.nn.Module):
                 c = blk["cout"]
                 upb = self._buf(f"upsampled{lv}", (N * 4 * h * w, c))
                 ops.upsample2x(x, upb, N, h, w, c)
-                self.launches += 1
                 out = self._buf(f"xup{lv - 1}_up", (N * 4 * h * w, c))
-                self._gemm(upb, blk["up"], out, N * 4 * h * w, conv=(N, 2 * h, 2 * w, c, 1))
+                linear(upb, blk["up"], out, N * 4 * h * w, conv=(N, 2 * h, 2 * w, c, 1))
                 x = out
         # ---- out: GroupNorm + SiLU + conv_out (+ layout change of line 862)
         h, w = hs[0], ws[0]
         g = self._buf("gn0", (N * h * w, ch[0]))
         self._gn(x, ch[0], None, 0, W["norm_out"], g, N, h * w, cfg.norm_eps, 1)
         ops.conv_out(g, W["conv_out"][0], W["conv_out"][1], st["out"], BN, ch[0], F, h, w, cfg.out_channels)
-        self.launches += 1
 
     @torch.no_grad()
     def forward(self, sample, timestep, encoder_hidden_states, timestep_cond=None, attention_mask=None,
@@ -838,9 +688,10 @@ class MVUNetMotionModel(torch.nn.Module):
         if graph is not None:
             graph.replay()
         else:
-            self.launches = self.collectives = self.collective_bytes = 0
+            self.collectives = self.collective_bytes = 0
+            n0 = ops.launches
             self._run(sig, st)
-            self.launches_per_forward = self.launches
+            self.launches_per_forward = ops.launches - n0
             st["calls"] += 1
             if self.use_cuda_graph and st["calls"] == 1:
                 # second pass under capture: same launches, same buffers

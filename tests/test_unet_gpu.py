@@ -8,17 +8,17 @@ import torch
 pytestmark = pytest.mark.gpu
 
 
-def _run(nv, nf, groups, seed=0, cond_zero=False, t=500, graph=True, ip_scale=1.0):
+def _run(nv, nf, groups, seed=0, cond_zero=False, t=500, graph=True, ip_scale=1.0, **geometry):
     from animate3d_b200.unet import MVUNetMotionModel
     from animate3d_b200.unet_config import UNetConfig
     from oracle import unet_oracle as O
-    ocfg = O.UNetConfig(num_views=nv, num_frames=nf, ip_scale=ip_scale)
+    ocfg = O.UNetConfig(num_views=nv, num_frames=nf, ip_scale=ip_scale, **geometry)
     sd = O.make_state_dict(ocfg, seed)
     sample, text, camera, img = O.synthetic_inputs(ocfg, groups, nv, nf, seed)
     torch.set_num_threads(min(16, os.cpu_count() or 1))   # many-core hosts: the fp32 oracle is fastest far below cpu_count
     with torch.no_grad():
         ref = O.unet_forward(sd, ocfg, sample, t, text, camera, img, nv, i2v_cond_time_zero=cond_zero)
-    model = MVUNetMotionModel(UNetConfig(num_views=nv, num_frames=nf, ip_scale=ip_scale))
+    model = MVUNetMotionModel(UNetConfig(num_views=nv, num_frames=nf, ip_scale=ip_scale, **geometry))
     model.use_cuda_graph = graph
     missing, unexpected = model.load_state_dict(sd)
     assert not missing and not unexpected
@@ -67,6 +67,13 @@ def test_unet_multiview_cfg_batch_matches_oracle():
 def test_unet_i2v_cond_time_zero():
     ref, outs, _ = _run(1, 4, 1, seed=5, cond_zero=True, graph=False)
     _check(ref, outs[0], "i2v_cond_time_zero")
+
+
+def test_unet_motion_heads_differ_from_spatial():
+    """Motion modules with 4 heads next to 8 spatial heads (head dims 40, 80 and 160): every processor packs and attends with
+    its own layer's head count."""
+    ref, outs, _ = _run(2, 3, 1, seed=8, graph=False, motion_num_attention_heads=4, block_out_channels=(320, 640, 640, 640))
+    _check(ref, outs[0], "motion heads 4, spatial heads 8")
 
 
 def _oracle_threads():
