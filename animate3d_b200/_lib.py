@@ -83,6 +83,12 @@ def load(require_gpu: bool = True) -> C.CDLL:
         lib.a3d_deform_backward_scratch_bytes.argtypes = [C.c_void_p]
         lib.a3d_arap_scratch_bytes.restype = C.c_size_t
         lib.a3d_arap_scratch_bytes.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]
+        lib.a3d_mesh_adjacency_scratch_bytes.restype = C.c_size_t
+        lib.a3d_mesh_adjacency_scratch_bytes.argtypes = [C.c_int, C.c_int]
+        lib.a3d_mesh_vertex_stats_scratch_bytes.restype = C.c_size_t
+        lib.a3d_mesh_vertex_stats_scratch_bytes.argtypes = [C.c_int, C.c_int, C.c_int]
+        lib.a3d_mesh_sample_neighbors.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_uint64, C.c_uint64, C.c_void_p,
+                                                  C.c_void_p]
         _lib = lib
     if require_gpu and not _inited:
         if not torch.cuda.is_available():

@@ -272,3 +272,17 @@ class Gaussian4DModel(torch.nn.Module):
         # means = R xyz + trans + delta = (xyz + delta) + (R xyz - xyz) + trans
         means = means + (torch.einsum("tij,pj->tpi", rmat, self._xyz) - self._xyz[None]) + trans[:, None]
         return means, scales, rots
+
+    def deform_frames(self, timestamps: torch.Tensor, deform_scale: bool = True, first_frame_trainable: bool = False):
+        """`deform_all` with the condition-frame rule of the reference renderer (diff_gaussian_rasterizer_advanced_4d.py:77-83):
+        unless `first_frame_trainable`, frames with timestamp == -1 are the static gaussians (`_xyz`, exp(`_scaling`),
+        normalised `_rotation`).  The renderer and the trajectory export both go through here."""
+        means, scales, rots = self.deform_all(timestamps, deform_scale=deform_scale)
+        if not first_frame_trainable:
+            first = timestamps.reshape(-1).float().to(self._xyz.device) == -1
+            if bool(first.any()):
+                keep = first[:, None, None]
+                means = torch.where(keep, self._xyz[None], means)
+                scales = torch.where(keep, torch.exp(self._scaling)[None], scales)
+                rots = torch.where(keep, torch.nn.functional.normalize(self._rotation, dim=-1)[None], rots)
+        return means, scales, rots

@@ -72,14 +72,9 @@ class Gaussian4DBatchRenderer:
             rots = torch.nn.functional.normalize(pc._rotation, dim=-1)[None].expand(bs, P, 4)
         else:
             uniq, inverse = torch.unique(ts.reshape(bs).float(), return_inverse=True)
-            means_t, scales_t, rots_t = pc.deform_all(uniq, deform_scale=bool(do_guidance))      # 132-137
-            if not self.cfg.first_frame_trainable:
-                first = (uniq == -1)
-                if bool(first.any()):     # static gaussians for the condition frame (77-83: hidden_feats stays None)
-                    keep = first[:, None, None]
-                    means_t = torch.where(keep, pc._xyz[None], means_t)
-                    scales_t = torch.where(keep, torch.exp(pc._scaling)[None], scales_t)
-                    rots_t = torch.where(keep, torch.nn.functional.normalize(pc._rotation, dim=-1)[None], rots_t)
+            # 132-137; static gaussians for the condition frame unless first_frame_trainable (77-83: hidden_feats stays None)
+            means_t, scales_t, rots_t = pc.deform_frames(uniq, deform_scale=bool(do_guidance),
+                                                         first_frame_trainable=self.cfg.first_frame_trainable)
             means, scales, rots = means_t[inverse], scales_t[inverse], rots_t[inverse]
         # per-camera tensors that are ON the autograd path (callers read / retain_grad `out["means3D"][i]` like the reference's
         # per-camera `means3D`): unbind first, render from the re-stacked batch

@@ -303,6 +303,36 @@ int a3d_arap(const float* nodes, int Nt, int Nv, const int32_t* nbr, int K, cons
 /* Scratch bytes a3d_arap needs for the same sizes (Ns of a NULL sample = Nv): 0 when deterministic is 0. */
 size_t a3d_arap_scratch_bytes(int Nt, int Nv, int K, int Ns, int deterministic);
 
+/* ---------------------------------------------------------------- mesh animation (SURVEY 8f-5) ---------------- */
+/* The device mesh graph is CSR: row_ptr [V+1] and col [E] int32, one row per vertex, its unique neighbours (both directions
+ * of every face edge) in ascending index order.  Nothing here uses atomics on an output: results are bit-identical per run. */
+/* Vertex adjacency of a triangle mesh, the graph of compute_edge_distances / find_and_save_connected_vertices
+ * (tools/mesh_animation/mesh2gaussian.py:36-63, 66-88): the 6 directed half-edges of every face as (src << 32 | dst) keys,
+ * CUB radix-sorted, duplicates dropped by a flag pass and a scan, row offsets from the source boundaries.  faces [F,3];
+ * a face with a corner outside [0, V) contributes no edge.  A repeated corner gives a self-edge, as in the reference.
+ * col must hold 6F entries (the upper bound); num_edges_host (pinned) receives E once the stream reaches it. */
+int a3d_mesh_adjacency(const int32_t* faces, int F, int V, int32_t* row_ptr, int32_t* col, int64_t* num_edges_host,
+                       void* scratch, size_t scratch_bytes, void* stream);
+/* Scratch bytes a3d_mesh_adjacency needs: 40 B per half-edge (6F) plus the CUB temporary.  0 for bad sizes. */
+size_t a3d_mesh_adjacency_scratch_bytes(int V, int F);
+/* mean_abs_edge [V,3]: the mean of |v_j - v_i| per axis over the CSR row of i, summed in CSR order (compute_edge_distances,
+ * mesh2gaussian.py:36-63); 0 for an empty row.  With corner_rgb [F,3,3] (per face-corner colours) also vertex_rgb [V,3]:
+ * the mean over the vertex's face corners with the count clamped to >= 1 (convert_to_textureVertex_with_average, 15-33),
+ * summed through a stable vertex -> corner sort in the reference's order (corner slot 0 of every face, then slot 1, then 2).
+ * corner_rgb NULL: faces / vertex_rgb / scratch are unused. */
+int a3d_mesh_vertex_stats(const float* verts, int V, const int32_t* row_ptr, const int32_t* col, const int32_t* faces, int F,
+                          const float* corner_rgb, float* mean_abs_edge, float* vertex_rgb, void* scratch, size_t scratch_bytes,
+                          void* stream);
+/* Scratch bytes a3d_mesh_vertex_stats needs (0 when with_rgb is 0). */
+size_t a3d_mesh_vertex_stats_scratch_bytes(int V, int F, int with_rgb);
+/* K <= 12 random neighbours per vertex without repetition, the per-step draw of the mesh-edge ARAP graph
+ * (sample_matrix_vectorized, custom/threestudio-animate3d/systems/util.py:320-344, called at systems/animate3d.py:224):
+ * slot j of row i gets the key = word 0 of Philox4x32-10 with counter (i, j, offset_lo, offset_hi) and key
+ * (seed_lo, seed_hi); the K smallest keys (ties by j) are written in ascending key order.  nbr [V,K], -1 past the row's
+ * degree: the ragged table a3d_arap reads.  A pure function of (seed, offset, CSR). */
+int a3d_mesh_sample_neighbors(const int32_t* row_ptr, const int32_t* col, int V, int K, uint64_t seed, uint64_t offset,
+                              int32_t* nbr, void* stream);
+
 /* debug hook: a device uint64 counter the tensor-core attention kernel bumps once per (warp, key step) that takes the
    lazy-rescale branch of the single-pass softmax (NULL = off; tests use it to prove adversarial inputs reach that branch). */
 int a3d_debug_set_attn_trace(void* device_counter_u64);
