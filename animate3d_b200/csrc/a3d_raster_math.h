@@ -115,6 +115,99 @@ A3D_HD bool preprocess_gaussian(const float* p, const float* s, const float* q, 
 }
 
 // ---------------------------------------------------------------------------------------------------------------
+// SH colour: rgb_ch = max(sum_k basis_k(dir) * sh_k,ch + 0.5, 0), dir = (mean - campos) / |mean - campos|
+// ---------------------------------------------------------------------------------------------------------------
+constexpr float kShC1 = 0.4886025119029199f;
+// scalar constants: constexpr arrays are not usable in device code
+constexpr float kShC2_0 = 1.0925484305920792f, kShC2_1 = -1.0925484305920792f, kShC2_2 = 0.31539156525252005f,
+                kShC2_3 = -1.0925484305920792f, kShC2_4 = 0.5462742152960396f;
+constexpr float kShC3_0 = -0.5900435899266435f, kShC3_1 = 2.890611442640554f, kShC3_2 = -0.4570457994644658f,
+                kShC3_3 = 0.3731763325901154f, kShC3_4 = -0.4570457994644658f, kShC3_5 = 1.445305721320277f,
+                kShC3_6 = -0.5900435899266435f;
+
+A3D_HD void sh_basis(int deg, float x, float y, float z, float* b) {
+  b[0] = kShC0;
+  if (deg > 0) {
+    b[1] = -kShC1 * y; b[2] = kShC1 * z; b[3] = -kShC1 * x;
+    if (deg > 1) {
+      const float xx = x * x, yy = y * y, zz = z * z, xy = x * y, yz = y * z, xz = x * z;
+      b[4] = kShC2_0 * xy; b[5] = kShC2_1 * yz; b[6] = kShC2_2 * (2.0f * zz - xx - yy);
+      b[7] = kShC2_3 * xz; b[8] = kShC2_4 * (xx - yy);
+      if (deg > 2) {
+        b[9] = kShC3_0 * y * (3.0f * xx - yy); b[10] = kShC3_1 * xy * z;
+        b[11] = kShC3_2 * y * (4.0f * zz - xx - yy); b[12] = kShC3_3 * z * (2.0f * zz - 3.0f * xx - 3.0f * yy);
+        b[13] = kShC3_4 * x * (4.0f * zz - xx - yy); b[14] = kShC3_5 * z * (xx - yy);
+        b[15] = kShC3_6 * x * (xx - 3.0f * yy);
+      }
+    }
+  }
+}
+
+// unit direction from the camera centre to the gaussian mean m: the direction the SH colour is evaluated in; returns |m - campos|
+A3D_HD float view_dir(const float* m, const float* campos, float& dx, float& dy, float& dz) {
+  dx = m[0] - campos[0]; dy = m[1] - campos[1]; dz = m[2] - campos[2];
+  const float n = sqrtf((dx * dx + dy * dy) + dz * dz);
+  dx /= n; dy /= n; dz /= n;
+  return n;
+}
+
+// forward colour of one (camera, gaussian) from its SH coefficients sh [(deg+1)^2][3]; bit ch of the result is set when
+// channel ch was clamped at 0
+A3D_HD uint32_t sh_colour(int deg, const float* m, const float* campos, const float* sh, float rgb[3]) {
+  float dx, dy, dz, b[16];
+  view_dir(m, campos, dx, dy, dz);
+  sh_basis(deg, dx, dy, dz, b);
+  const int nb = (deg + 1) * (deg + 1);
+  uint32_t clamped = 0;
+  for (int ch = 0; ch < 3; ++ch) {
+    float v = 0.f;
+    for (int k = 0; k < nb; ++k) v += b[k] * sh[3 * k + ch];
+    v += 0.5f;
+    if (v < 0.f) { clamped |= 1u << ch; v = 0.f; }
+    rgb[ch] = v;
+  }
+  return clamped;
+}
+
+// Backward of sh_colour for one (camera, gaussian).  In: g = dL/drgb.  Out: g masked by the clamp bits, the basis b (so
+// dL/dsh_k,ch = b[k] * g[ch]), and dL/dmean through the view direction ADDED to dmean.  The colour depends on the mean
+// through dir even when the coefficients are frozen, so this term is needed whenever the mean gradient is.
+A3D_HD void sh_backward(int deg, const float* m, const float* campos, const float* sh, uint32_t clamped, float g[3], float b[16],
+                        float dmean[3]) {
+  for (int ch = 0; ch < 3; ++ch)
+    if (clamped & (1u << ch)) g[ch] = 0.f;
+  float x, y, z;
+  const float n = view_dir(m, campos, x, y, z);
+  sh_basis(deg, x, y, z, b);
+  if (deg == 0) return;
+  // s_k = dL/dbasis_k; then dL/ddir = sum_k s_k * grad(basis_k)
+  float s[16];
+  const int nb = (deg + 1) * (deg + 1);
+#pragma unroll
+  for (int k = 1; k < 16; ++k) s[k] = k < nb ? (sh[3 * k] * g[0] + sh[3 * k + 1] * g[1]) + sh[3 * k + 2] * g[2] : 0.f;
+  float gx = -kShC1 * s[3], gy = -kShC1 * s[1], gz = kShC1 * s[2];
+  if (deg > 1) {
+    const float xx = x * x, yy = y * y, zz = z * z, xy = x * y, yz = y * z, xz = x * z;
+    gx += kShC2_0 * y * s[4] - 2.f * kShC2_2 * x * s[6] + kShC2_3 * z * s[7] + 2.f * kShC2_4 * x * s[8];
+    gy += kShC2_0 * x * s[4] + kShC2_1 * z * s[5] - 2.f * kShC2_2 * y * s[6] - 2.f * kShC2_4 * y * s[8];
+    gz += kShC2_1 * y * s[5] + 4.f * kShC2_2 * z * s[6] + kShC2_3 * x * s[7];
+    if (deg > 2) {
+      gx += kShC3_0 * 6.f * xy * s[9] + kShC3_1 * yz * s[10] - kShC3_2 * 2.f * xy * s[11] - kShC3_3 * 6.f * xz * s[12] +
+            kShC3_4 * (4.f * zz - 3.f * xx - yy) * s[13] + kShC3_5 * 2.f * xz * s[14] + kShC3_6 * 3.f * (xx - yy) * s[15];
+      gy += kShC3_0 * 3.f * (xx - yy) * s[9] + kShC3_1 * xz * s[10] + kShC3_2 * (4.f * zz - xx - 3.f * yy) * s[11] -
+            kShC3_3 * 6.f * yz * s[12] - kShC3_4 * 2.f * xy * s[13] - kShC3_5 * 2.f * yz * s[14] - kShC3_6 * 6.f * xy * s[15];
+      gz += kShC3_1 * xy * s[10] + kShC3_2 * 8.f * yz * s[11] + kShC3_3 * (6.f * zz - 3.f * xx - 3.f * yy) * s[12] +
+            kShC3_4 * 8.f * xz * s[13] + kShC3_5 * (xx - yy) * s[14];
+    }
+  }
+  // dir = d / |d|: dL/dd = (I - dir dir^T) dL/ddir / |d|
+  const float dot = (x * gx + y * gy) + z * gz;
+  dmean[0] += (gx - x * dot) / n;
+  dmean[1] += (gy - y * dot) / n;
+  dmean[2] += (gz - z * dot) / n;
+}
+
+// ---------------------------------------------------------------------------------------------------------------
 // blending: one (pixel, gaussian) step, forward and backward
 // ---------------------------------------------------------------------------------------------------------------
 // returns alpha (0 when the gaussian does not contribute)

@@ -6,31 +6,6 @@
 
 namespace a3d {
 
-__device__ __forceinline__ void sh_basis(int deg, float x, float y, float z, float* b) {
-  b[0] = kShC0;
-  if (deg > 0) {
-    b[1] = -0.4886025119029199f * y; b[2] = 0.4886025119029199f * z; b[3] = -0.4886025119029199f * x;
-    if (deg > 1) {
-      const float xx = x * x, yy = y * y, zz = z * z, xy = x * y, yz = y * z, xz = x * z;
-      b[4] = 1.0925484305920792f * xy; b[5] = -1.0925484305920792f * yz; b[6] = 0.31539156525252005f * (2.0f * zz - xx - yy);
-      b[7] = -1.0925484305920792f * xz; b[8] = 0.5462742152960396f * (xx - yy);
-      if (deg > 2) {
-        b[9] = -0.5900435899266435f * y * (3.0f * xx - yy); b[10] = 2.890611442640554f * xy * z;
-        b[11] = -0.4570457994644658f * y * (4.0f * zz - xx - yy); b[12] = 0.3731763325901154f * z * (2.0f * zz - 3.0f * xx - 3.0f * yy);
-        b[13] = -0.4570457994644658f * x * (4.0f * zz - xx - yy); b[14] = 1.445305721320277f * z * (xx - yy);
-        b[15] = -0.5900435899266435f * x * (xx - 3.0f * yy);
-      }
-    }
-  }
-}
-
-// unit direction from the camera centre to the gaussian mean m: the direction the SH colour is evaluated in
-__device__ __forceinline__ void view_dir(const float* m, const a3d_raster_cam& c, float& dx, float& dy, float& dz) {
-  dx = m[0] - c.campos[0]; dy = m[1] - c.campos[1]; dz = m[2] - c.campos[2];
-  const float n = sqrtf((dx * dx + dy * dy) + dz * dz);
-  dx /= n; dy /= n; dz /= n;
-}
-
 __global__ void raster_preprocess_kernel(RasterDev a, RasterWs ws, int32_t* __restrict__ radii) {
   const int idx = blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= a.num_cams * a.P) return;
@@ -53,18 +28,7 @@ __global__ void raster_preprocess_kernel(RasterDev a, RasterWs ws, int32_t* __re
   if (a.colors_precomp) {
     for (int ch = 0; ch < 3; ++ch) rgb[ch] = a.colors_precomp[3 * i + ch];
   } else {
-    float dx, dy, dz, b[16];
-    view_dir(a.means3D + 3 * gi, c, dx, dy, dz);
-    sh_basis(a.sh_degree, dx, dy, dz, b);
-    const int nb = (a.sh_degree + 1) * (a.sh_degree + 1);
-    const float* sh = a.shs + (size_t)i * a.sh_coeffs * 3;
-    for (int ch = 0; ch < 3; ++ch) {
-      float v = 0.f;
-      for (int k = 0; k < nb; ++k) v += b[k] * sh[3 * k + ch];
-      v += 0.5f;
-      if (v < 0.f) { clamped |= 1u << ch; v = 0.f; }
-      rgb[ch] = v;
-    }
+    clamped = sh_colour(a.sh_degree, a.means3D + 3 * gi, c.campos, a.shs + (size_t)i * a.sh_coeffs * 3, rgb);
   }
   ws.rgb_depth[idx] = make_float4(rgb[0], rgb[1], rgb[2], o.depth);
   ws.clamped[idx] = (uint8_t)clamped;
@@ -114,12 +78,13 @@ __global__ void raster_ranges_kernel(RasterWs ws, long long n, long long total_t
 
 // Per-(camera, gaussian) part of the preprocess backward, shared by both kernels, for a visible pair idx (camera cam, geometry
 // slot gi): the (dconic, dmean2D, ddepth) gradients pushed through the projection into dm / ds / dr, the dmeans2D write
-// (upstream convention: gradient w.r.t. NDC coordinates), and with sh_grad the SH basis of the view direction and the clamp
-// mask of the forward colours.  colour = clamp(sum_k basis_k(dir) * sh_k + 0.5) is linear in the coefficients; the dependence
-// of the basis on the view direction is not differentiated (Animate3D's features are frozen buffers, gaussian_4d.py:262-297).
-__device__ __forceinline__ void pair_backward(const RasterDev& a, const RasterWs& ws, int cam, size_t idx, size_t gi, float* dmeans2D,
+// (upstream convention: gradient w.r.t. NDC coordinates), and with sh_grad the SH colour backward (sh_backward): dL/drgb
+// masked by the forward clamp bits into g, the basis into b, and the view-direction term added to dm.  The colour depends on
+// the mean through the view direction even when the SH features themselves are frozen buffers, so sh_grad is set whenever
+// colours come from SH and either the SH or the mean gradient is requested.
+__device__ __forceinline__ void pair_backward(const RasterDev& a, const RasterWs& ws, int cam, int i, size_t idx, size_t gi, float* dmeans2D,
                                               bool sh_grad, float (&dm)[3], float (&ds)[3], float (&dr)[4], float (&b)[16],
-                                              uint32_t& clamped) {
+                                              float (&g)[3]) {
   const a3d_raster_cam& c = a.cams[cam];
   const float gpx = ws.g_mean2d[2 * idx], gpy = ws.g_mean2d[2 * idx + 1];
   preprocess_backward(a.means3D + 3 * gi, a.scales + 3 * gi, a.rotations + 4 * gi, a.scale_modifier, c.viewmatrix, c.projmatrix,
@@ -130,12 +95,9 @@ __device__ __forceinline__ void pair_backward(const RasterDev& a, const RasterWs
     dmeans2D[3 * idx + 1] = gpy * 0.5f * (float)a.H;
     dmeans2D[3 * idx + 2] = 0.f;
   }
-  if (sh_grad) {
-    float dx, dy, dz;
-    view_dir(a.means3D + 3 * gi, c, dx, dy, dz);
-    sh_basis(a.sh_degree, dx, dy, dz, b);
-    clamped = ws.clamped[idx];
-  }
+  for (int ch = 0; ch < 3; ++ch) g[ch] = ws.g_rgb[3 * idx + ch];
+  if (sh_grad)
+    sh_backward(a.sh_degree, a.means3D + 3 * gi, c.campos, a.shs + (size_t)i * a.sh_coeffs * 3, ws.clamped[idx], g, b, dm);
 }
 
 // per-gaussian backward: (dconic, dmean2D, ddepth, drgb) of every camera -> means3D / scales / rotations / colors / SH
@@ -148,22 +110,22 @@ __global__ void raster_preprocess_backward_kernel(RasterDev a, RasterWs ws, cons
   if (radii[idx] <= 0) return;
   const int cam = idx / a.P, i = idx % a.P;
   const size_t gi = (size_t)(a.per_cam_geometry ? cam : 0) * a.P + i;
-  float dm[3], ds[3], dr[4], b[16];
-  uint32_t cl = 0;
-  pair_backward(a, ws, cam, idx, gi, dmeans2D, !a.colors_precomp && dshs, dm, ds, dr, b, cl);
+  float dm[3], ds[3], dr[4], b[16], g[3];
+  pair_backward(a, ws, cam, i, idx, gi, dmeans2D, !a.colors_precomp && (dshs || dmeans3D), dm, ds, dr, b, g);
   for (int k = 0; k < 3; ++k) {
     if (dmeans3D) atomicAdd(dmeans3D + 3 * gi + k, dm[k]);
     if (dscales) atomicAdd(dscales + 3 * gi + k, ds[k]);
   }
   if (drots) for (int k = 0; k < 4; ++k) atomicAdd(drots + 4 * gi + k, dr[k]);
-  const float* grgb = ws.g_rgb + 3 * (size_t)idx;
   if (a.colors_precomp) {
-    if (dcolors) for (int ch = 0; ch < 3; ++ch) atomicAdd(dcolors + 3 * i + ch, grgb[ch]);
+    if (dcolors) for (int ch = 0; ch < 3; ++ch) atomicAdd(dcolors + 3 * i + ch, g[ch]);
   } else if (dshs) {
     const int nb = (a.sh_degree + 1) * (a.sh_degree + 1);
     for (int ch = 0; ch < 3; ++ch) {
-      if (cl & (1u << ch)) continue;
-      for (int k = 0; k < nb; ++k) atomicAdd(dshs + ((size_t)i * a.sh_coeffs + k) * 3 + ch, b[k] * grgb[ch]);
+      if (g[ch] == 0.f) continue;   // clamped channel (or nothing to add)
+#pragma unroll
+      for (int k = 0; k < 16; ++k)
+        if (k < nb) atomicAdd(dshs + ((size_t)i * a.sh_coeffs + k) * 3 + ch, b[k] * g[ch]);
     }
   }
 }
@@ -212,9 +174,8 @@ __global__ void raster_preprocess_backward_det_kernel(RasterDev a, RasterWs ws, 
     aop += op_part[idx];
     if (radii[idx] <= 0) continue;
     const size_t gi = (size_t)(a.per_cam_geometry ? cam : 0) * a.P + i;
-    float dm[3], ds[3], dr[4], b[16];
-    uint32_t cl = 0;
-    pair_backward(a, ws, cam, idx, gi, dmeans2D, !a.colors_precomp && dshs, dm, ds, dr, b, cl);
+    float dm[3], ds[3], dr[4], b[16], g[3];
+    pair_backward(a, ws, cam, i, idx, gi, dmeans2D, !a.colors_precomp && (dshs || dmeans3D), dm, ds, dr, b, g);
     if (a.per_cam_geometry) {   // one camera per gradient entry: written directly
       for (int k = 0; k < 3; ++k) {
         if (dmeans3D) dmeans3D[3 * gi + k] += dm[k];
@@ -225,16 +186,14 @@ __global__ void raster_preprocess_backward_det_kernel(RasterDev a, RasterWs ws, 
       for (int k = 0; k < 3; ++k) { am[k] += dm[k]; as[k] += ds[k]; }
       for (int k = 0; k < 4; ++k) ar[k] += dr[k];
     }
-    const float* grgb = ws.g_rgb + 3 * idx;
     if (a.colors_precomp) {
-      for (int ch = 0; ch < 3; ++ch) acol[ch] += grgb[ch];
+      for (int ch = 0; ch < 3; ++ch) acol[ch] += g[ch];
     } else if (dshs) {
 #pragma unroll
       for (int k = 0; k < 16; ++k)
         if (k < nb)
 #pragma unroll
-          for (int ch = 0; ch < 3; ++ch)
-            if (!(cl & (1u << ch))) ash[k][ch] += b[k] * grgb[ch];
+          for (int ch = 0; ch < 3; ++ch) ash[k][ch] += b[k] * g[ch];   // g is 0 on clamped channels
     }
   }
   if (dopacity) dopacity[i] += aop;

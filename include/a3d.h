@@ -220,7 +220,9 @@ size_t a3d_raster_backward_scratch_bytes(const a3d_raster_args* args, int64_t ma
  * (torch.use_deterministic_algorithms of the caller), the render backward reduces the 8 warp partials of a list entry in
  * warp order and stores one 10-float record per (camera, tile, gaussian) pair in the pair's pre-sort slot; a
  * per-(camera, gaussian) kernel sums its slots in slot (= tile) order, and a per-gaussian kernel pushes every camera's
- * gradients through the projection, summing cameras in camera order. */
+ * gradients through the projection, summing cameras in camera order.  With SH colours (colors_precomp NULL),
+ * dL_dmeans3D includes the colour's dependence on the mean through the view direction (mean - campos) / |mean - campos|,
+ * whether or not dL_dshs is requested; channels clamped at 0 in the forward pass no gradient. */
 int a3d_raster_backward(const a3d_raster_args* args, const float* dL_dcolor, const float* dL_ddepth,
                         const float* dL_dalpha, const int32_t* radii, void* workspace, size_t workspace_bytes,
                         int64_t max_rendered, float* dL_dmeans3D, float* dL_dscales, float* dL_drotations,

@@ -223,9 +223,19 @@ def binning(pre: Preprocessed, H: int, W: int):
 
 
 # ------------------------------------------------------------------------------------------------ render (C.3)
-def render(pre: Preprocessed, point_list: np.ndarray, ranges: np.ndarray, H: int, W: int, bg: torch.Tensor):
+def render(pre: Preprocessed, point_list: np.ndarray, ranges: np.ndarray, H: int, W: int, bg: torch.Tensor,
+           stats: Optional[dict] = None):
     """Front-to-back alpha blending per 16x16 tile; differentiable w.r.t. xy / conic / opacity / rgb / depth.
-    Returns color [3,H,W], depth [1,H,W], alpha [1,H,W], n_contrib [H,W] (int64), final_T [H,W]."""
+    Returns color [3,H,W], depth [1,H,W], alpha [1,H,W], n_contrib [H,W] (int64), final_T [H,W].
+
+    With a `stats` dict, also counts which branches the blend took: "alpha_clamped" (contributions whose opacity * G was
+    clamped to 0.99), "stopped" (pixels ended by the T < 1e-4 test), and collects in "near_threshold" (a set) every gaussian
+    with a pixel where its alpha lies within 1e-6 relative of 1/255 or the T after it within 1e-6 relative of 1e-4: there
+    the last bit of exp() decides the branch, so another fp32 implementation may blend that pixel differently."""
+    if stats is not None:
+        stats.setdefault("alpha_clamped", 0)
+        stats.setdefault("stopped", 0)
+        stats.setdefault("near_threshold", set())
     gx, gy = (W + BLOCK - 1) // BLOCK, (H + BLOCK - 1) // BLOCK
     color = torch.zeros(3, H, W) + bg.reshape(3, 1, 1)
     depth = torch.zeros(1, H, W)
@@ -265,6 +275,16 @@ def render(pre: Preprocessed, point_list: np.ndarray, ranges: np.ndarray, H: int
         Tf = torch.where(last_alive > 0, torch.gather(Tfin, 0, (last_alive - 1).clamp(min=0)[None])[0], torch.ones(pxf.shape[1]))
         contrib_idx = torch.where(live & alive, torch.arange(1, len(ids) + 1)[:, None], torch.zeros(1, 1, dtype=torch.int64))
         n_last = contrib_idx.max(0).values
+        if stats is not None:
+            evaluated = (torch.cumsum(stop.to(torch.int64), dim=0) - stop.to(torch.int64)) == 0   # up to the first stop
+            ad, Td = a_raw.detach(), T_after.detach()
+            on_edge = evaluated & (power <= 0) & ((ad - 1.0 / 255.0).abs() <= 1e-6 / 255.0)
+            on_edge |= evaluated & live & ((Td - 1e-4).abs() <= 1e-4 * 1e-6)
+            hit = on_edge.any(1)
+            if bool(hit.any()):
+                stats["near_threshold"].update(ids[hit].tolist())
+            stats["alpha_clamped"] += int((live & alive & (ad > 0.99)).sum())
+            stats["stopped"] += int(stop.any(0).sum())
         rgb = pre.rgb[ids]
         dep = pre.depth[ids]
         C = (w[:, None, :] * rgb[:, :, None]).sum(0) + Tf[None] * bg.reshape(3, 1)

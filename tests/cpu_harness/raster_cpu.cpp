@@ -9,14 +9,32 @@
 
 using namespace a3d;
 
+// colours of every gaussian: the precomputed rgb [P,3], or with colors == nullptr the SH colour (sh_colour) of shs
+// [P, sh_coeffs, 3] at sh_degree seen from campos, with the clamp bits
+static std::vector<float> gaussian_colours(int P, const float* means, const float* colors, const float* shs, int sh_degree,
+                                           int sh_coeffs, const float* campos, std::vector<uint32_t>& clamped) {
+  std::vector<float> col(3 * (size_t)P);
+  clamped.assign(P, 0u);
+  for (int i = 0; i < P; ++i) {
+    if (colors) for (int ch = 0; ch < 3; ++ch) col[3 * i + ch] = colors[3 * i + ch];
+    else clamped[i] = sh_colour(sh_degree, means + 3 * i, campos, shs + (size_t)i * sh_coeffs * 3, &col[3 * i]);
+  }
+  return col;
+}
+
 extern "C" {
 
-// colors: precomputed rgb [P,3].  Returns number of (tile, gaussian) pairs.
+// colors: precomputed rgb [P,3], or nullptr for SH colours (shs, sh_degree, sh_coeffs, campos).  Returns number of
+// (tile, gaussian) pairs.
 long raster_cpu_forward(int P, const float* means, const float* scales, const float* rots, const float* opac, const float* colors,
+                        const float* shs, int sh_degree, int sh_coeffs, const float* campos,
                         const float* vm, const float* pm, float tanfovx, float tanfovy, int H, int W, const float* bg, float mod,
                         float* out_color, float* out_depth, float* out_alpha, int* radii, int* n_contrib, float* final_T,
                         unsigned long long* keys, unsigned int* vals, long cap, long long* ranges, float* pre_dump) {
   const int gx = (W + kTile - 1) / kTile, gy = (H + kTile - 1) / kTile;
+  std::vector<uint32_t> clamped;
+  const std::vector<float> col = gaussian_colours(P, means, colors, shs, sh_degree, sh_coeffs, campos, clamped);
+  colors = col.data();
   std::vector<PreGauss> pre(P);
   std::vector<std::pair<unsigned long long, unsigned int>> kv;
   for (int i = 0; i < P; ++i) {
@@ -70,12 +88,19 @@ long raster_cpu_forward(int P, const float* means, const float* scales, const fl
   return R;
 }
 
+// g_colors receives dL/drgb per gaussian; with SH colours g_shs [P, sh_coeffs, 3] receives dL/dsh and g_means also the
+// view-direction term of the colour (sh_backward)
 void raster_cpu_backward(int P, const float* means, const float* scales, const float* rots, const float* opac, const float* colors,
+                         const float* shs, int sh_degree, int sh_coeffs, const float* campos,
                          const float* vm, const float* pm, float tanfovx, float tanfovy, int H, int W, const float* bg, float mod,
                          const unsigned int* vals, const long long* ranges, const int* n_contrib, const float* final_T,
                          const float* dL_dcolor, const float* dL_ddepth, const float* dL_dalpha,
-                         float* g_means, float* g_scales, float* g_rots, float* g_opac, float* g_colors) {
+                         float* g_means, float* g_scales, float* g_rots, float* g_opac, float* g_colors, float* g_shs) {
   const int gx = (W + kTile - 1) / kTile;
+  std::vector<uint32_t> clamped;
+  const bool sh = colors == nullptr;
+  const std::vector<float> col = gaussian_colours(P, means, colors, shs, sh_degree, sh_coeffs, campos, clamped);
+  colors = col.data();
   std::vector<PreGauss> pre(P);
   for (int i = 0; i < P; ++i) preprocess_gaussian(means + 3 * i, scales + 3 * i, rots + 4 * i, mod, vm, pm, tanfovx, tanfovy, H, W, pre[i]);
   std::vector<float> gcon(3 * (size_t)P, 0.f), gm2(2 * (size_t)P, 0.f), gdep((size_t)P, 0.f);
@@ -113,6 +138,12 @@ void raster_cpu_backward(int P, const float* means, const float* scales, const f
                         gcon[3 * i + 2], gm2[2 * i], gm2[2 * i + 1], gdep[i], dm, ds, dr);
     for (int k = 0; k < 3; ++k) { g_means[3 * i + k] += dm[k]; g_scales[3 * i + k] += ds[k]; }
     for (int k = 0; k < 4; ++k) g_rots[4 * i + k] += dr[k];
+    if (sh) {
+      float g[3] = {g_colors[3 * i], g_colors[3 * i + 1], g_colors[3 * i + 2]}, b[16];
+      sh_backward(sh_degree, means + 3 * i, campos, shs + (size_t)i * sh_coeffs * 3, clamped[i], g, b, g_means + 3 * i);
+      for (int k = 0; k < (sh_degree + 1) * (sh_degree + 1); ++k)
+        for (int ch = 0; ch < 3; ++ch) g_shs[((size_t)i * sh_coeffs + k) * 3 + ch] += b[k] * g[ch];
+    }
   }
 }
 }

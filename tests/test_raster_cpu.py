@@ -10,6 +10,7 @@ import numpy as np
 import pytest
 import torch
 
+import test_raster_backward_oracle_gpu as BW   # the per-gaussian metric and the scene / oracle drivers of the GPU backward tests
 from oracle import raster_oracle as R
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -29,29 +30,35 @@ def fp(a):
     return a.ctypes.data_as(C.c_void_p)
 
 
-def run_harness(lib, xyz, s, q, o, col, wv, full, tf, H, W, bg, grads=None):
+def run_harness(lib, xyz, s, q, o, col, wv, full, tf, H, W, bg, grads=None, sh=None, deg=0, campos=None, mod=1.0):
+    """col: precomputed colours [P,3], or None for SH colours from sh [P,K,3] at degree deg seen from campos."""
     P = xyz.shape[0]
     f = lambda t: np.ascontiguousarray(t.detach().numpy().astype(np.float32))
-    xyz_, s_, q_, o_, col_, wv_, full_ = f(xyz), f(s), f(q), f(o), f(col), f(wv), f(full)
+    xyz_, s_, q_, o_, wv_, full_ = f(xyz), f(s), f(q), f(o), f(wv), f(full)
+    col_ = None if col is None else f(col)
+    sh_ = None if sh is None else f(sh)
+    cp_ = None if campos is None else f(campos)
+    K = 0 if sh is None else sh.shape[1]
     bg_ = f(bg)
+    opt = lambda a: None if a is None else fp(a)
     gx, gy = (W + 15) // 16, (H + 15) // 16
     color = np.zeros((3, H, W), np.float32); depth = np.zeros((H, W), np.float32); alpha = np.zeros((H, W), np.float32)
     radii = np.zeros(P, np.int32); ncon = np.zeros((H, W), np.int32); fT = np.zeros((H, W), np.float32)
     cap = P * gx * gy
     keys = np.zeros(cap, np.uint64); vals = np.zeros(cap, np.uint32); ranges = np.zeros((gx * gy, 2), np.int64)
     pre = np.zeros((P, 8), np.float32)
-    n = lib.raster_cpu_forward(P, fp(xyz_), fp(s_), fp(q_), fp(o_), fp(col_), fp(wv_), fp(full_), C.c_float(tf), C.c_float(tf), H, W,
-                               fp(bg_), C.c_float(1.0), fp(color), fp(depth), fp(alpha), fp(radii), fp(ncon), fp(fT), fp(keys),
+    n = lib.raster_cpu_forward(P, fp(xyz_), fp(s_), fp(q_), fp(o_), opt(col_), opt(sh_), deg, K, opt(cp_), fp(wv_), fp(full_),
+                               C.c_float(tf), C.c_float(tf), H, W, fp(bg_), C.c_float(mod), fp(color), fp(depth), fp(alpha), fp(radii), fp(ncon), fp(fT), fp(keys),
                                fp(vals), C.c_long(cap), fp(ranges), fp(pre))
     res = dict(color=color, depth=depth, alpha=alpha, radii=radii, ncon=ncon, fT=fT, keys=keys[:n], vals=vals[:n], ranges=ranges, pre=pre)
     if grads is not None:
         dC, dD, dA = [np.ascontiguousarray(g.numpy().astype(np.float32)) for g in grads]
         gm = np.zeros((P, 3), np.float32); gs = np.zeros((P, 3), np.float32); gr = np.zeros((P, 4), np.float32)
-        go = np.zeros(P, np.float32); gc = np.zeros((P, 3), np.float32)
-        lib.raster_cpu_backward(P, fp(xyz_), fp(s_), fp(q_), fp(o_), fp(col_), fp(wv_), fp(full_), C.c_float(tf), C.c_float(tf), H, W,
-                                fp(bg_), C.c_float(1.0), fp(vals), fp(ranges), fp(ncon), fp(fT), fp(dC), fp(dD), fp(dA),
-                                fp(gm), fp(gs), fp(gr), fp(go), fp(gc))
-        res.update(gm=gm, gs=gs, gr=gr, go=go, gc=gc)
+        go = np.zeros(P, np.float32); gc = np.zeros((P, 3), np.float32); gsh = np.zeros((P, max(K, 1), 3), np.float32)
+        lib.raster_cpu_backward(P, fp(xyz_), fp(s_), fp(q_), fp(o_), opt(col_), opt(sh_), deg, K, opt(cp_), fp(wv_), fp(full_),
+                                C.c_float(tf), C.c_float(tf), H, W, fp(bg_), C.c_float(mod), fp(vals), fp(ranges), fp(ncon), fp(fT),
+                                fp(dC), fp(dD), fp(dA), fp(gm), fp(gs), fp(gr), fp(go), fp(gc), fp(gsh))
+        res.update(gm=gm, gs=gs, gr=gr, go=go, gc=gc, gsh=gsh)
     return res
 
 
@@ -123,3 +130,118 @@ def test_cam_info_matches_reference_source(golden_dir):
     torch.testing.assert_close(full, torch.stack([c["full"] for c in cams]), rtol=1e-5, atol=1e-6)
     torch.testing.assert_close(centre, torch.stack([c["center"] for c in cams]), rtol=1e-5, atol=1e-6)
     torch.testing.assert_close(tx, torch.tan(torch.tensor([c["fovx"] for c in cams]) * 0.5))
+
+
+# ------------------------------------------------------------------------------------------------ SH colour backward
+
+
+@pytest.mark.parametrize("deg,H,W,mod,seed", [(1, 37, 53, 1.0, 5), (2, 40, 72, 0.8, 6), (3, 45, 30, 1.3, 7)])
+def test_sh_backward_matches_oracle_per_gaussian(harness, deg, H, W, mod, seed):
+    """SH colours at degree 1-3 on non-square images with partial tiles: dmeans3D (with the view-direction term of the
+    colour), dshs, dscales, drotations and dopacity per gaussian against autograd through the oracle.  A third of the
+    (gaussian, channel) colours sit near 0, so the clamp mask is exercised too."""
+    g = torch.Generator().manual_seed(seed)
+    xyz, s, q, o, sh = BW.random_part(500, seed, deg)
+    sh = BW.clamp_dc(sh, 0.3, g)
+    cam = BW._cams(1, seed)
+    wv, full, cp, tf = cam[0]
+    bg = torch.tensor([0.5, 0.3, 0.7])
+    grads = BW.loss_grads(1, H, W, seed)
+    ora = BW.oracle_run((xyz, s, q), o, sh, None, deg, False, cam, H, W, bg, mod, grads)
+    assert int(ora["clamp"].any(-1)[0][ora["radii"][0] > 0].sum()) >= 20, "the colour clamp was not reached"
+    got = run_harness(harness, xyz, s, q, o, None, wv, full, tf, H, W, bg, grads=[t[0] for t in grads], sh=sh, deg=deg,
+                      campos=cp, mod=mod)
+    assert np.array_equal(got["radii"], ora["radii"][0].numpy())
+    ex = BW.excluded_mask(ora, xyz.shape[0])
+    visible = torch.from_numpy(got["radii"] > 0)
+    assert int((ex & visible).sum()) <= BW.MAX_EXCLUDED * int(visible.sum())
+    for name, mine, item in (("means3D", got["gm"], 1), ("shs", got["gsh"], 2), ("scales", got["gs"], 1),
+                             ("rotations", got["gr"], 1), ("opacity", got["go"][:, None], 1)):
+        e = BW.per_gaussian_err(torch.from_numpy(mine), ora["grads"][name], item, ex)
+        assert float(e.max()) <= BW.TAU, f"grad {name}: per-gaussian error {float(e.max()):.3e} at {int(e.argmax())}"
+        assert not np.any(mine[~visible.numpy()]), f"grad {name}: non-zero on a culled gaussian"
+
+
+# ------------------------------------------------------------------------------------------------ negative controls
+# The per-gaussian metric must flag each of these mutations of the oracle's own gradients by at least 10x its tolerance.
+def _controls_scene(deg, seed, n=400):
+    xyz, s, q, o, sh = BW.random_part(n, seed, deg)
+    return xyz, s, q, o, sh
+
+
+def test_metric_flags_detached_sh_direction():
+    deg, H, W = 1, 40, 56
+    xyz, s, q, o, sh = _controls_scene(deg, 11)
+    cams = BW._cams(1, 11)
+    grads = BW.loss_grads(1, H, W, 11)
+    bg = torch.zeros(3)
+    ref = BW.oracle_run((xyz, s, q), o, sh, None, deg, False, cams, H, W, bg, 1.0, grads)
+    # the same colours with the view direction detached: the mean gradient misses the colour's direction term
+    cp = cams[0][2]
+    m = xyz.clone().requires_grad_(True)
+    d = (m - cp[None]).detach()
+    col = torch.clamp(R.eval_sh(deg, sh, d / d.norm(dim=-1, keepdim=True)) + 0.5, min=0)
+    mut = BW.oracle_run((xyz, s, q), o, None, col, deg, False, cams, H, W, bg, 1.0, grads)
+    e = BW.per_gaussian_err(mut["grads"]["means3D"], ref["grads"]["means3D"])
+    assert float(e.max()) >= 10 * BW.TAU, float(e.max())
+
+
+def test_metric_flags_swapped_means2D_scale():
+    H, W = 40, 72
+    xyz, s, q, o, sh = _controls_scene(0, 12)
+    cams = BW._cams(1, 12)
+    grads = BW.loss_grads(1, H, W, 12)
+    col = torch.clamp(R.SH_C0 * sh[:, 0] + 0.5, min=0)
+    ref = BW.oracle_run((xyz, s, q), o, None, col, 0, False, cams, H, W, torch.zeros(3), 1.0, grads)
+    mut = BW.oracle_run((xyz, s, q), o, None, col, 0, False, cams, H, W, torch.zeros(3), 1.0, grads, means2D_scale=(H / 2, W / 2))
+    e = BW.per_gaussian_err(mut["grads"]["means2D"], ref["grads"]["means2D"])
+    assert float(e.max()) >= 10 * BW.TAU, float(e.max())
+
+
+def test_metric_flags_ignored_colour_clamp():
+    deg, H, W = 1, 40, 56
+    g = torch.Generator().manual_seed(13)
+    xyz, s, q, o, sh = _controls_scene(deg, 13)
+    sh = BW.clamp_dc(sh, 0.4, g)
+    cams = BW._cams(1, 13)
+    grads = BW.loss_grads(1, H, W, 13)
+    bg = torch.zeros(3)
+    ref = BW.oracle_run((xyz, s, q), o, sh, None, deg, False, cams, H, W, bg, 1.0, grads)
+    # the forward keeps the clamp; the backward lets the gradient through clamped channels
+    shl = sh.clone().requires_grad_(True)
+    m = xyz.clone().requires_grad_(True)
+    d = m - cams[0][2][None]
+    raw = R.eval_sh(deg, shl, d / torch.sqrt((d[:, 0] * d[:, 0] + d[:, 1] * d[:, 1]) + d[:, 2] * d[:, 2])[:, None]) + 0.5
+    col = raw + (torch.clamp(raw, min=0) - raw).detach()
+    mut = BW.oracle_run((xyz, s, q), o, None, col.detach(), deg, False, cams, H, W, bg, 1.0, grads)
+    col.backward(mut["grads"]["colors"])
+    e = BW.per_gaussian_err(shl.grad, ref["grads"]["shs"], 2)
+    assert float(e.max()) >= 10 * BW.TAU, float(e.max())
+
+
+def test_metric_flags_one_dropped_camera_contribution():
+    H, W = 40, 56
+    xyz, s, q, o, sh = _controls_scene(0, 14)
+    col = torch.clamp(R.SH_C0 * sh[:, 0] + 0.5, min=0)
+    cams = BW._cams(3, 14)
+    grads = BW.loss_grads(3, H, W, 14)
+    bg = torch.zeros(3)
+    ref = BW.oracle_run((xyz, s, q), o, None, col, 0, False, cams, H, W, bg, 1.0, grads)
+    cam0 = BW.oracle_run((xyz, s, q), o, None, col, 0, False, cams[:1], H, W, bg, 1.0, [t[:1] for t in grads])
+    # drop camera 0's part of the mean gradient of one gaussian seen by every camera (the median one by gradient size)
+    seen = torch.nonzero((ref["radii"] > 0).all(0)).reshape(-1)
+    i = int(seen[ref["grads"]["means3D"][seen].norm(dim=-1).argsort()[len(seen) // 2]])
+    mut = ref["grads"]["means3D"].clone()
+    mut[i] -= cam0["grads"]["means3D"][i]
+    e = BW.per_gaussian_err(mut, ref["grads"]["means3D"])
+    assert float(e.max()) >= 10 * BW.TAU, float(e.max())
+
+
+def test_metric_flags_scale_modifier_applied_twice():
+    H, W, mod = 40, 56, 0.6
+    xyz, s, q, o, sh = _controls_scene(0, 15)
+    col = torch.clamp(R.SH_C0 * sh[:, 0] + 0.5, min=0)
+    cams = BW._cams(1, 15)
+    ref = BW.oracle_run((xyz, s, q), o, None, col, 0, False, cams, H, W, torch.zeros(3), mod, BW.loss_grads(1, H, W, 15))
+    e = BW.per_gaussian_err(ref["grads"]["scales"] * mod, ref["grads"]["scales"])
+    assert float(e.max()) >= 10 * BW.TAU, float(e.max())

@@ -165,7 +165,16 @@ def test_reference_style_api_and_sh_colour():
     assert color.shape == (3, H, W) and radii.shape == (P,) and depth.shape == (1, H, W) and alpha.shape == (1, H, W)
     torch.testing.assert_close(color.cpu(), ora["color"], rtol=1e-4, atol=5e-5)
     color.sum().backward()
-    assert m2.grad is not None and m2.grad.abs().sum() > 0 and shc.grad.abs().sum() > 0
+    # dshs and the screen-space (NDC) means2D gradient per gaussian against autograd through the oracle
+    from test_raster_backward_oracle_gpu import TAU, oracle_run, per_gaussian_err
+    ref = oracle_run((xyz, s, q), o, sh, None, 2, False, raw, H, W, bg, 1.0,
+                     (torch.ones(1, 3, H, W), torch.zeros(1, 1, H, W), torch.zeros(1, 1, H, W)))
+    ex = torch.zeros(P, dtype=torch.bool)
+    ex[list(ref["stats"]["near_threshold"])] = True
+    assert int(ex.sum()) <= 0.005 * P
+    assert float(per_gaussian_err(shc.grad, ref["grads"]["shs"], 2, ex).max()) <= TAU
+    assert float(per_gaussian_err(m2.grad, ref["grads"]["means2D"][0], 1, ex).max()) <= TAU
+    assert m2.grad.abs().sum() > 0 and shc.grad.abs().sum() > 0
     with pytest.raises(Exception):
         GaussianRasterizer(settings[0])(xyz.cuda(), m2, o.cuda(), scales=s.cuda(), rotations=q.cuda())
 
