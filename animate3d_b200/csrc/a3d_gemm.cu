@@ -91,9 +91,41 @@ __device__ __forceinline__ void wgmma_tile(float (&d)[BN / 2], uint64_t adesc, u
 // EPI: 0 = bias/row-bias only, 1 = + residuals / row permutation, 2 = GEGLU, 3 = fp32 output
 enum { kEpiPlain = 0, kEpiRes = 1, kEpiGeglu = 2, kEpiF32 = 3 };
 
+// The epilogue walks a thread's 8-column groups in chunks of G groups, both of its rows at once.  All global operands of a
+// chunk are requested together, and (kAhead) those of the next chunk before the current one is stored, so a thread waits for
+// memory once per chunk rather than once per group and row.  A GEGLU chunk holds G / 2 value groups and their gates.  The
+// operands sit in registers next to the accumulators, and a 288-thread CTA puts three warps on one SM sub-partition, which
+// caps a thread at 168 registers.  At BN = 256 the 128 accumulator registers leave room for one chunk's operands only, so
+// there the next chunk is requested after the current one is stored.  Residual rows are fetched into L2 ahead of the
+// epilogue at every BN (see the main loop).
+template <int BN, int EPI>
+struct EpiChunk {
+  static constexpr int G = BN == 256 ? 1 + (EPI == kEpiGeglu) : 2;
+  static constexpr bool kAhead = BN != 256;
+  float bias[G][2];
+  float rb[2][G][2];                  // [row][group][column]
+  uint32_t r1[2][G], r2[2][G];        // fp16x2 residuals (kEpiRes only)
+};
+
+// accumulator group (8 columns) of slot s of chunk c; GEGLU: slots < G / 2 hold values u of output group o, the others
+// their gates, 4 groups further (the accumulator columns come as (u[32] | g[32]) blocks)
+template <int EPI, int G>
+__device__ __forceinline__ constexpr int epi_group(int c, int s) {
+  if constexpr (EPI != kEpiGeglu) {
+    return c * G + s;
+  } else {
+    const int o = c * (G / 2) + s % (G / 2);
+    return (o / 4) * 8 + o % 4 + (s >= G / 2 ? 4 : 0);
+  }
+}
+
+__device__ __forceinline__ void prefetch_l2(const void* a) { asm volatile("prefetch.global.L2 [%0];" ::"l"(a)); }
+
 template <int BN, int EPI>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_tc_kernel(const GemmDev p, const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB) {
+  static_assert(EPI != kEpiGeglu || BN % 64 == 0, "GEGLU pairs a value with its gate inside 64-column blocks");
+  static_assert((BN / 8) % EpiChunk<BN, EPI>::G == 0, "the tile's column groups split into whole chunks");
   using Cfg = GemmCfg<BN>;
   constexpr int kStages = Cfg::kStages;
   extern __shared__ uint8_t smem_raw[];
@@ -161,9 +193,40 @@ gemm_tc_kernel(const GemmDev p, const __grid_constant__ CUtensorMap mapA, const 
     const int mt = tile / p.tiles_n, nt = tile % p.tiles_n;
     const bool tr = p.trace && blockIdx.x == 0 && threadIdx.x == 0 && tcount < 60;
     if (tr) p.trace[tcount * 16 + 0] = clock64();
+    // epilogue rows of this thread: row[h] = 16 w + g + 8 h of the warpgroup's 64; group j = columns 8 j + 2 t, +1.
+    // R2 and C are read / written at the same (orow, n) by the same thread, so R2 may be C.  R1 is read at (row, n), which
+    // another thread writes when the rows are permuted: R1 must not alias C then (see a3d.h).
+    const int64_t col_base = (int64_t)nt * BN + 2 * t;
+    int64_t row[2], orow[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      row[h] = (int64_t)mt * kBM + wg * 64 + (warp & 3) * 16 + g + 8 * h;
+      orow[h] = (EPI == kEpiRes) ? perm_row(row[h], p.perm_a, p.perm_b) : row[h];
+    }
     // ---- main loop: one wgmma group in flight; the stage of k-block kb-1 is released once group kb-1 has retired
     int prev_stage = -1;
     for (int kb = 0; kb < p.num_k_blocks; ++kb) {
+      if constexpr (EPI == kEpiRes) {
+        // the residual rows of this tile into L2 two k-blocks before the epilogue reads them: far enough ahead to cover an
+        // HBM miss, close enough that the operand stream of a long-K tile does not evict them first.  The four lanes of a
+        // row take its 128-byte lines t, t + 4 (a row's BN halves span at most 2 BN / 128 + 1 lines).
+        if (kb == (p.num_k_blocks > 2 ? p.num_k_blocks - 2 : 0)) {
+          const int64_t ncols = p.N - (int64_t)nt * BN < BN ? p.N - (int64_t)nt * BN : BN;
+          auto fetch = [&](const __half* a, bool ok) {
+            const uintptr_t e = reinterpret_cast<uintptr_t>(a + ncols), l0 = reinterpret_cast<uintptr_t>(a) & ~uintptr_t(127);
+#pragma unroll
+            for (int i = 0; i < (2 * BN / 128 + 4) / 4; ++i) {
+              const uintptr_t l = l0 + 128 * (t + 4 * i);
+              if (ok && l < e) prefetch_l2(reinterpret_cast<const void*>(l));
+            }
+          };
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            fetch(p.R1 + row[h] * p.ldr1 + (int64_t)nt * BN, p.R1 && row[h] < p.M);
+            fetch(p.R2 + orow[h] * p.ldr2 + (int64_t)nt * BN, p.R2 && row[h] < p.M);
+          }
+        }
+      }
       mbar_wait(&full_bar[stage], phase);
       const uint32_t a0 = smem_u32(smem_a + stage * Cfg::kABytes + wg * (64 * 128));
       const uint32_t b0 = smem_u32(smem_b + stage * Cfg::kBBytes);
@@ -178,64 +241,128 @@ gemm_tc_kernel(const GemmDev p, const __grid_constant__ CUtensorMap mapA, const 
       prev_stage = stage;
       if (++stage == kStages) { stage = 0; phase ^= 1; }
     }
+
+    // ---- epilogue from registers, chunk by chunk (EpiChunk): chunk c covers groups epi_group(c, 0 .. G - 1) of both rows
+    using Chunk = EpiChunk<BN, EPI>;
+    constexpr int G = Chunk::G;
+    constexpr int kChunks = BN / 8 / G;
+    const float* rb[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) rb[h] = p.rowbias ? p.rowbias + ((row[h] / p.rb_div) % p.rb_mod) * p.rb_ld : nullptr;
+    Chunk op;
+    auto load_chunk = [&](int c) {
+#pragma unroll
+      for (int s = 0; s < G; ++s) {
+        const int64_t n = col_base + 8 * epi_group<EPI, G>(c, s);
+        const bool col_ok = n < p.N;
+        // coherent loads, unlike __ldg: they cannot be hoisted above the previous chunk's stores, which would hold the
+        // operands of every chunk in registers at once
+        op.bias[s][0] = (p.bias && col_ok) ? p.bias[n] : 0.f;
+        op.bias[s][1] = (p.bias && col_ok) ? p.bias[n + 1] : 0.f;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const bool ok = col_ok && row[h] < p.M;
+          op.rb[h][s][0] = (rb[h] && ok) ? rb[h][n] : 0.f;
+          op.rb[h][s][1] = (rb[h] && ok) ? rb[h][n + 1] : 0.f;
+          if constexpr (EPI == kEpiRes) {
+            op.r1[h][s] = (p.R1 && ok) ? *reinterpret_cast<const uint32_t*>(p.R1 + row[h] * p.ldr1 + n) : 0u;
+            op.r2[h][s] = (p.R2 && ok) ? *reinterpret_cast<const uint32_t*>(p.R2 + orow[h] * p.ldr2 + n) : 0u;
+          }
+        }
+      }
+    };
+    // same order as the SIMT kernel: (acc + bias + row-bias) * acc_scale, then + r1_scale R1, + R2
+    auto finish = [&](float v, int h, int s, int e) {
+      if (p.bias) v += op.bias[s][e];
+      if (rb[h]) v += op.rb[h][s][e];
+      return v * p.acc_scale;
+    };
+    auto half2_float2 = [](uint32_t u) { return __half22float2(*reinterpret_cast<const __half2*>(&u)); };
+
+    if constexpr (Chunk::kAhead) load_chunk(0);   // under the last MMA group
     wgmma_wait<0>();
     reg_fence(acc);
     if (lane == 0) mbar_arrive(&empty_bar[prev_stage]);
     if (tr) p.trace[tcount * 16 + 1] = clock64();
 
-    // ---- epilogue from registers: row r_h = 16 w + g + 8 h of the warpgroup's 64 rows; columns 8 j + 2 t, +1
-    const int64_t col_base = (int64_t)nt * BN + 2 * t;
 #pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const int64_t row = (int64_t)mt * kBM + wg * 64 + (warp & 3) * 16 + g + 8 * h;
-      if (row >= p.M) continue;
-      const float* rb = p.rowbias ? p.rowbias + ((row / p.rb_div) % p.rb_mod) * p.rb_ld : nullptr;
-      auto finish = [&](float v, int64_t n) {
-        if (p.bias) v += __ldg(p.bias + n);
-        if (rb) v += __ldg(rb + n);
-        return v * p.acc_scale;
-      };
+    for (int c = 0; c < kChunks; ++c) {
+      if constexpr (!Chunk::kAhead) load_chunk(c);
       if constexpr (EPI == kEpiGeglu) {
-        // accumulator columns come as (u[32] | g[32]) blocks: n-block j (j % 8 < 4) holds u, n-block j + 4 its gate
-        __half* crow = reinterpret_cast<__half*>(p.C) + row * p.ldc;
+        uint32_t out[2][G / 2];
 #pragma unroll
-        for (int j = 0; j < BN / 8; ++j) {
-          if ((j & 7) >= 4) continue;
-          const int64_t n = col_base + 8 * j;
-          if (n >= p.N) continue;
-          const float u0 = finish(acc[4 * j + 2 * h], n), u1 = finish(acc[4 * j + 2 * h + 1], n + 1);
-          const float g0 = finish(acc[4 * (j + 4) + 2 * h], n + 32), g1 = finish(acc[4 * (j + 4) + 2 * h + 1], n + 33);
-          const int64_t oc = (int64_t)nt * (BN / 2) + (j >> 3) * 32 + 8 * (j & 7) + 2 * t;
-          *reinterpret_cast<uint32_t*>(crow + oc) = pack_f16x2(u0 * gelu_erf(g0), u1 * gelu_erf(g1));
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+          for (int s = 0; s < G / 2; ++s) {
+            const int ju = epi_group<EPI, G>(c, s), jg = epi_group<EPI, G>(c, s + G / 2);
+            const float u0 = finish(acc[4 * ju + 2 * h], h, s, 0), u1 = finish(acc[4 * ju + 2 * h + 1], h, s, 1);
+            const float g0 = finish(acc[4 * jg + 2 * h], h, s + G / 2, 0), g1 = finish(acc[4 * jg + 2 * h + 1], h, s + G / 2, 1);
+            out[h][s] = pack_f16x2(u0 * gelu_erf(g0), u1 * gelu_erf(g1));
+          }
+        if (Chunk::kAhead && c + 1 < kChunks) load_chunk(c + 1);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          if (row[h] >= p.M) continue;
+          __half* crow = reinterpret_cast<__half*>(p.C) + row[h] * p.ldc;
+#pragma unroll
+          for (int s = 0; s < G / 2; ++s) {
+            if (col_base + 8 * epi_group<EPI, G>(c, s) >= p.N) continue;
+            const int o = c * (G / 2) + s;   // output group: columns 8 o + 2 t, +1 of the tile's BN / 2
+            *reinterpret_cast<uint32_t*>(crow + (int64_t)nt * (BN / 2) + 8 * o + 2 * t) = out[h][s];
+          }
         }
       } else if constexpr (EPI == kEpiF32) {
-        float* crow = reinterpret_cast<float*>(p.C) + row * p.ldc;
+        float out[2][G][2];
 #pragma unroll
-        for (int j = 0; j < BN / 8; ++j) {
-          const int64_t n = col_base + 8 * j;
-          if (n >= p.N) continue;
-          crow[n] = finish(acc[4 * j + 2 * h], n);
-          crow[n + 1] = finish(acc[4 * j + 2 * h + 1], n + 1);
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+          for (int s = 0; s < G; ++s)
+#pragma unroll
+            for (int e = 0; e < 2; ++e) out[h][s][e] = finish(acc[4 * (c * G + s) + 2 * h + e], h, s, e);
+        if (Chunk::kAhead && c + 1 < kChunks) load_chunk(c + 1);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          if (row[h] >= p.M) continue;
+          float* crow = reinterpret_cast<float*>(p.C) + row[h] * p.ldc;
+#pragma unroll
+          for (int s = 0; s < G; ++s) {
+            const int64_t n = col_base + 8 * (c * G + s);
+            if (n >= p.N) continue;
+            crow[n] = out[h][s][0];
+            crow[n + 1] = out[h][s][1];
+          }
         }
       } else {
-        const int64_t orow = (EPI == kEpiRes) ? perm_row(row, p.perm_a, p.perm_b) : row;
-        __half* crow = reinterpret_cast<__half*>(p.C) + orow * p.ldc;
+        uint32_t out[2][G];
 #pragma unroll
-        for (int j = 0; j < BN / 8; ++j) {
-          const int64_t n = col_base + 8 * j;
-          if (n >= p.N) continue;
-          float v0 = finish(acc[4 * j + 2 * h], n), v1 = finish(acc[4 * j + 2 * h + 1], n + 1);
-          if constexpr (EPI == kEpiRes) {
-            if (p.R1) {
-              const float2 f = __half22float2(*reinterpret_cast<const __half2*>(p.R1 + row * p.ldr1 + n));
-              v0 += p.r1_scale * f.x; v1 += p.r1_scale * f.y;
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+          for (int s = 0; s < G; ++s) {
+            const int j = c * G + s;
+            float v0 = finish(acc[4 * j + 2 * h], h, s, 0), v1 = finish(acc[4 * j + 2 * h + 1], h, s, 1);
+            if constexpr (EPI == kEpiRes) {
+              if (p.R1) {
+                const float2 f = half2_float2(op.r1[h][s]);
+                v0 += p.r1_scale * f.x; v1 += p.r1_scale * f.y;
+              }
+              if (p.R2) {
+                const float2 f = half2_float2(op.r2[h][s]);
+                v0 += f.x; v1 += f.y;
+              }
             }
-            if (p.R2) {
-              const float2 f = __half22float2(*reinterpret_cast<const __half2*>(p.R2 + orow * p.ldr2 + n));
-              v0 += f.x; v1 += f.y;
-            }
+            out[h][s] = pack_f16x2(v0, v1);
           }
-          *reinterpret_cast<uint32_t*>(crow + n) = pack_f16x2(v0, v1);
+        if (Chunk::kAhead && c + 1 < kChunks) load_chunk(c + 1);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          if (row[h] >= p.M) continue;
+          __half* crow = reinterpret_cast<__half*>(p.C) + orow[h] * p.ldc;
+#pragma unroll
+          for (int s = 0; s < G; ++s) {
+            const int64_t n = col_base + 8 * (c * G + s);
+            if (n >= p.N) continue;
+            *reinterpret_cast<uint32_t*>(crow + n) = out[h][s];
+          }
         }
       }
     }
@@ -314,7 +441,10 @@ static int launch_tc_epi(const GemmDev& dev, const CUtensorMap* mapA, const CUte
 template <int BN>
 static int launch_tc(const GemmDev& dev, const CUtensorMap* mapA, const CUtensorMap* mapB, cudaStream_t st) {
   if (dev.out_f32) return launch_tc_epi<BN, kEpiF32>(dev, mapA, mapB, st);
-  if (dev.geglu) return launch_tc_epi<BN, kEpiGeglu>(dev, mapA, mapB, st);
+  if (dev.geglu) {
+    if constexpr (BN % 64 == 0) return launch_tc_epi<BN, kEpiGeglu>(dev, mapA, mapB, st);
+    else return fail(A3D_EINVAL, "a3d_gemm: GEGLU needs a 128- or 256-column tile");
+  }
   if (dev.R1 || dev.R2 || dev.perm_a) return launch_tc_epi<BN, kEpiRes>(dev, mapA, mapB, st);
   return launch_tc_epi<BN, kEpiPlain>(dev, mapA, mapB, st);
 }

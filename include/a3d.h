@@ -66,8 +66,10 @@ typedef struct a3d_gemm_args {
   const float* rowbias;       /* [rb_rows, rb_ld] or NULL */
   int64_t rb_ld, rb_div, rb_mod;
   float acc_scale;            /* multiplies the accumulator: MUST be set (1.0 if unused; 0.0 is honoured, not remapped) */
-  const void* R1; int64_t ldr1; float r1_scale;   /* fp16 or NULL */
-  const void* R2; int64_t ldr2;                   /* fp16 or NULL */
+  const void* R1; int64_t ldr1; float r1_scale;   /* fp16 or NULL; read at the unpermuted row m: it may alias C only
+                                                     when perm_a == 0 (with a permutation another row's store can land
+                                                     on R1[m, n] before it is read) */
+  const void* R2; int64_t ldr2;                   /* fp16 or NULL; read at the output element om, n itself: may be C */
   int geglu;
   int out_f32;
   int64_t perm_a, perm_b;     /* 0,0 = identity */
