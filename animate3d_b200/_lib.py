@@ -13,6 +13,8 @@ LIB_PATH = os.path.join(_HERE, "liba3d.so")
 
 A_PLAIN, A_CONV3 = 0, 1
 IMPL_AUTO, IMPL_TC, IMPL_SIMT = 0, 1, 2
+EPI_GEGLU, EPI_GELU = 1, 2                       # a3d_gemm_args.geglu
+CLIP_SRC_F32_NCHW, CLIP_SRC_U8_NHWC, CLIP_SRC_PIXELS = 0, 1, 2
 
 
 class GemmArgs(C.Structure):
@@ -43,6 +45,14 @@ class AttnArgs(C.Structure):
                 ("heads", C.c_int), ("d", C.c_int), ("scale", C.c_float),
                 ("kv_div", C.c_int), ("kv_i3_zero", C.c_int),
                 ("accumulate", C.c_int), ("out_scale", C.c_float), ("impl", C.c_int)]
+
+
+class ClipPrepArgs(C.Structure):
+    _fields_ = [("src", C.c_void_p), ("src_format", C.c_int), ("n", C.c_int), ("h", C.c_int), ("w", C.c_int),
+                ("resize_h", C.c_int), ("resize_w", C.c_int),
+                ("bounds_y", C.c_void_p), ("coeffs_y", C.c_void_p), ("ksize_y", C.c_int),
+                ("bounds_x", C.c_void_p), ("coeffs_x", C.c_void_p), ("ksize_x", C.c_int),
+                ("patches", C.c_void_p), ("pixel_values", C.c_void_p)]
 
 
 class RasterCam(C.Structure):
@@ -89,6 +99,8 @@ def load(require_gpu: bool = True) -> C.CDLL:
         lib.a3d_mesh_vertex_stats_scratch_bytes.argtypes = [C.c_int, C.c_int, C.c_int]
         lib.a3d_mesh_sample_neighbors.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_uint64, C.c_uint64, C.c_void_p,
                                                   C.c_void_p]
+        lib.a3d_clip_resize_plan.argtypes = [C.c_int, C.c_int] + [C.POINTER(C.c_int)] * 4
+        lib.a3d_clip_resize_coeffs.argtypes = [C.c_int, C.c_int, C.c_void_p, C.c_void_p]
         _lib = lib
     if require_gpu and not _inited:
         if not torch.cuda.is_available():

@@ -14,7 +14,7 @@ CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "liba3d.so")
 OBJ = os.path.join(HERE, "build")
 SOURCES = ["a3d_api.cu", "a3d_gemm.cu", "a3d_attn.cu", "a3d_ops.cu", "a3d_raster.cu", "a3d_raster_pre.cu", "a3d_deform.cu", "a3d_arap.cu",
-           "a3d_mesh.cu"]
+           "a3d_mesh.cu", "a3d_clip.cu"]
 # index-defining rasterizer arithmetic must not be contracted into FMAs (bit parity with oracle/raster_oracle.py)
 EXTRA = {"a3d_raster_pre.cu": ["--fmad=false"]}
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")

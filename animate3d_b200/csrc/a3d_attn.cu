@@ -24,7 +24,7 @@ struct AttnDev {
   int q_tiles, kv_tiles;
   int rows_q, rows_k;            // valid rows per q tile (<= 128) / in the LAST kv tile (<= 64)
   int heads;
-  int q_t1, q_box1, q_box2, q_e3;
+  int q_t1, q_box1, q_box2, q_e1, q_e3;   // q_e1: rows at or past it belong to the next batch (ragged last query tile)
   int k_t1, k_box1, k_box2, k_e3, kv_div, kv_i3_zero;
   uint32_t q_box_bytes, k_box_bytes;   // bytes one 64-column TMA box delivers
   float scale_log2;
@@ -230,9 +230,9 @@ attn_tc_kernel(const AttnDev p, const __grid_constant__ CUtensorMap mapQ, const 
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
     const int r = wg * 64 + (warp & 3) * 16 + g + 8 * h;
-    if (r >= p.rows_q) continue;
-    const float inv = p.out_scale / (h ? l_hi : l_lo);
     const int i1 = q_i1 + r % p.q_box1;
+    if (r >= p.rows_q || i1 >= p.q_e1) continue;   // rows TMA zero-filled past e1 are computed but never stored
+    const float inv = p.out_scale / (h ? l_hi : l_lo);
     const int i2 = q_i2 + r / p.q_box1;
     __half* orow = p.out + (int64_t)i1 * p.os1 + (int64_t)i2 * p.os2 + (int64_t)q_i3 * p.os3 + (int64_t)q_i4 * p.os4 +
                    head * D + 2 * t;
@@ -570,8 +570,10 @@ static int launch_shortkeys(const a3d_attn_args* a, int dqk, int dv, int kv_div,
 
 static int tile_geom(const a3d_view5& v, int* box1, int* box2, int* t1, int* tiles, int* rows) {
   if (v.e1 >= 128) {
-    if (v.e1 % 128) return fail(A3D_EINVAL, "a3d_attention: inner extent %d must be a multiple of 128", v.e1);
-    *box1 = 128; *box2 = 1; *t1 = v.e1 / 128; *tiles = *t1 * v.e2; *rows = 128;
+    // a ragged last tile reads rows past e1 as TMA's zero fill; with e2 > 1 they would be the next i2's rows instead
+    if ((v.e1 % 128) && v.e2 != 1)
+      return fail(A3D_EINVAL, "a3d_attention: inner extent %d is not a multiple of 128 and needs e2 == 1 (got %d)", v.e1, v.e2);
+    *box1 = 128; *box2 = 1; *t1 = (v.e1 + 127) / 128; *tiles = *t1 * v.e2; *rows = 128;
   } else {
     int b2 = 128 / v.e1;
     if (b2 > v.e2) b2 = v.e2;
@@ -704,7 +706,7 @@ extern "C" int a3d_attention(const a3d_attn_args* a, void* stream) {
   if (int r = tile_geom(a->q, &qb1, &qb2, &qt1, &qtiles, &qrows)) return r;
   dev.q_tiles = qtiles; dev.rows_q = qrows;
   dev.heads = a->heads;
-  dev.q_t1 = qt1; dev.q_box1 = qb1; dev.q_box2 = qb2; dev.q_e3 = a->q.e3;
+  dev.q_t1 = qt1; dev.q_box1 = qb1; dev.q_box2 = qb2; dev.q_e1 = a->q.e1; dev.q_e3 = a->q.e3;
   dev.k_e3 = a->k.e3;
   dev.kv_div = kv_div; dev.kv_i3_zero = a->kv_i3_zero;
   dev.q_box_bytes = 128u * qrows;

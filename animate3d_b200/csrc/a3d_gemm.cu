@@ -88,8 +88,8 @@ __device__ __forceinline__ void wgmma_tile(float (&d)[BN / 2], uint64_t adesc, u
   else wgmma_ss_n128<0>(d, adesc, bdesc, acc);
 }
 
-// EPI: 0 = bias/row-bias only, 1 = + residuals / row permutation, 2 = GEGLU, 3 = fp32 output
-enum { kEpiPlain = 0, kEpiRes = 1, kEpiGeglu = 2, kEpiF32 = 3 };
+// EPI: 0 = bias/row-bias only, 1 = + residuals / row permutation, 2 = GEGLU, 3 = fp32 output, 4 = GELU of the biased value
+enum { kEpiPlain = 0, kEpiRes = 1, kEpiGeglu = 2, kEpiF32 = 3, kEpiGelu = 4 };
 
 // The epilogue walks a thread's 8-column groups in chunks of G groups, both of its rows at once.  All global operands of a
 // chunk are requested together, and (kAhead) those of the next chunk before the current one is stored, so a thread waits for
@@ -340,6 +340,9 @@ gemm_tc_kernel(const GemmDev p, const __grid_constant__ CUtensorMap mapA, const 
           for (int s = 0; s < G; ++s) {
             const int j = c * G + s;
             float v0 = finish(acc[4 * j + 2 * h], h, s, 0), v1 = finish(acc[4 * j + 2 * h + 1], h, s, 1);
+            if constexpr (EPI == kEpiGelu) {
+              v0 = gelu_erf(v0); v1 = gelu_erf(v1);
+            }
             if constexpr (EPI == kEpiRes) {
               if (p.R1) {
                 const float2 f = half2_float2(op.r1[h][s]);
@@ -377,7 +380,7 @@ struct SimtConv { int n, h, w, c, s, oh, ow, pad; };
 
 __global__ void gemm_simt_kernel(const GemmDev p, const __half* __restrict__ A, int64_t lda, const __half* __restrict__ B,
                                  SimtConv cv) {
-  const int64_t n_out = p.geglu ? p.N / 2 : p.N;
+  const int64_t n_out = p.geglu == 1 ? p.N / 2 : p.N;
   const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= p.M * n_out) return;
   const int64_t m = idx / n_out;
@@ -409,7 +412,7 @@ __global__ void gemm_simt_kernel(const GemmDev p, const __half* __restrict__ A, 
     if (rb) v += rb[n];
     return v * p.acc_scale;
   };
-  if (p.geglu) {
+  if (p.geglu == 1) {
     const int64_t blk = j / 32, e = j % 32;
     const int64_t nu = blk * 64 + e, ng = nu + 32;
     const float u = finish(nu), g = finish(ng);
@@ -417,6 +420,7 @@ __global__ void gemm_simt_kernel(const GemmDev p, const __half* __restrict__ A, 
     return;
   }
   float v = finish(j);
+  if (p.geglu == 2) v = gelu_erf(v);
   if (p.R1) v += p.r1_scale * __half2float(p.R1[m * p.ldr1 + j]);
   if (p.R2) v += __half2float(p.R2[orow * p.ldr2 + j]);
   if (p.out_f32) reinterpret_cast<float*>(p.C)[orow * p.ldc + j] = v;
@@ -441,10 +445,11 @@ static int launch_tc_epi(const GemmDev& dev, const CUtensorMap* mapA, const CUte
 template <int BN>
 static int launch_tc(const GemmDev& dev, const CUtensorMap* mapA, const CUtensorMap* mapB, cudaStream_t st) {
   if (dev.out_f32) return launch_tc_epi<BN, kEpiF32>(dev, mapA, mapB, st);
-  if (dev.geglu) {
+  if (dev.geglu == 1) {
     if constexpr (BN % 64 == 0) return launch_tc_epi<BN, kEpiGeglu>(dev, mapA, mapB, st);
     else return fail(A3D_EINVAL, "a3d_gemm: GEGLU needs a 128- or 256-column tile");
   }
+  if (dev.geglu == 2) return launch_tc_epi<BN, kEpiGelu>(dev, mapA, mapB, st);
   if (dev.R1 || dev.R2 || dev.perm_a) return launch_tc_epi<BN, kEpiRes>(dev, mapA, mapB, st);
   return launch_tc_epi<BN, kEpiPlain>(dev, mapA, mapB, st);
 }
@@ -477,8 +482,12 @@ extern "C" int a3d_gemm(const a3d_gemm_args* a, void* stream) {
   d.C = a->C; d.ldc = a->ldc; d.geglu = a->geglu; d.out_f32 = a->out_f32;
   d.perm_a = a->perm_a; d.perm_b = a->perm_b;
   d.trace = g_gemm_trace;
-  if (a->geglu && (a->out_f32 || a->R1 || a->R2 || a->perm_a || (a->N % 128)))
+  if (a->geglu < 0 || a->geglu > 2) return fail(A3D_EINVAL, "a3d_gemm: geglu must be 0 (none), 1 (GEGLU) or 2 (GELU)");
+  const bool geglu = a->geglu == 1;
+  if (geglu && (a->out_f32 || a->R1 || a->R2 || a->perm_a || (a->N % 128)))
     return fail(A3D_EINVAL, "a3d_gemm: GEGLU epilogue takes bias / row-bias only, fp16 output, N %% 128 == 0");
+  if (a->geglu == 2 && (a->out_f32 || a->R1 || a->R2 || a->perm_a))
+    return fail(A3D_EINVAL, "a3d_gemm: GELU epilogue takes bias / row-bias only, fp16 output");
   if (a->out_f32 && (a->R1 || a->R2 || a->perm_a))
     return fail(A3D_EINVAL, "a3d_gemm: fp32 output supports bias / row-bias only");
 
@@ -496,7 +505,7 @@ extern "C" int a3d_gemm(const a3d_gemm_args* a, void* stream) {
   }
 
   // ---- can the tensor-core path take it?
-  bool tc_ok = (a->K % kBK == 0) && (a->N % (a->geglu ? 16 : 8) == 0) && ((reinterpret_cast<uintptr_t>(a->A) & 15) == 0) &&
+  bool tc_ok = (a->K % kBK == 0) && (a->N % (geglu ? 16 : 8) == 0) && ((reinterpret_cast<uintptr_t>(a->A) & 15) == 0) &&
                ((reinterpret_cast<uintptr_t>(a->B) & 15) == 0) && (a->ldc % 16 == 0) &&
                ((reinterpret_cast<uintptr_t>(a->C) & 31) == 0);
   if (a->a_mode == A3D_A_PLAIN) tc_ok = tc_ok && (a->lda % 8 == 0) && a->lda >= a->K;
@@ -525,7 +534,7 @@ extern "C" int a3d_gemm(const a3d_gemm_args* a, void* stream) {
                 (long long)a->M, (long long)a->N, (long long)a->K);
 
   if (impl == A3D_GEMM_SIMT) {
-    const int64_t n_out = a->geglu ? a->N / 2 : a->N;
+    const int64_t n_out = geglu ? a->N / 2 : a->N;
     const int64_t total = a->M * n_out;
     const int threads = 128;
     const int64_t blocks = (total + threads - 1) / threads;
@@ -537,7 +546,7 @@ extern "C" int a3d_gemm(const a3d_gemm_args* a, void* stream) {
 
   // ---- tile shape
   int BN;
-  if (a->geglu) BN = (a->N % 256 == 0) ? 256 : 128;
+  if (geglu) BN = (a->N % 256 == 0) ? 256 : 128;
   else if (a->N % 256 == 0) BN = 256;
   else if (a->K <= 640 && a->N > 512 && (256 * ((a->N + 255) / 256) - a->N) * 8 <= a->N) {
     // short-K GEMMs are bound by the epilogue / output stores, where the 256-wide tile amortises the per-tile handshakes
@@ -548,9 +557,9 @@ extern "C" int a3d_gemm(const a3d_gemm_args* a, void* stream) {
   {
     static int force = -1;
     if (force < 0) { const char* e = getenv("A3D_GEMM_BN"); force = e ? atoi(e) : 0; }
-    if (!a->geglu && (force == 128 || force == 160 || force == 256)) BN = force;   // tuning override
+    if (!geglu && (force == 128 || force == 160 || force == 256)) BN = force;   // tuning override
   }
-  if (a->geglu && a->N % BN) return fail(A3D_EINVAL, "a3d_gemm: GEGLU needs N %% 128 == 0");
+  if (geglu && a->N % BN) return fail(A3D_EINVAL, "a3d_gemm: GEGLU needs N %% 128 == 0");
   d.num_k_blocks = (int)(a->K / kBK);
   d.tiles_m = (int)((a->M + kBM - 1) / kBM);
   d.tiles_n = (int)((a->N + BN - 1) / BN);

@@ -30,9 +30,11 @@ def gemm(A: torch.Tensor, B: torch.Tensor, out: torch.Tensor, *, M: int, N: int,
          conv: Optional[Tuple[int, int, int, int, int]] = None, bias=None, rowbias=None, rb_div: int = 1, rb_mod: int = 0,
          rb_ld: int = 0,
          acc_scale: float = 1.0, R1=None, ldr1: int = 0, r1_scale: float = 1.0, R2=None, ldr2: int = 0, geglu: bool = False,
-         out_f32: bool = False, perm: Tuple[int, int] = (0, 0), impl: int = L.IMPL_AUTO, conv_nopad_lo: bool = False) -> torch.Tensor:
+         out_f32: bool = False, perm: Tuple[int, int] = (0, 0), impl: int = L.IMPL_AUTO, conv_nopad_lo: bool = False,
+         gelu: bool = False) -> torch.Tensor:
     """out = epilogue(A @ B^T); see a3d_gemm in include/a3d.h.  `conv` = (n_img, H, W, C, stride) selects the implicit
-    3x3 convolution A operand."""
+    3x3 convolution A operand; `gelu` applies the erf GELU to the biased value (CLIP's MLP)."""
+    assert not (geglu and gelu)
     lib = L.load()
     a = L.GemmArgs()
     a.A, a.B, a.C = A.data_ptr(), B.data_ptr(), out.data_ptr()
@@ -53,7 +55,8 @@ def gemm(A: torch.Tensor, B: torch.Tensor, out: torch.Tensor, *, M: int, N: int,
     a.acc_scale = acc_scale
     a.R1, a.ldr1, a.r1_scale = L.ptr(R1), ldr1 or N, r1_scale
     a.R2, a.ldr2 = L.ptr(R2), ldr2 or N
-    a.geglu, a.out_f32 = int(geglu), int(out_f32)
+    a.geglu = L.EPI_GEGLU if geglu else (L.EPI_GELU if gelu else 0)
+    a.out_f32 = int(out_f32)
     a.perm_a, a.perm_b = perm
     a.impl = impl
     _enqueued(lib.a3d_gemm(C.byref(a), L.stream_ptr()))
@@ -174,3 +177,37 @@ def ddim_cfg_step(latents, noise_pred, first_frame, bn, c, f, hw, guidance, alph
                                   C.c_void_p(L.ptr(first_frame)), bn, c, f, hw, C.c_float(guidance), C.c_float(alpha_t),
                                   C.c_float(alpha_prev), int(uncond_first), L.stream_ptr()))
     return latents
+
+
+def clip_resize_tables(h: int, w: int):
+    """Host-built Pillow bicubic tables of the CLIP resize of an h x w image: (resize_h, resize_w, (bounds_y, coeffs_y,
+    ksize_y), (bounds_x, coeffs_x, ksize_x)) with int32 CPU tensors."""
+    lib = L.load(require_gpu=False)
+    rh, rw, ky, kx = C.c_int(), C.c_int(), C.c_int(), C.c_int()
+    L.check(lib.a3d_clip_resize_plan(h, w, C.byref(rh), C.byref(rw), C.byref(ky), C.byref(kx)))
+    tabs = []
+    for n_in, n_out, k in ((h, rh.value, ky.value), (w, rw.value, kx.value)):
+        b = torch.empty(n_out, 2, dtype=torch.int32)
+        c = torch.empty(n_out, k, dtype=torch.int32)
+        L.check(lib.a3d_clip_resize_coeffs(n_in, n_out, C.c_void_p(b.data_ptr()), C.c_void_p(c.data_ptr())))
+        tabs.append((b, c, k))
+    return rh.value, rw.value, tabs[0], tabs[1]
+
+
+def clip_preprocess(src: torch.Tensor, src_format: int, patches: Optional[torch.Tensor], pixel_values: Optional[torch.Tensor] = None,
+                    tables=None) -> None:
+    """a3d_clip_preprocess.  `tables` = (resize_h, resize_w, (bounds_y, coeffs_y, ksize_y), (bounds_x, coeffs_x, ksize_x)) with
+    the tensors on the device (None for CLIP_SRC_PIXELS)."""
+    lib = L.load()
+    a = L.ClipPrepArgs()
+    a.src, a.src_format = src.data_ptr(), src_format
+    a.n = src.shape[0]
+    if src_format == L.CLIP_SRC_U8_NHWC:
+        a.h, a.w = src.shape[1], src.shape[2]
+    else:
+        a.h, a.w = src.shape[2], src.shape[3]
+    if tables is not None:
+        a.resize_h, a.resize_w, (by, cy, a.ksize_y), (bx, cx, a.ksize_x) = tables
+        a.bounds_y, a.coeffs_y, a.bounds_x, a.coeffs_x = by.data_ptr(), cy.data_ptr(), bx.data_ptr(), cx.data_ptr()
+    a.patches, a.pixel_values = L.ptr(patches), L.ptr(pixel_values)
+    _enqueued(lib.a3d_clip_preprocess(C.byref(a), L.stream_ptr()))

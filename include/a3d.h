@@ -15,6 +15,8 @@
  *   a3d_layer_norm      torch LayerNorm in BasicTransformerBlock
  *   a3d_conv_in/out     unet_motion_mv_model.py:767-768 (permute + conv_in) and 859-862 (conv_out + permute back)
  *   a3d_ddim_cfg_step   animatediff/pipelines/pipeline.py:1023-1031 (CFG combine + DDIMScheduler.step + frame-0 re-injection)
+ *   a3d_clip_preprocess .cpu() -> PIL -> CLIPImageProcessor -> patch embedding of the IP-Adapter image encoder at
+ *                       custom/threestudio-animate3d/guidance/animatemv_guidance.py:546-555
  *   a3d_raster_*        diff_gaussian_rasterization._C.rasterize_gaussians / rasterize_gaussians_backward, called at
  *                       custom/threestudio-animate3d/renderer/diff_gaussian_rasterizer_advanced_4d.py:161-170
  */
@@ -44,7 +46,9 @@ int a3d_init(void);
  *                               k index = (ky*3+kx)*C + c ; M = n_img*OH*OW
  * Epilogue:  v = acc + bias[n] + rowbias[((m / rb_div) % rb_mod) * rb_ld + n]
  *            v = acc_scale * v + r1_scale * R1[m, n] + R2[om, n]          (om = permuted output row, see below)
- *            GEGLU: columns come in interleaved blocks of 32 (u | g); out[.., j] = u_j * gelu_erf(g_j), N_out = N/2
+ *            GEGLU (geglu = 1): columns come in interleaved blocks of 32 (u | g); out[.., j] = u_j * gelu_erf(g_j), N_out = N/2
+ *            GELU (geglu = 2): out[.., n] = gelu_erf(v) (CLIP's hidden_act="gelu" MLP); like GEGLU it takes bias / row-bias
+ *            only and an fp16 output
  *            out[om, n] stored as fp16 (or fp32 when out_f32)
  * Row permutation (perm_a, perm_b > 0): om = (m / (a*b))*(a*b) + (m % b)*a + (m / b) % a   ("(x a b) -> (x b a)").
  */
@@ -70,7 +74,7 @@ typedef struct a3d_gemm_args {
                                                      when perm_a == 0 (with a permutation another row's store can land
                                                      on R1[m, n] before it is read) */
   const void* R2; int64_t ldr2;                   /* fp16 or NULL; read at the output element om, n itself: may be C */
-  int geglu;
+  int geglu;                  /* 0 = none, 1 = GEGLU, 2 = GELU */
   int out_f32;
   int64_t perm_a, perm_b;     /* 0,0 = identity */
   int impl;                   /* A3D_GEMM_* */
@@ -93,6 +97,8 @@ int a3d_gemm(const a3d_gemm_args* args, void* stream);
  * [h*dv, h*dv+dv) with dv = roundup16(d+1) whose column d holds 1.0 (the row sum then falls out of the PV product).
  * Output: fp16 [.., heads*d] written through the same view geometry as Q with row stride ldo:
  *   out = (accumulate ? out : 0) + out_scale * O.
+ * Tensor-core tiles: 128 query rows.  e1 >= 128 that is not a multiple of 128 needs e2 == 1 (CLIP's 257 tokens per image):
+ * the last tile's rows past e1 are zero-filled on load and never stored.  Keys come in tiles of 64 with the same rule.
  */
 typedef struct a3d_view5 {
   const void* base;
@@ -336,6 +342,44 @@ size_t a3d_mesh_vertex_stats_scratch_bytes(int V, int F, int with_rgb);
  * degree: the ragged table a3d_arap reads.  A pure function of (seed, offset, CSR). */
 int a3d_mesh_sample_neighbors(const int32_t* row_ptr, const int32_t* col, int V, int K, uint64_t seed, uint64_t offset,
                               int32_t* nbr, void* stream);
+
+/* ---------------------------------------------------------------- CLIP image preprocessing (IP-Adapter encoder) ---- */
+/* The frame-0 renders (or decoded condition images) -> the A operand of the ViT-H/14 patch-embedding GEMM, in one launch.
+ * Replaces the host round trip at custom/threestudio-animate3d/guidance/animatemv_guidance.py:546-555 -- .cpu(),
+ * (x*255).astype(np.uint8), PIL, CLIPImageProcessor (transformers 4.25-4.28: PIL bicubic resize of the short edge to 224,
+ * centre crop 224, rescale 1/255, OpenAI CLIP mean / std) -- and the Conv2d(3, C, 14, 14) patchify of CLIPVisionEmbeddings
+ * (reached from animatediff/utils/util.py:268-287, IPAdapterImageProcessor.encode_image).
+ * Arithmetic (animate3d_b200/csrc/a3d_resize_math.h): u = trunc(fp32(x) * 255) clamped to [0, 255] for fp32 input; Pillow's
+ * two-pass fixed-point bicubic resize (horizontal first); crop at floor((size - 224) / 2); v = (fp32(u) / 255 - mean) / std.
+ * Sources: A3D_CLIP_SRC_F32_NCHW  fp32 [n, 3, h, w] in [0, 1]
+ *          A3D_CLIP_SRC_U8_NHWC   uint8 [n, h, w, 3]
+ *          A3D_CLIP_SRC_PIXELS    fp32 [n, 3, 224, 224], already normalised: only the patchify (h, w and the tables unused)
+ * patches: fp16 [n * 257, 640]; row 0 of each image is zero (the class token comes from the GEMM's row-bias table), column
+ *          k < 588 of patch row 1 + 16 py + px holds crop pixel (c, 14 py + ky, 14 px + kx) with k = (c * 14 + ky) * 14 + kx,
+ *          columns 588..639 are zero.  May be NULL when pixel_values is given.
+ * pixel_values: fp32 [n, 3, 224, 224] or NULL (resizing sources only).
+ * The tables come from a3d_clip_resize_plan / a3d_clip_resize_coeffs (host functions) for this h, w, copied to the device. */
+enum { A3D_CLIP_SRC_F32_NCHW = 0, A3D_CLIP_SRC_U8_NHWC = 1, A3D_CLIP_SRC_PIXELS = 2 };
+typedef struct a3d_clip_prep_args {
+  const void* src;
+  int src_format;             /* A3D_CLIP_SRC_* */
+  int n, h, w;
+  int resize_h, resize_w;     /* the plan's resized size */
+  const int32_t* bounds_y;    /* [resize_h, 2] (first row, taps) */
+  const int32_t* coeffs_y;    /* [resize_h, ksize_y] 22-bit fixed point */
+  int ksize_y;
+  const int32_t* bounds_x;    /* [resize_w, 2] */
+  const int32_t* coeffs_x;    /* [resize_w, ksize_x] */
+  int ksize_x;
+  void* patches;              /* fp16 [n * 257, 640] or NULL */
+  float* pixel_values;        /* fp32 [n, 3, 224, 224] or NULL */
+} a3d_clip_prep_args;
+int a3d_clip_preprocess(const a3d_clip_prep_args* args, void* stream);
+/* Host only: the resized size of an h x w image (short edge 224, long edge int(224 * long / short)) and the taps per output
+ * sample of each axis. */
+int a3d_clip_resize_plan(int h, int w, int* resize_h, int* resize_w, int* ksize_y, int* ksize_x);
+/* Host only: Pillow's bicubic tables for in_size -> out_size: bounds_host [out_size, 2], coeffs_host [out_size, ksize]. */
+int a3d_clip_resize_coeffs(int in_size, int out_size, int32_t* bounds_host, int32_t* coeffs_host);
 
 /* debug hook: a device uint64 counter the tensor-core attention kernel bumps once per (warp, key step) that takes the
    lazy-rescale branch of the single-pass softmax (NULL = off; tests use it to prove adversarial inputs reach that branch). */
