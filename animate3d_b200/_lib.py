@@ -87,6 +87,8 @@ def load(require_gpu: bool = True) -> C.CDLL:
         lib.a3d_group_norm_ws_bytes.restype = C.c_size_t
         lib.a3d_raster_workspace_bytes.restype = C.c_size_t
         lib.a3d_raster_workspace_bytes.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int64]
+        lib.a3d_raster_counters_offset.restype = C.c_size_t
+        lib.a3d_raster_counters_offset.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int64]
         lib.a3d_raster_backward_scratch_bytes.restype = C.c_size_t
         lib.a3d_raster_backward_scratch_bytes.argtypes = [C.c_void_p, C.c_int64]
         lib.a3d_deform_backward_scratch_bytes.restype = C.c_size_t
@@ -99,6 +101,7 @@ def load(require_gpu: bool = True) -> C.CDLL:
         lib.a3d_mesh_vertex_stats_scratch_bytes.argtypes = [C.c_int, C.c_int, C.c_int]
         lib.a3d_mesh_sample_neighbors.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_uint64, C.c_uint64, C.c_void_p,
                                                   C.c_void_p]
+        lib.a3d_mesh_sample_neighbors_state.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
         lib.a3d_clip_resize_plan.argtypes = [C.c_int, C.c_int] + [C.POINTER(C.c_int)] * 4
         lib.a3d_clip_resize_coeffs.argtypes = [C.c_int, C.c_int, C.c_void_p, C.c_void_p]
         _lib = lib

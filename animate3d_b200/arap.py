@@ -50,8 +50,25 @@ def cal_connectivity_from_points(points: torch.Tensor, radius: float = 0.1, K: i
     ii = torch.arange(nv, device=dev)[:, None].expand(nv, K).reshape(-1)
     jj = nn_idx.reshape(-1)
     nn = torch.arange(K, device=dev)[None].expand(nv, K).reshape(-1)
+    return drop_missing_edges(ii, jj, nn) + (weight,)
+
+
+def drop_missing_edges(ii, jj, nn):
+    """The edges with jj != -1.  The boolean selection reads its count from the device, so inside a CUDA-graph capture the
+    full lists are returned: cal_arap_error writes their -1 entries into the table's -1 fill, which gives the same table."""
+    if torch.cuda.is_current_stream_capturing():
+        return ii, jj, nn
     keep = jj != -1
-    return ii[keep], jj[keep], nn[keep], weight
+    return ii[keep], jj[keep], nn[keep]
+
+
+def sample_nodes(nv: int, sample_num: int, device) -> torch.Tensor:
+    """`sample_num` node indices drawn uniformly with replacement (the distribution of np.random.choice(nv, sample_num)) from
+    torch's CUDA generator, whose draws a CUDA graph replays with a fresh offset each time."""
+    return torch.randint(0, nv, (sample_num,), device=device)
+
+
+last_sample_idx: Optional[torch.Tensor] = None    # the node sample of the most recent cal_arap_error (None: all nodes)
 
 
 class _Arap(torch.autograd.Function):
@@ -82,13 +99,19 @@ def cal_arap_error(nodes_sequence: torch.Tensor, ii, jj, nn, K: int = 10, weight
                    sample_num: int = 512, sample_idx: Optional[torch.Tensor] = None) -> torch.Tensor:
     """util.py:183-215.  nodes_sequence [Nt,Nv,3]; (ii, jj, nn) the edge list of `cal_connectivity_from_points`;
     weight [Nv,K] or None (1 on existing edges).  When Nv > sample_num a random node subset is drawn with
-    np.random.choice(Nv, sample_num) like the reference (pass `sample_idx` to fix it)."""
+    np.random.choice(Nv, sample_num) like the reference (pass `sample_idx` to fix it); inside a CUDA-graph capture it is
+    drawn on the device by `sample_nodes`.  `last_sample_idx` holds the sample used."""
+    global last_sample_idx
     nt, nv, _ = nodes_sequence.shape
     dev = nodes_sequence.device
     nbr = torch.full((nv, K), -1, dtype=torch.int32, device=dev)
     nbr[ii, nn] = jj.to(torch.int32)
     if sample_idx is None and nv > sample_num:
-        sample_idx = torch.from_numpy(np.random.choice(nv, sample_num)).to(dev)
+        if torch.cuda.is_current_stream_capturing():
+            sample_idx = sample_nodes(nv, sample_num, dev)
+        else:
+            sample_idx = torch.from_numpy(np.random.choice(nv, sample_num)).to(dev)
     s = None if sample_idx is None else sample_idx.to(device=dev, dtype=torch.int32).contiguous()
+    last_sample_idx = s
     w = None if weight is None else weight.detach().contiguous().float()
     return _Arap.apply(nodes_sequence, nbr, w, s)

@@ -177,11 +177,14 @@ __device__ __forceinline__ uint32_t philox_word0(uint32_t c0, uint32_t c1, uint3
 }
 
 // Per row: every slot j gets the key philox(i, j); the K smallest (key, j) in ascending order are kept in registers
-// (insertion with a strict compare, so an equal key keeps the smaller j); missing slots stay -1.
+// (insertion with a strict compare, so an equal key keeps the smaller j); missing slots stay -1.  With state non-null,
+// (seed, offset) are read from state[0], state[1] instead of the arguments.
 __global__ void __launch_bounds__(128) mesh_sample_kernel(const int32_t* __restrict__ row_ptr, const int32_t* __restrict__ col, int V,
-                                                          int K, uint64_t seed, uint64_t offset, int32_t* __restrict__ nbr) {
+                                                          int K, uint64_t seed, uint64_t offset, const uint64_t* __restrict__ state,
+                                                          int32_t* __restrict__ nbr) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= V) return;
+  if (state) { seed = state[0]; offset = state[1]; }
   uint32_t bk[kMeshMaxK];
   int bj[kMeshMaxK];
 #pragma unroll
@@ -207,6 +210,9 @@ __global__ void __launch_bounds__(128) mesh_sample_kernel(const int32_t* __restr
   for (int k = 0; k < kMeshMaxK; ++k)
     if (k < K) nbr[(int64_t)i * K + k] = bj[k] < 0 ? -1 : col[b + bj[k]];
 }
+
+// stream-ordered after the draw that read state[1]
+__global__ void mesh_advance_offset_kernel(uint64_t* state) { state[1] += 1; }
 
 }  // namespace a3d
 
@@ -273,7 +279,19 @@ extern "C" int a3d_mesh_sample_neighbors(const int32_t* row_ptr, const int32_t* 
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   if (!row_ptr || !col || !nbr || V < 1 || K < 1 || K > kMeshMaxK)
     return fail(A3D_EINVAL, "a3d_mesh_sample_neighbors: need V >= 1, 1 <= K <= %d (got V=%d, K=%d)", kMeshMaxK, V, K);
-  mesh_sample_kernel<<<(V + 127) / 128, 128, 0, st>>>(row_ptr, col, V, K, seed, offset, nbr);
+  mesh_sample_kernel<<<(V + 127) / 128, 128, 0, st>>>(row_ptr, col, V, K, seed, offset, nullptr, nbr);
+  A3D_LAUNCH_CHECK();
+  return A3D_OK;
+}
+
+extern "C" int a3d_mesh_sample_neighbors_state(const int32_t* row_ptr, const int32_t* col, int V, int K, uint64_t* state, int32_t* nbr,
+                                               void* stream) {
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  if (!row_ptr || !col || !nbr || !state || V < 1 || K < 1 || K > kMeshMaxK)
+    return fail(A3D_EINVAL, "a3d_mesh_sample_neighbors_state: need a state, V >= 1, 1 <= K <= %d (got V=%d, K=%d)", kMeshMaxK, V, K);
+  mesh_sample_kernel<<<(V + 127) / 128, 128, 0, st>>>(row_ptr, col, V, K, 0, 0, state, nbr);
+  A3D_LAUNCH_CHECK();
+  mesh_advance_offset_kernel<<<1, 1, 0, st>>>(state);
   A3D_LAUNCH_CHECK();
   return A3D_OK;
 }

@@ -324,6 +324,13 @@ extern "C" size_t a3d_raster_workspace_bytes(int P, int H, int W, int num_cams, 
   return raster_layout(nullptr, P, H, W, num_cams, max_rendered).bytes;
 }
 
+// The carve only adds aligned offsets to its base, so carving over a 256-aligned stand-in address yields the offsets.
+extern "C" size_t a3d_raster_counters_offset(int P, int H, int W, int num_cams, int64_t max_rendered) {
+  char* const probe = reinterpret_cast<char*>(256);
+  const RasterLayout l = raster_layout(probe, P, H, W, num_cams, max_rendered);
+  return (size_t)(reinterpret_cast<char*>(l.ws.counters) - probe);
+}
+
 extern "C" int a3d_raster_forward(const a3d_raster_args* a, float* color, float* depth, float* alpha, int32_t* radii,
                                   void* workspace, size_t workspace_bytes, int64_t max_rendered, int64_t* num_rendered_host,
                                   void* stream) {
@@ -414,7 +421,7 @@ extern "C" int a3d_raster_backward(const a3d_raster_args* a, const float* dL_dco
   A3D_LAUNCH_CHECK();
   stamp(7, st);
   if (a->deterministic) {
-    launch_gather_records(d, ws, records, op_part, st);
+    launch_gather_records(d, ws, records, op_part, max_rendered, st);
     launch_preprocess_backward_det(d, ws, radii, op_part, dL_dmeans3D, dL_dscales, dL_drotations, dL_dopacity, dL_dcolors, dL_dshs,
                                    dL_dmeans2D, st);
   } else {

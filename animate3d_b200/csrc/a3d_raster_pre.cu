@@ -130,15 +130,17 @@ __global__ void raster_preprocess_backward_kernel(RasterDev a, RasterWs ws, cons
   }
 }
 
-// deterministic backward, stage 1: every (camera, gaussian) sums the records of its pair slots in slot (= tile) order
-__global__ void raster_gather_records_kernel(RasterDev a, RasterWs ws, const float* __restrict__ records, float* __restrict__ op_part) {
+// deterministic backward, stage 1: every (camera, gaussian) sums the records of its pair slots in slot (= tile) order.  The
+// slots are clamped to the capacity: after an overflow the forward dropped the pairs past it and the scratch ends there.
+__global__ void raster_gather_records_kernel(RasterDev a, RasterWs ws, const float* __restrict__ records, float* __restrict__ op_part,
+                                             long long cap) {
   const int idx = blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= a.num_cams * a.P) return;
   float acc[10];
 #pragma unroll
   for (int k = 0; k < 10; ++k) acc[k] = 0.f;
   if (ws.tiles[idx] != 0) {
-    const size_t lo = idx ? ws.offsets[idx - 1] : 0u, hi = ws.offsets[idx];
+    const size_t lo = min((long long)(idx ? ws.offsets[idx - 1] : 0u), cap), hi = min((long long)ws.offsets[idx], cap);
     for (size_t slot = lo; slot < hi; ++slot) {
       const float2* r = reinterpret_cast<const float2*>(records + slot * 10);
 #pragma unroll
@@ -234,9 +236,10 @@ void launch_preprocess_backward(const RasterDev& a, const RasterWs& ws, const in
   raster_preprocess_backward_kernel<<<(n + 255) / 256, 256, 0, st>>>(a, ws, radii, dmeans3D, dscales, drots, dcolors, dshs, dmeans2D);
 }
 
-void launch_gather_records(const RasterDev& a, const RasterWs& ws, const float* records, float* op_part, cudaStream_t st) {
+void launch_gather_records(const RasterDev& a, const RasterWs& ws, const float* records, float* op_part, long long cap,
+                           cudaStream_t st) {
   const int n = a.num_cams * a.P;
-  raster_gather_records_kernel<<<(n + 255) / 256, 256, 0, st>>>(a, ws, records, op_part);
+  raster_gather_records_kernel<<<(n + 255) / 256, 256, 0, st>>>(a, ws, records, op_part, cap);
 }
 void launch_preprocess_backward_det(const RasterDev& a, const RasterWs& ws, const int32_t* radii, const float* op_part, float* dmeans3D,
                                     float* dscales, float* drots, float* dopacity, float* dcolors, float* dshs, float* dmeans2D,

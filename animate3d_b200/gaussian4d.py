@@ -280,7 +280,8 @@ class Gaussian4DModel(torch.nn.Module):
         means, scales, rots = self.deform_all(timestamps, deform_scale=deform_scale)
         if not first_frame_trainable:
             first = timestamps.reshape(-1).float().to(self._xyz.device) == -1
-            if bool(first.any()):
+            # the any() test reads the device; a CUDA-graph capture applies the (then exact no-op) selection unconditionally
+            if torch.cuda.is_current_stream_capturing() or bool(first.any()):
                 keep = first[:, None, None]
                 means = torch.where(keep, self._xyz[None], means)
                 scales = torch.where(keep, torch.exp(self._scaling)[None], scales)

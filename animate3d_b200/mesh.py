@@ -22,6 +22,7 @@ import numpy as np
 import torch
 
 from . import _lib as L
+from .arap import drop_missing_edges
 
 C0 = 0.28209479177387814
 MAX_K = 12
@@ -190,18 +191,43 @@ class MeshGraph:
         np.cumsum(np.bincount(key // num_points, minlength=num_points), out=row_ptr[1:])
         return cls(torch.from_numpy(row_ptr.astype(np.int32)).to(device), torch.from_numpy((key % num_points).astype(np.int32)).to(device))
 
+    sample_state: Optional[torch.Tensor] = None     # device int64 [2] (seed, next offset) of captured draws
+
+    def set_sample_state(self, seed: int, offset: int = 0) -> None:
+        """Seed the draws of `sample` inside CUDA-graph captures: replay k of a graph that captured one `sample(K)` writes
+        the table of the eager `sample(K, seed, offset + k)`.  Call it outside the capture; `sample_offset()` reads where
+        the state has got to."""
+        if not (0 <= seed < 2 ** 63 and 0 <= offset < 2 ** 63):
+            raise ValueError("seed and offset must lie in [0, 2^63)")
+        self.sample_state = torch.tensor([seed, offset], dtype=torch.int64, device=self.row_ptr.device)
+
+    def sample_offset(self) -> int:
+        """The offset the next captured draw will use (one host read)."""
+        return int(self.sample_state[1])
+
     def sample(self, K: int, seed: Optional[int] = None, offset: int = 0) -> torch.Tensor:
         """K <= 12 distinct random neighbours per vertex -> nbr [V, K] int32, -1 past the degree (a3d_mesh_sample_neighbors).
-        `seed` defaults to a draw from torch's default CPU generator (no device sync), so torch.manual_seed fixes a run."""
+        `seed` defaults to a draw from torch's default CPU generator (no device sync), so torch.manual_seed fixes a run.
+        Inside a CUDA-graph capture the (seed, offset) come from the device state of `set_sample_state`, and every
+        replay advances its offset (a3d_mesh_sample_neighbors_state)."""
         if not 1 <= K <= MAX_K:
             raise ValueError(f"K must be in [1, {MAX_K}], got {K}")
-        if seed is None:
+        capturing = torch.cuda.is_current_stream_capturing()
+        if capturing and (seed is not None or offset or self.sample_state is None):
+            raise ValueError("a captured MeshGraph.sample draws from the device state: call set_sample_state(seed, offset) "
+                             "before the capture and pass neither seed nor offset")
+        if seed is None and not capturing:
             seed = int(torch.randint(0, 2 ** 62, (1,)))
         lib = L.load()
         nbr = torch.empty(self.num_points, K, dtype=torch.int32, device=self.row_ptr.device)
         col = self.col if self.col.numel() else self.row_ptr       # any valid pointer: an edgeless graph reads no col entry
-        L.check(lib.a3d_mesh_sample_neighbors(C.c_void_p(self.row_ptr.data_ptr()), C.c_void_p(col.data_ptr()), self.num_points, K,
-                                              seed, offset, C.c_void_p(nbr.data_ptr()), L.stream_ptr()))
+        if capturing:
+            L.check(lib.a3d_mesh_sample_neighbors_state(C.c_void_p(self.row_ptr.data_ptr()), C.c_void_p(col.data_ptr()),
+                                                        self.num_points, K, C.c_void_p(self.sample_state.data_ptr()),
+                                                        C.c_void_p(nbr.data_ptr()), L.stream_ptr()))
+        else:
+            L.check(lib.a3d_mesh_sample_neighbors(C.c_void_p(self.row_ptr.data_ptr()), C.c_void_p(col.data_ptr()), self.num_points,
+                                                  K, seed, offset, C.c_void_p(nbr.data_ptr()), L.stream_ptr()))
         return nbr
 
 
@@ -211,8 +237,7 @@ def edge_list(nbr: torch.Tensor):
     ii = torch.arange(nv, device=nbr.device)[:, None].expand(nv, K).reshape(-1)
     jj = nbr.long().reshape(-1)
     nn = torch.arange(K, device=nbr.device)[None].expand(nv, K).reshape(-1)
-    keep = jj != -1
-    return ii[keep], jj[keep], nn[keep]
+    return drop_missing_edges(ii, jj, nn)
 
 
 def vertex_stats(verts: torch.Tensor, graph: MeshGraph, faces: Optional[torch.Tensor] = None,

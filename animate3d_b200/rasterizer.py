@@ -12,6 +12,7 @@ memory, the stream and the autograd tape.  Under torch.use_deterministic_algorit
 in a fixed order (bit-reproducible), at the cost of 40 B of scratch per (tile, gaussian) pair."""
 from __future__ import annotations
 
+import contextlib
 import ctypes as C
 from typing import List, NamedTuple, Optional, Sequence
 
@@ -38,6 +39,54 @@ class GaussianRasterizationSettings(NamedTuple):
 _cap_hint = {}
 last_num_rendered = 0      # (tile, gaussian) pairs of the most recent forward (diagnostics / bench roofline)
 last_backward_scratch_bytes = 0   # deterministic-backward scratch of the most recent backward (0 with the flag off)
+
+# ---- CUDA-graph capture.  An eager forward reads the pair count back and retries with a larger capacity on overflow; a
+# captured one cannot.  It runs at a fixed capacity (the eager hint of its (P, H, W, cams) key times CAPTURE_SLACK) and
+# leaves its counters on the device, where the caller checks the overflow flag after each replay.
+CAPTURE_SLACK = 1.2
+_pair_log: Optional[list] = None
+
+
+def capture_capacity(hint: int) -> int:
+    """Pair capacity of a captured forward whose eager hint is `hint`."""
+    return int(hint * CAPTURE_SLACK)
+
+
+def grow_hint(key, needed: int) -> int:
+    """After a replay whose forward of `key` needed `needed` pairs and overflowed: the hint the eager path would have set."""
+    _cap_hint[key] = max(_cap_hint.get(key, 0), int(needed * 1.08) + 1024, 1 << 16)
+    return _cap_hint[key]
+
+
+@contextlib.contextmanager
+def collect_pair_counts():
+    """Forwards captured inside this context append (key, counts) to the yielded list: counts is a device int64
+    [total pairs, overflow flag] that every replay rewrites.  A captured forward outside it raises, since nobody would check
+    whether its render was complete."""
+    global _pair_log
+    prev, _pair_log = _pair_log, []
+    try:
+        yield _pair_log
+    finally:
+        _pair_log = prev
+
+
+def _captured_forward(lib, key, args, outs, dev):
+    if _pair_log is None:
+        raise L.A3DError("a rasterizer forward captured into a CUDA graph must run inside rasterizer.collect_pair_counts(), "
+                         "whose owner checks the overflow flag after every replay")
+    if key not in _cap_hint:
+        raise L.A3DError(f"no eager forward of (P, H, W, cams) = {key} yet: the captured capacity is sized from one")
+    P, H, W, ncam = key
+    cap = capture_capacity(_cap_hint[key])
+    nbytes = lib.a3d_raster_workspace_bytes(P, H, W, ncam, C.c_int64(cap))
+    ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+    L.check(lib.a3d_raster_forward(C.byref(args), *[C.c_void_p(t.data_ptr()) for t in outs], C.c_void_p(ws.data_ptr()),
+                                   C.c_size_t(nbytes), C.c_int64(cap), None, L.stream_ptr()))
+    off = lib.a3d_raster_counters_offset(P, H, W, ncam, C.c_int64(cap))
+    counters = ws[off:off + 8 * (ncam + 2)].view(torch.int64)
+    _pair_log.append((key, counters[ncam:].clone()))     # a copy: the workspace is reused once the backward has run
+    return cap, nbytes, ws, counters[:ncam]
 
 
 def _pack_cams(settings: Sequence[GaussianRasterizationSettings], device) -> torch.Tensor:
@@ -81,6 +130,15 @@ class _RasterizeBatch(torch.autograd.Function):
         alpha = torch.empty(ncam, 1, H, W, device=dev)
         radii = torch.empty(ncam, P, dtype=torch.int32, device=dev)
         key = (P, H, W, ncam)
+        if torch.cuda.is_current_stream_capturing():
+            args = _make_args(P, H, W, cams_t, means3D, scales, rotations, opacities, shs, colors_precomp, sh_degree, per_cam,
+                              scale_modifier, bg)
+            cap, nbytes, ws, ctx.num_rendered = _captured_forward(lib, key, args, (color, depth, alpha, radii), dev)
+            ctx.save_for_backward(means3D, scales, rotations, opacities, shs, colors_precomp, cams_t, radii, ws)
+            ctx.meta = (meta, cap, nbytes, P, ncam)
+            ctx.m2_shape = None if means2D is None else tuple(means2D.shape)
+            ctx.mark_non_differentiable(radii)
+            return color, radii, depth, alpha
         cap = _cap_hint.get(key, max(1 << 16, 4 * P * ncam))
         counts = torch.empty(ncam + 2, dtype=torch.int64).pin_memory()
         while True:

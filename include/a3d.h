@@ -218,6 +218,12 @@ size_t a3d_raster_workspace_bytes(int P, int H, int W, int num_cams, int64_t max
 int a3d_raster_forward(const a3d_raster_args* args, float* color, float* depth, float* alpha, int32_t* radii,
                        void* workspace, size_t workspace_bytes, int64_t max_rendered, int64_t* num_rendered_host,
                        void* stream);
+/* Byte offset (a multiple of 256) of the forward's pair counters inside its workspace: int64 [num_cams] per-camera pair
+ * counts, then the total, then the overflow flag (1 when the total exceeded max_rendered).  a3d_raster_forward writes them on
+ * the stream whether or not num_rendered_host is given, so a caller that cannot read the host copy (a CUDA-graph capture)
+ * reads them here.  After an overflow the pairs past max_rendered are dropped (the render is incomplete but every access
+ * stays inside the workspace, and a3d_raster_backward stays inside its scratch). */
+size_t a3d_raster_counters_offset(int P, int H, int W, int num_cams, int64_t max_rendered);
 /* Scratch bytes a3d_raster_backward needs: 0 when args->deterministic is 0, else 40 B per (tile, gaussian) pair slot of
  * max_rendered plus 4 B per (camera, gaussian). */
 size_t a3d_raster_backward_scratch_bytes(const a3d_raster_args* args, int64_t max_rendered);
@@ -342,6 +348,11 @@ size_t a3d_mesh_vertex_stats_scratch_bytes(int V, int F, int with_rgb);
  * degree: the ragged table a3d_arap reads.  A pure function of (seed, offset, CSR). */
 int a3d_mesh_sample_neighbors(const int32_t* row_ptr, const int32_t* col, int V, int K, uint64_t seed, uint64_t offset,
                               int32_t* nbr, void* stream);
+/* a3d_mesh_sample_neighbors with (seed, offset) read from device memory, state = uint64 [2] (seed, offset); once the draw
+ * has read them, state[1] is advanced by one on the stream.  A CUDA graph that captured this call therefore draws new
+ * neighbours on every replay: replay k writes the table of a3d_mesh_sample_neighbors(seed, offset0 + k). */
+int a3d_mesh_sample_neighbors_state(const int32_t* row_ptr, const int32_t* col, int V, int K, uint64_t* state, int32_t* nbr,
+                                    void* stream);
 
 /* ---------------------------------------------------------------- CLIP image preprocessing (IP-Adapter encoder) ---- */
 /* The frame-0 renders (or decoded condition images) -> the A operand of the ViT-H/14 patch-embedding GEMM, in one launch.
