@@ -14,16 +14,49 @@ kernel reads as `found_inf`, so the parameters and the optimizer state stay exac
 once per step, grows the capacity, captures again and re-runs the step.
 
 Tensors a graph leaves alive (the outputs `step_fn` keeps, `arap.last_sample_idx`) hold the values of that graph's last
-replay until another graph of the same pool replays."""
+replay until another graph of the same pool replays.
+
+The engine networks a refine step calls (the UNet, the CLIP tower, the VAE) keep persistent buffers and packed weights that
+a graph records by address.  Each keeps a counter, `capture_version`, that it bumps whenever one of those tensors may have
+moved (buffer growth, `load_state_dict`, `.to()`, repacking).  Recorded under a capture, such a module registers itself and
+its counter (`note_module`); before each replay `step` compares the counters and captures again on any change, so a replay
+never runs on freed or stale memory.  These recaptures are counted in `pointer_recaptures`, overflow ones in `recaptures`."""
 from __future__ import annotations
 
-from typing import Callable, Dict, Hashable
+import contextlib
+from typing import Callable, Dict, Hashable, List, Optional, Tuple
 
 import torch
 
 from . import rasterizer
 
 MAX_RETRIES = 3
+_module_log: Optional[list] = None
+
+
+@contextlib.contextmanager
+def collect_modules():
+    """Modules recorded inside this context (through `note_module`) append (module, its capture_version) to the yielded
+    list, once each."""
+    global _module_log
+    prev, _module_log = _module_log, []
+    try:
+        yield _module_log
+    finally:
+        _module_log = prev
+
+
+def capturing(device) -> bool:
+    """Whether the current stream of `device` is being captured into a CUDA graph (False for a CPU device, where the query
+    itself would need a driver)."""
+    return torch.device(device).type == "cuda" and torch.cuda.is_current_stream_capturing()
+
+
+def note_module(module) -> None:
+    """Called by a module whose kernels are being recorded into a graph: the graph depends on its buffers and weights staying
+    where they are, which `module.capture_version` tracks."""
+    if _module_log is not None and all(m is not module for m, _ in _module_log):
+        _module_log.append((module, module.capture_version))
 
 
 class StepGraphs:
@@ -40,7 +73,9 @@ class StepGraphs:
         self.graphs: Dict[Hashable, tuple] = {}        # key -> (CUDAGraph, [(raster key, device [pairs, overflow])])
         self.static: Dict[Hashable, Dict[str, torch.Tensor]] = {}
         self.warm = set()
-        self.recaptures = 0
+        self.modules: Dict[Hashable, List[Tuple[object, int]]] = {}     # key -> the modules its graph recorded, and their versions
+        self.recaptures = 0             # after an overflowed replay
+        self.pointer_recaptures = 0     # after a recorded module's buffers or weights moved
         self.pool = None
         self.found_inf = None
 
@@ -53,12 +88,26 @@ class StepGraphs:
             return False
         if key not in self.graphs:
             self.capture(key, inputs)
+        elif self.stale(key):
+            self.capture(key, inputs)
+            self.pointer_recaptures += 1
         for _ in range(MAX_RETRIES):
             if not self.replay(key, inputs):
                 return True
             self.capture(key, inputs)
             self.recaptures += 1
         raise RuntimeError(f"layout {key!r}: the render still overflowed after {MAX_RETRIES} larger captures")
+
+    def release(self) -> None:
+        """Drop every graph and the memory pool they share; the next step of each layout captures again (no eager first
+        step).  A process that alternates with large eager work can hand the pool's memory back this way."""
+        self.graphs.clear()
+        self.modules.clear()
+        self.pool = None
+
+    def stale(self, key: Hashable) -> bool:
+        """Whether a module the graph of `key` recorded has bumped its capture_version since."""
+        return any(m.capture_version != v for m, v in self.modules.get(key, ()))
 
     def eager(self, inputs: Dict[str, torch.Tensor]) -> None:
         """The step without a graph."""
@@ -87,7 +136,7 @@ class StepGraphs:
         g = torch.cuda.CUDAGraph()
         self.optimizer.found_inf = self.found_inf
         try:
-            with rasterizer.collect_pair_counts() as log, torch.cuda.graph(g, pool=self.pool):
+            with rasterizer.collect_pair_counts() as log, collect_modules() as mods, torch.cuda.graph(g, pool=self.pool):
                 self.step_fn(st)
                 if log:
                     self.found_inf.copy_(torch.stack([c[1] for _, c in log]).amax())
@@ -97,6 +146,7 @@ class StepGraphs:
         finally:
             del self.optimizer.found_inf
         self.graphs[key] = (g, list(log))
+        self.modules[key] = list(mods)
 
     def replay(self, key: Hashable, inputs: Dict[str, torch.Tensor]) -> bool:
         """Copy `inputs` into the static buffers of `key` and replay its graph.  Returns True when a render overflowed: the

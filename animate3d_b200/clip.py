@@ -6,6 +6,7 @@ processor in front of it, as drop-ins for the objects the reference's `load_ip_a
   patch GEMM (+ position / class row-bias table) -> pre_layrnorm -> layers of
   [LN1 -> fused QKV GEMM -> attention (257 queries and keys per image) -> out-proj GEMM + residual -> LN2 -> fc1 GEMM + GELU
   -> fc2 GEMM + residual] -> post_layernorm -> visual_projection (fp32 out), captured in one CUDA graph per batch size.
+  Inside a caller's capture (a captured refine step) it records into that graph instead, on the buffers of an eager call.
 * `CLIPImageProcessor`: `__call__(images, return_tensors="pt").pixel_values` through `a3d_clip_preprocess`.
 * `IPAdapterImageProcessor`: `encode_image(images)`; images go from their raw form (float renders in [0, 1] on the device,
   uint8 [n, H, W, 3], PIL) straight into the patch GEMM's operand in one launch.  A float device tensor never leaves the
@@ -25,6 +26,7 @@ import torch
 
 from . import _lib as L
 from . import ops
+from .capture import capturing, note_module
 
 HALF = torch.float16
 TOKENS, PATCH_K, PATCH_K_PAD, CROP, PATCH = 257, 588, 640, 224, 14
@@ -69,6 +71,8 @@ class CLIPVisionModelWithProjection:
         self._graphs: Dict[int, torch.cuda.CUDAGraph] = {}
         self.launches_per_forward = 0
         self.use_cuda_graph = True          # off for per-launch checks that synchronise between launches
+        # bumped whenever the packed weights or the static buffers a recorded graph uses may have moved
+        self.capture_version = 0
 
     # -------------------------------------------------------------------------------------------- loading
     @classmethod
@@ -149,12 +153,16 @@ class CLIPVisionModelWithProjection:
                 raise KeyError(f"unexpected keys for the vision tower: {extra[:8]}")
         self.w, self.layers = w, layers
         self._static.clear(); self._graphs.clear()
+        self.capture_version += 1
         return self
 
     # -------------------------------------------------------------------------------------------- forward
     def _buffers(self, n: int) -> dict:
         st = self._static.get(n)
         if st is None:
+            if capturing(self.device):
+                raise ValueError(f"CLIP tower: no buffers for batch size {n} inside a CUDA-graph capture; one eager call of "
+                                 "this batch size must come first")
             c, T = self.cfg, n * TOKENS
             H, nh = c.hidden_size, c.num_attention_heads
             d = H // nh
@@ -200,7 +208,15 @@ class CLIPVisionModelWithProjection:
 
     def run_patches(self, n: int) -> torch.Tensor:
         """The tower on the operand already in patch_buffer(n): image_embeds fp32 [n, projection_dim].  The first call per
-        batch size runs eagerly, the second is captured, later ones replay the graph."""
+        batch size runs eagerly, the second is captured, later ones replay the graph.  Inside a caller's capture the kernels
+        are recorded into the caller's graph."""
+        if capturing(self.device):
+            if not self.layers:
+                raise ValueError("CLIP tower: no weights loaded")
+            st = self._buffers(n)
+            note_module(self)
+            self._run(n, st)
+            return st["out"].clone()
         st = self._buffers(n)
         graph = self._graphs.get(n)
         if graph is not None:
@@ -248,6 +264,9 @@ class _Tables:
         key = (h, w, str(device))
         t = self._cache.get(key)
         if t is None:
+            if capturing(device):
+                raise ValueError(f"CLIP processor: no resize tables for {h}x{w} images inside a CUDA-graph capture (they are "
+                                 "uploaded from the host); one eager call of this image size must come first")
             rh, rw, (by, cy, ky), (bx, cx, kx) = ops.clip_resize_tables(h, w)
             t = (rh, rw, (by.to(device), cy.to(device), ky), (bx.to(device), cx.to(device), kx))
             self._cache[key] = t
@@ -331,6 +350,14 @@ class IPAdapterImageProcessor:
         self.feature_extractor, self.image_encoder = feature_extractor, image_encoder
 
     def encode_image(self, images) -> torch.Tensor:
+        """Inside a caller's CUDA-graph capture, images must be a device tensor whose batch size and image size had an eager
+        call before (the buffers and resize tables are not allocated under capture: ValueError)."""
+        if capturing(self.image_encoder.device):
+            if not (isinstance(images, torch.Tensor) and images.device.type == "cuda"):
+                raise ValueError("CLIP processor: a captured encode_image needs the images as a CUDA tensor")
+            src = images if images.dim() == 4 else images[None]
+            h, w = src.shape[1:3] if images.dtype == torch.uint8 else src.shape[2:4]
+            self.feature_extractor.tables.get(int(h), int(w), self.feature_extractor.device)   # raises when missing
         n = _count(images)
         patches = self.image_encoder.patch_buffer(n)
         got = self.feature_extractor.write(images, patches)

@@ -26,6 +26,7 @@ from typing import Any, Optional
 import torch
 import torch.nn.functional as F
 
+from .capture import capturing
 from .registry import BaseObject, C, register
 from .scheduler import DDIMScheduler
 
@@ -140,8 +141,23 @@ class AnimateMVDiffusionGuidance(BaseObject):
 
     # ---------------------------------------------------------------------------------------------- small helpers
     def set_min_max_steps(self, min_step_percent: float = 0.02, max_step_percent: float = 0.98):
+        """Also writes [min_step, max_step] into the device tensor `step_bounds` in place, where a captured step's
+        `draw_timestep` reads them at every replay."""
         self.min_step = int(self.num_train_timesteps * min_step_percent)
         self.max_step = int(self.num_train_timesteps * max_step_percent)
+        if getattr(self, "step_bounds", None) is None:
+            self.step_bounds = torch.tensor([self.min_step, self.max_step], dtype=torch.long, device=self.device)
+        else:
+            self.step_bounds[0].fill_(self.min_step)
+            self.step_bounds[1].fill_(self.max_step)
+
+    def draw_timestep(self, batch_size: int) -> torch.Tensor:
+        """[batch_size] int64 timesteps drawn uniformly from min_step .. max_step inclusive, on the device and from torch's
+        generator of that device, with the bounds read from `step_bounds`: no host read, so a CUDA graph that records the
+        draw follows `set_min_max_steps` / `update_step` at every replay."""
+        lo, hi = self.step_bounds[0], self.step_bounds[1]
+        u = torch.rand(batch_size, dtype=torch.float64, device=self.step_bounds.device)
+        return torch.minimum(lo + (u * (hi - lo + 1)).long(), hi)
 
     def forward_unet(self, latents, t, encoder_hidden_states, camera, i2v_cond_time_zero: bool, added_cond_kwargs=None):
         """animatemv_guidance.py:328-346 (the dtype casts there are the engine's own fp16 entry)."""
@@ -233,7 +249,14 @@ class AnimateMVDiffusionGuidance(BaseObject):
                  guidance_eval: bool = False, **kwargs):
         """animatemv_guidance.py:515-600.  rgb [B,H,W,3] in [0,1] with grad, B = b * n_view * n_frame.
         Extra keyword hooks (not in the reference): `image_embeds` [b*n_view, 1024] bypasses the CLIP image encoder,
-        `timestep` [b] fixes the draw of line 556."""
+        `timestep` [b] fixes the draw of line 556.
+
+        Inside a CUDA-graph capture the timestep is drawn by `draw_timestep` (eagerly by torch.randint, as the reference
+        does); either way `last_timestep` holds the draw.  guidance_eval reads the device from the host and raises there."""
+        in_capture = capturing(self.device)
+        if guidance_eval and in_capture:
+            raise ValueError("guidance_eval reads the device from the host and runs 25 more UNet evaluations: it cannot be "
+                             "part of a captured step; call it eagerly")
         cfg = self.cfg
         batch_size = rgb.shape[0] // (cfg.n_view * cfg.n_frame)
         rgb_bchw = rgb.permute(0, 3, 1, 2)
@@ -250,7 +273,11 @@ class AnimateMVDiffusionGuidance(BaseObject):
                 image_embeds = self.ip_image_processor.encode_image(cond)
         t = kwargs.get("timestep")
         if t is None:
-            t = torch.randint(self.min_step, self.max_step + 1, [batch_size], dtype=torch.long, device=latents.device)
+            if in_capture:
+                t = self.draw_timestep(batch_size)
+            else:
+                t = torch.randint(self.min_step, self.max_step + 1, [batch_size], dtype=torch.long, device=latents.device)
+        self.last_timestep = t
         loss, aux = self.compute_mvdream_recon_loss(latents, t, prompt_utils, elevation, azimuth, camera_distances, c2w, image_embeds)
         out = {"loss_sds": loss, "min_step": self.min_step, "max_step": self.max_step}
         if guidance_eval:

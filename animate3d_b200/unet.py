@@ -15,7 +15,8 @@ signature and `UNet3DConditionOutput(sample=...)` result.  What differs is every
     row-bias table computed once at load
   * text / IP-adapter K,V are computed once per (view) instead of once per frame (unet_motion_mv_model.py:754, 763 repeat
     them F times)
-  * the whole forward is captured in one CUDA graph after the first call
+  * the whole forward is captured in one CUDA graph after the first call; inside a caller's capture (a captured refine step,
+    capture.StepGraphs) it records its kernels into that graph instead, on the buffers of an earlier eager call
 Torch is used for device memory and the stream only; there is no fallback path.
 """
 from __future__ import annotations
@@ -28,6 +29,7 @@ import torch
 from . import _lib as L
 from . import ops
 from . import processor_exec as P
+from .capture import capturing, note_module
 from .modules import attn_processors_of, build_tree
 from .processor_exec import HALF, _Lin, linear
 from .unet_config import UNetConfig, key_plan, up_plan
@@ -74,6 +76,8 @@ class MVUNetMotionModel(torch.nn.Module):
         self._bufs: Dict[str, torch.Tensor] = {}
         self._graphs: Dict[tuple, torch.cuda.CUDAGraph] = {}
         self._static: Dict[tuple, dict] = {}
+        # bumped whenever a tensor the recorded kernels read or write may have moved (capture.StepGraphs recaptures then)
+        self.capture_version = 0
         # View-sharded forwards run eagerly: capturing the asynchronous NCCL all-gathers of torch 2.11 / NCCL 2.28 in a CUDA graph
         # deadlocks on this stack; the kernels between two gathers are long enough for the launch stream to stay ahead.
         self.use_cuda_graph = view_group is None
@@ -109,6 +113,7 @@ class MVUNetMotionModel(torch.nn.Module):
             self._device = torch.device(device)
             self._prepared = False
             self._bufs.clear(); self._graphs.clear(); self._static.clear()
+            self.capture_version += 1
         return self
 
     def half(self):
@@ -143,6 +148,7 @@ class MVUNetMotionModel(torch.nn.Module):
                     module.set_processor(new)
                     self._loaded.update(f"{key}.{k}" for k in cur[key].state_dict())
         self._prepared = False
+        self.capture_version += 1
 
     @classmethod
     def from_unet2d(cls, unet, motion_adapter=None, load_weights: bool = True, device: str = "cuda", **kwargs):
@@ -212,6 +218,7 @@ class MVUNetMotionModel(torch.nn.Module):
         plan = key_plan(self.cfg)
         self._loaded.update(k for k in sd if k in plan)
         self._prepared = False
+        self.capture_version += 1
         return res
 
     def share_packed_weights(self, other: "MVUNetMotionModel"):
@@ -227,6 +234,7 @@ class MVUNetMotionModel(torch.nn.Module):
         for p_ in list(self.parameters()) + list(self.buffers()):
             p_.data = torch.empty(0, device=p_.device, dtype=p_.dtype)
         self._graphs.clear(); self._static.clear()
+        self.capture_version += 1
 
     def drop_reference_weights(self):
         """Free the fp32 master copies (6 GB for the released geometry) once the packed operands exist; `state_dict()` is then
@@ -244,6 +252,9 @@ class MVUNetMotionModel(torch.nn.Module):
 
     def _prepare(self):
         """Repack the reference-layout fp32 weights into the fused fp16 operands the kernels consume."""
+        if capturing(self.device):
+            raise ValueError("MVUNetMotionModel: the packed weights cannot be (re)built inside a CUDA-graph capture; one eager "
+                             "call of this shape must come first")
         L.load()
         if self._masters_dropped:
             raise RuntimeError("the fp32 masters were released; the packed operands cannot be rebuilt")
@@ -370,6 +381,7 @@ class MVUNetMotionModel(torch.nn.Module):
         self._prepared = True
         self._graphs.clear()
         self._static.clear()
+        self.capture_version += 1
 
     # ------------------------------------------------------------------------------------------------ buffers
     def _buf(self, name: str, shape, dtype=HALF) -> torch.Tensor:
@@ -379,6 +391,9 @@ class MVUNetMotionModel(torch.nn.Module):
         for s in shape:
             numel *= s
         if t is None or t.numel() < numel or t.dtype != dtype:
+            if capturing(self.device):
+                raise ValueError(f"MVUNetMotionModel: buffer {name!r} would have to grow inside a CUDA-graph capture; one eager "
+                                 "call of this shape must come first")
             if t is not None and self._graphs:
                 # graphs captured for other shape keys hold the old pointer: drop them, every key recaptures lazily
                 self._graphs.clear()
@@ -386,6 +401,7 @@ class MVUNetMotionModel(torch.nn.Module):
                     st["calls"] = 0
             t = torch.empty(numel, dtype=dtype, device=self.device)
             self._bufs[key] = t
+            self.capture_version += 1
         return t[:numel].view(*shape)
 
     # ------------------------------------------------------------------------------------------------ building blocks
@@ -648,7 +664,18 @@ class MVUNetMotionModel(torch.nn.Module):
                 cross_attention_kwargs=None, added_cond_kwargs=None, down_block_additional_residuals=None,
                 mid_block_additional_residual=None, return_dict: bool = True, camera=None, num_views: int = 4,
                 i2v_cond_time_zero: bool = False):
-        """Signature of unet_motion_mv_model.py:633-649.  sample [B*Nv, 4, F, h, w]; returns `.sample` of the same shape."""
+        """Signature of unet_motion_mv_model.py:633-649.  sample [B*Nv, 4, F, h, w]; returns `.sample` of the same shape.
+
+        Inside a caller's CUDA-graph capture the kernels are recorded into the caller's graph (no inner capture, replay or
+        synchronise).  That allocates nothing, so an eager call of the same shape must have come first; otherwise, and for a
+        view-sharded model (its NCCL gathers cannot be captured), it raises ValueError before recording anything."""
+        in_capture = capturing(self.device)
+        if in_capture and self.view_group is not None:
+            raise ValueError("a view-sharded MVUNetMotionModel cannot be recorded into a CUDA graph: its K|V all-gathers run "
+                             "eagerly")
+        if in_capture and not self._prepared:
+            raise ValueError("MVUNetMotionModel: no packed weights inside a CUDA-graph capture; one eager call of this shape "
+                             "must come first")
         if not self._prepared:
             self._prepare()
         if attention_mask is not None or timestep_cond is not None or down_block_additional_residuals is not None \
@@ -670,6 +697,9 @@ class MVUNetMotionModel(torch.nn.Module):
         n_text = encoder_hidden_states.shape[1]
         key = sig + (n_text,)
         st = self._static.get(key)
+        if in_capture and st is None:
+            raise ValueError(f"MVUNetMotionModel: no buffers for shape {key} inside a CUDA-graph capture; one eager call of "
+                             "this shape must come first")
         if st is None:
             st = {"sample": torch.empty(BN, cin, F, h0, w0, device=dev, dtype=torch.float32),
                   "t": torch.empty(BN, device=dev, dtype=torch.float32),
@@ -679,13 +709,19 @@ class MVUNetMotionModel(torch.nn.Module):
                   "out": torch.empty(BN, self.cfg.out_channels, F, h0, w0, device=dev, dtype=torch.float32), "calls": 0}
             self._static[key] = st
         st["sample"].copy_(sample)
-        t = torch.as_tensor(timestep, dtype=torch.float32, device=dev)
-        st["t"].copy_(t.reshape(-1).expand(BN) if t.numel() in (1, BN) else t)
+        if in_capture and not isinstance(timestep, torch.Tensor):
+            st["t"].fill_(float(timestep))                  # an upload of a host scalar cannot be captured
+        else:
+            t = torch.as_tensor(timestep, dtype=torch.float32, device=dev)
+            st["t"].copy_(t.reshape(-1).expand(BN) if t.numel() in (1, BN) else t)
         st["text"].copy_(encoder_hidden_states)
         st["camera"].copy_(camera.reshape(BN, -1))
         st["image_embeds"].copy_(added_cond_kwargs["image_embeds"])
         graph = self._graphs.get(key)
-        if graph is not None:
+        if in_capture:
+            note_module(self)
+            self._run(sig, st)
+        elif graph is not None:
             graph.replay()
         else:
             self.collectives = self.collective_bytes = 0

@@ -23,6 +23,7 @@ import torch.nn.functional as F
 
 from . import _lib as L
 from . import ops
+from .capture import capturing, note_module
 
 HALF = torch.float16
 GROUPS = 32
@@ -245,6 +246,8 @@ class AutoencoderKL(torch.nn.Module):
         self._device = torch.device(device)
         self.eps = 1e-6
         self.W: Optional[Dict[str, dict]] = None
+        # bumped when the packed weights are replaced: a CUDA graph that recorded the VAE reads them by address
+        self.capture_version = 0
 
     @property
     def device(self):
@@ -335,6 +338,7 @@ class AutoencoderKL(torch.nn.Module):
         W["dec_norm"] = gn("decoder.conv_norm_out")
         W["dec_out"] = edge("decoder.conv_out")
         self.W = W
+        self.capture_version += 1
         return missing, unexpected
 
     # ------------------------------------------------------------------------------------------------ blocks
@@ -361,6 +365,8 @@ class AutoencoderKL(torch.nn.Module):
         """x [N, 3, H, W] in [-1, 1] (fp32, may require grad) -> moments [N, 8, H/8, W/8] fp32."""
         if self.W is None:
             raise RuntimeError("AutoencoderKL: load_state_dict first")
+        if capturing(self._device):
+            note_module(self)
         W = self.W
         n, _, h, w = x.shape
         if h % 8 or w % 8 or (w > 128 and w % 128) or (w <= 128 and 128 % w):
@@ -386,6 +392,8 @@ class AutoencoderKL(torch.nn.Module):
         """z [N, 4, h, w] (latents / scaling_factor) -> `.sample` [N, 3, 8h, 8w] fp32.  Forward only."""
         if self.W is None:
             raise RuntimeError("AutoencoderKL: load_state_dict first")
+        if capturing(self._device):
+            note_module(self)
         W = self.W
         n, _, h, w = z.shape
         t = F.conv2d(z.to(self._device, torch.float32), W["post_quant"][0], W["post_quant"][1])
