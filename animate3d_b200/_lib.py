@@ -87,6 +87,8 @@ def load(require_gpu: bool = True) -> C.CDLL:
         lib.a3d_group_norm_ws_bytes.restype = C.c_size_t
         lib.a3d_raster_workspace_bytes.restype = C.c_size_t
         lib.a3d_raster_workspace_bytes.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int64]
+        lib.a3d_raster_forward_rgba8_workspace_bytes.restype = C.c_size_t
+        lib.a3d_raster_forward_rgba8_workspace_bytes.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int64]
         lib.a3d_raster_counters_offset.restype = C.c_size_t
         lib.a3d_raster_counters_offset.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int64]
         lib.a3d_raster_backward_scratch_bytes.restype = C.c_size_t

@@ -16,9 +16,14 @@ namespace a3d {
 
 constexpr int kBlockPix = kTile * kTile;
 
+// Output mode of the tile render.  kOutFloat: colour / depth / alpha planes plus the backward's n_contrib / final_T.
+// kOutRGBA8: one uchar4 per pixel, (clamp01(C + T bg), alpha) quantised as the reference saves its test renders; nothing else.
+enum RenderOut { kOutFloat = 0, kOutRGBA8 = 1 };
+
+template <int kOut>
 __global__ void __launch_bounds__(kBlockPix)
 raster_render_forward_kernel(RasterDev a, RasterWs ws, float* __restrict__ out_color, float* __restrict__ out_depth,
-                             float* __restrict__ out_alpha) {
+                             float* __restrict__ out_alpha, uchar4* __restrict__ out_rgba) {
   const int gx = (a.W + kTile - 1) / kTile, gy = (a.H + kTile - 1) / kTile;
   const int cam = blockIdx.z;
   const int tile = blockIdx.y * gx + blockIdx.x;
@@ -60,7 +65,11 @@ raster_render_forward_kernel(RasterDev a, RasterWs ws, float* __restrict__ out_c
       last = contributor;
     }
   }
-  if (inside) {
+  if (inside && kOut == kOutRGBA8) {
+    const size_t hw = (size_t)a.H * a.W, pix = (size_t)py * a.W + px;
+    out_rgba[(size_t)cam * hw + pix] = make_uchar4(quantise_u8(clamp01(C0 + T * a.bg[0])), quantise_u8(clamp01(C1 + T * a.bg[1])),
+                                                   quantise_u8(clamp01(C2 + T * a.bg[2])), quantise_u8(A));
+  } else if (inside) {
     const size_t hw = (size_t)a.H * a.W, pix = (size_t)py * a.W + px;
     out_color[((size_t)cam * 3 + 0) * hw + pix] = C0 + T * a.bg[0];
     out_color[((size_t)cam * 3 + 1) * hw + pix] = C1 + T * a.bg[1];
@@ -249,13 +258,13 @@ struct RasterLayout {
   RasterWs ws;
 };
 
-static RasterLayout raster_layout(void* base, int P, int H, int W, int cams, long long cap) {
+static RasterLayout raster_layout(void* base, int P, int H, int W, int cams, long long cap, bool forward_only = false) {
   RasterLayout l;
   l.gx = (W + kTile - 1) / kTile;
   l.gy = (H + kTile - 1) / kTile;
   l.total_tiles = (long long)cams * l.gx * l.gy;
   l.end_bit = sort_bits(l.total_tiles);
-  l.bytes = carve_workspace(base, P, H, W, cams, cap, cub_temp_bytes(cams * P, cap, l.end_bit), &l.ws);
+  l.bytes = carve_workspace(base, P, H, W, cams, cap, cub_temp_bytes(cams * P, cap, l.end_bit), &l.ws, forward_only);
   return l;
 }
 
@@ -331,16 +340,10 @@ extern "C" size_t a3d_raster_counters_offset(int P, int H, int W, int num_cams, 
   return (size_t)(reinterpret_cast<char*>(l.ws.counters) - probe);
 }
 
-extern "C" int a3d_raster_forward(const a3d_raster_args* a, float* color, float* depth, float* alpha, int32_t* radii,
-                                  void* workspace, size_t workspace_bytes, int64_t max_rendered, int64_t* num_rendered_host,
-                                  void* stream) {
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  if (int r = check_args(a, max_rendered)) return r;
-  if (!color || !depth || !alpha || !radii || !workspace) return fail(A3D_EINVAL, "a3d_raster_forward: null output");
-  const RasterLayout l = raster_layout(workspace, a->P, a->H, a->W, a->num_cams, max_rendered);
-  if (l.bytes > workspace_bytes) return fail(A3D_EINVAL, "a3d_raster_forward: workspace %zu < %zu bytes", workspace_bytes, l.bytes);
+// preprocess, scan, key duplication, radix sort and tile ranges: everything of a forward before the tile render
+static int forward_binning(const a3d_raster_args* a, const RasterLayout& l, const RasterDev& d, int32_t* radii, int64_t max_rendered,
+                           cudaStream_t st) {
   const RasterWs& ws = l.ws;
-  const RasterDev d = make_dev(a);
   const int n = a->num_cams * a->P;
   A3D_CUDA_CHECK(cudaMemsetAsync(ws.keys_a, 0xFF, (size_t)max_rendered * 8, st));
   A3D_CUDA_CHECK(cudaMemsetAsync(ws.ranges, 0, (size_t)l.total_tiles * 8, st));
@@ -360,8 +363,47 @@ extern "C" int a3d_raster_forward(const a3d_raster_args* a, float* color, float*
   stamp(3, st);
   launch_ranges(ws, max_rendered, l.total_tiles, st);
   stamp(4, st);
+  return A3D_OK;
+}
+
+extern "C" int a3d_raster_forward(const a3d_raster_args* a, float* color, float* depth, float* alpha, int32_t* radii,
+                                  void* workspace, size_t workspace_bytes, int64_t max_rendered, int64_t* num_rendered_host,
+                                  void* stream) {
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  if (int r = check_args(a, max_rendered)) return r;
+  if (!color || !depth || !alpha || !radii || !workspace) return fail(A3D_EINVAL, "a3d_raster_forward: null output");
+  const RasterLayout l = raster_layout(workspace, a->P, a->H, a->W, a->num_cams, max_rendered);
+  if (l.bytes > workspace_bytes) return fail(A3D_EINVAL, "a3d_raster_forward: workspace %zu < %zu bytes", workspace_bytes, l.bytes);
+  const RasterWs& ws = l.ws;
+  const RasterDev d = make_dev(a);
+  if (int r = forward_binning(a, l, d, radii, max_rendered, st)) return r;
   dim3 grid(l.gx, l.gy, a->num_cams), block(kTile, kTile);
-  raster_render_forward_kernel<<<grid, block, 0, st>>>(d, ws, color, depth, alpha);
+  raster_render_forward_kernel<kOutFloat><<<grid, block, 0, st>>>(d, ws, color, depth, alpha, nullptr);
+  A3D_LAUNCH_CHECK();
+  stamp(5, st);
+  g_fwd_rec = g_timing;
+  if (num_rendered_host)
+    A3D_CUDA_CHECK(cudaMemcpyAsync(num_rendered_host, ws.counters, sizeof(long long) * (a->num_cams + 2), cudaMemcpyDeviceToHost, st));
+  return A3D_OK;
+}
+
+extern "C" size_t a3d_raster_forward_rgba8_workspace_bytes(int P, int H, int W, int num_cams, int64_t max_rendered) {
+  return raster_layout(nullptr, P, H, W, num_cams, max_rendered, true).bytes;
+}
+
+extern "C" int a3d_raster_forward_rgba8(const a3d_raster_args* a, uint8_t* rgba, int32_t* radii, void* workspace,
+                                        size_t workspace_bytes, int64_t max_rendered, int64_t* num_rendered_host, void* stream) {
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  if (int r = check_args(a, max_rendered)) return r;
+  if (!rgba || !workspace) return fail(A3D_EINVAL, "a3d_raster_forward_rgba8: null output");
+  const RasterLayout l = raster_layout(workspace, a->P, a->H, a->W, a->num_cams, max_rendered, true);
+  if (l.bytes > workspace_bytes)
+    return fail(A3D_EINVAL, "a3d_raster_forward_rgba8: workspace %zu < %zu bytes", workspace_bytes, l.bytes);
+  const RasterWs& ws = l.ws;
+  const RasterDev d = make_dev(a);
+  if (int r = forward_binning(a, l, d, radii ? radii : ws.radii, max_rendered, st)) return r;
+  dim3 grid(l.gx, l.gy, a->num_cams), block(kTile, kTile);
+  raster_render_forward_kernel<kOutRGBA8><<<grid, block, 0, st>>>(d, ws, nullptr, nullptr, nullptr, reinterpret_cast<uchar4*>(rgba));
   A3D_LAUNCH_CHECK();
   stamp(5, st);
   g_fwd_rec = g_timing;

@@ -223,6 +223,23 @@ A3D_HD float splat_alpha(float gx, float gy, float conA, float conB, float conC,
   return alpha;
 }
 
+// ---------------------------------------------------------------------------------------------------------------
+// RGBA8 test renders: the reference saves cat(render.clamp(0, 1), mask) as (rgba * 255).astype(np.uint8)
+// (diff_gaussian_rasterizer_advanced_4d.py:180, systems/animate3d.py:439-445)
+// ---------------------------------------------------------------------------------------------------------------
+A3D_HD float clamp01(float v) { return fminf(fmaxf(v, 0.0f), 1.0f); }
+
+// One rounded fp32 multiply by 255 (never contracted into an FMA), then numpy's float32 -> uint8 cast on x86: truncation
+// toward zero to int32 and the low 8 bits of that (so 1.5 -> 126, -0.5 -> 129).  Defined for |v * 255| < 2^31.
+A3D_HD uint8_t quantise_u8(float v) {
+#if defined(__CUDA_ARCH__)
+  const float p = __fmul_rn(v, 255.0f);
+#else
+  const float p = v * 255.0f;
+#endif
+  return (uint8_t)(uint32_t)(int32_t)p;
+}
+
 struct SplatGrad {   // partial derivatives of the loss w.r.t. one gaussian's screen-space quantities from ONE pixel
   float dmx, dmy;          // d/d(mean2D in pixels)
   float dconA, dconB, dconC;

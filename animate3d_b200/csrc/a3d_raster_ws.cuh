@@ -32,18 +32,21 @@ struct RasterWs {
   uint64_t *keys_a, *keys_b;
   uint32_t *vals_a, *vals_b;
   uint2* ranges;
-  // per pixel
+  // per pixel (backward state: null in a forward-only workspace)
   uint32_t* n_contrib;
   float* final_T;
   long long* counters;   // [cams] pair counts, [cams] total, [cams+1] overflow flag
-  // backward scratch, per (camera, gaussian)
+  // backward scratch, per (camera, gaussian) (null in a forward-only workspace)
   float *g_mean2d, *g_conic, *g_depth, *g_rgb;
+  int32_t* radii;        // forward-only workspace: radii of a caller that asked for none, per (camera, gaussian)
   void* cub_temp;
   size_t cub_bytes;
 };
 
-// Carves `base` (may be null for a size query) and returns the bytes needed.
-inline size_t carve_workspace(void* base, int P, int H, int W, int cams, long long cap, size_t cub_bytes, RasterWs* ws) {
+// Carves `base` (may be null for a size query) and returns the bytes needed.  forward_only (the RGBA8 render) leaves out
+// the per-pixel backward state and the backward scratch and adds a radii buffer; the training layout is unchanged by it.
+inline size_t carve_workspace(void* base, int P, int H, int W, int cams, long long cap, size_t cub_bytes, RasterWs* ws,
+                              bool forward_only = false) {
   Carve c{static_cast<char*>(base)};
   const size_t n = (size_t)cams * P;
   const int gx = (W + kTile - 1) / kTile, gy = (H + kTile - 1) / kTile;
@@ -61,13 +64,22 @@ inline size_t carve_workspace(void* base, int P, int H, int W, int cams, long lo
   w.vals_a = c.take<uint32_t>(cap);
   w.vals_b = c.take<uint32_t>(cap);
   w.ranges = c.take<uint2>((size_t)cams * gx * gy);
-  w.n_contrib = c.take<uint32_t>((size_t)cams * H * W);
-  w.final_T = c.take<float>((size_t)cams * H * W);
-  w.counters = c.take<long long>(cams + 2);
-  w.g_mean2d = c.take<float>(2 * n);
-  w.g_conic = c.take<float>(3 * n);
-  w.g_depth = c.take<float>(n);
-  w.g_rgb = c.take<float>(3 * n);
+  w.n_contrib = nullptr;
+  w.final_T = nullptr;
+  w.g_mean2d = w.g_conic = w.g_depth = w.g_rgb = nullptr;
+  w.radii = nullptr;
+  if (forward_only) {
+    w.counters = c.take<long long>(cams + 2);
+    w.radii = c.take<int32_t>(n);
+  } else {
+    w.n_contrib = c.take<uint32_t>((size_t)cams * H * W);
+    w.final_T = c.take<float>((size_t)cams * H * W);
+    w.counters = c.take<long long>(cams + 2);
+    w.g_mean2d = c.take<float>(2 * n);
+    w.g_conic = c.take<float>(3 * n);
+    w.g_depth = c.take<float>(n);
+    w.g_rgb = c.take<float>(3 * n);
+  }
   w.cub_temp = c.take<char>(cub_bytes);
   w.cub_bytes = cub_bytes;
   if (ws) *ws = w;

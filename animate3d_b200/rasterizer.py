@@ -211,6 +211,60 @@ def rasterize_batch(means3D, scales, rotations, opacities, shs, colors_precomp, 
     return _RasterizeBatch.apply(means3D, means2D, scales, rotations, opacities, shs, colors_precomp, cams_t, meta)
 
 
+class PairBudgetExceeded(L.A3DError):
+    """A multi-camera RGBA8 render needs more (tile, gaussian) pairs than its budget: render fewer cameras per call."""
+
+
+class RGBA8Renderer:
+    """Forward-only renders straight to RGBA8 (a3d_raster_forward_rgba8): no autograd, no float planes, no backward state.
+    One workspace is reused across calls and grown when a call needs more.  The pair capacity of a call comes from the pairs
+    per camera of the previous one; on overflow the call grows it and renders again, like the eager training forward."""
+
+    def __init__(self, max_pairs: int = 1 << 27):
+        self.max_pairs = max_pairs
+        self.ws: Optional[torch.Tensor] = None
+        self.pairs_per_cam = 0.0
+        self.overflows = 0          # re-renders after an overflow, over the renderer's lifetime
+        self.last_total = 0         # pairs of the last call
+        self._counts: Optional[torch.Tensor] = None
+
+    def render(self, cams_t, H: int, W: int, means3D, scales, rotations, opacities, shs, colors, sh_degree: int, per_cam: bool,
+               bg, scale_modifier: float = 1.0, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """rgba [cams, H, W, 4] uint8 (into `out` when given, which must be contiguous).  Arguments as `_make_args`;
+        means3D / scales / rotations are [cams, P, *] with per_cam, else [P, *].  Synchronises the stream once per render."""
+        lib = L.load()
+        ncam, P, dev = cams_t.shape[0], means3D.shape[-2], means3D.device
+        if out is None:
+            out = torch.empty(ncam, H, W, 4, dtype=torch.uint8, device=dev)
+        if out.shape != (ncam, H, W, 4) or out.dtype != torch.uint8 or not out.is_contiguous():
+            raise ValueError(f"out must be a contiguous uint8 [{ncam}, {H}, {W}, 4] tensor")
+        if self._counts is None or self._counts.numel() < ncam + 2:
+            self._counts = torch.empty(ncam + 2, dtype=torch.int64).pin_memory()
+        counts = self._counts
+        args = _make_args(P, H, W, cams_t, means3D, scales, rotations, opacities, shs, colors, sh_degree, per_cam, scale_modifier, bg)
+        cap = max(int(self.pairs_per_cam * ncam * 1.08) + 1024, 1 << 16) if self.pairs_per_cam else max(1 << 16, 4 * P * ncam)
+        cap = min(cap, self.max_pairs if ncam > 1 else 0x7FFFFFFF)
+        while True:
+            nbytes = lib.a3d_raster_forward_rgba8_workspace_bytes(P, H, W, ncam, C.c_int64(cap))
+            if self.ws is None or self.ws.numel() < nbytes:
+                self.ws = None                              # free the old one first
+                self.ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+            L.check(lib.a3d_raster_forward_rgba8(C.byref(args), C.c_void_p(out.data_ptr()), None, C.c_void_p(self.ws.data_ptr()),
+                                                 C.c_size_t(self.ws.numel()), C.c_int64(cap), C.c_void_p(counts.data_ptr()),
+                                                 L.stream_ptr()))
+            torch.cuda.current_stream().synchronize()
+            total = int(counts[ncam])
+            if int(counts[ncam + 1]) == 0:
+                break
+            self.overflows += 1
+            cap = int(total * 1.25) + 1024
+            if cap > self.max_pairs and ncam > 1:
+                raise PairBudgetExceeded(f"{ncam} cameras need {total} pairs, over the budget of {self.max_pairs}")
+        self.last_total = total
+        self.pairs_per_cam = total / ncam
+        return out
+
+
 class GaussianRasterizer(torch.nn.Module):
     def __init__(self, raster_settings: GaussianRasterizationSettings):
         super().__init__()

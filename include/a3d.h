@@ -224,6 +224,18 @@ int a3d_raster_forward(const a3d_raster_args* args, float* color, float* depth, 
  * reads them here.  After an overflow the pairs past max_rendered are dropped (the render is incomplete but every access
  * stays inside the workspace, and a3d_raster_backward stays inside its scratch). */
 size_t a3d_raster_counters_offset(int P, int H, int W, int num_cams, int64_t max_rendered);
+/* Forward-only render straight to RGBA8, for test-view renders.  Replaces the per-camera test path of the reference:
+ * rasterize_gaussians at custom/threestudio-animate3d/renderer/diff_gaussian_rasterizer_advanced_4d.py:161-170, the clamp at
+ * :180, and systems/animate3d.py:439-445, which saves cat(render, mask) as (rgba * 255).astype(np.uint8).
+ * rgba [cams,H,W,4] uint8: per pixel (q(clamp(C + T*bg, 0, 1)), q(alpha)) with q(v) = (uint8)(int32)(v *rn 255) -- one
+ * rounded fp32 multiply, truncation toward zero, the low 8 bits (numpy's cast on x86); alpha is not clamped.  The same
+ * preprocess, binning and sort as a3d_raster_forward, so the bytes equal quantising that call's color / alpha.  radii may
+ * be NULL.  No float planes and no backward state are written, so the workspace (a3d_raster_forward_rgba8_workspace_bytes)
+ * is smaller than a3d_raster_workspace_bytes; it cannot serve a3d_raster_backward.  Counters and overflow behave as in
+ * a3d_raster_forward (num_rendered_host: pinned [cams+2], optional). */
+size_t a3d_raster_forward_rgba8_workspace_bytes(int P, int H, int W, int num_cams, int64_t max_rendered);
+int a3d_raster_forward_rgba8(const a3d_raster_args* args, uint8_t* rgba, int32_t* radii, void* workspace, size_t workspace_bytes,
+                             int64_t max_rendered, int64_t* num_rendered_host, void* stream);
 /* Scratch bytes a3d_raster_backward needs: 0 when args->deterministic is 0, else 40 B per (tile, gaussian) pair slot of
  * max_rendered plus 4 B per (camera, gaussian). */
 size_t a3d_raster_backward_scratch_bytes(const a3d_raster_args* args, int64_t max_rendered);
