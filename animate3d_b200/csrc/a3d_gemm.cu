@@ -3,6 +3,8 @@
 //     of the 128-row tile, issues wgmma.mma_async on the staged operands and runs the epilogue straight from its fp32
 //     accumulator registers while the producer already fills the ring for the next tile
 //   * operands staged by TMA into 128B-swizzled shared memory (K-major) through a ring of mbarrier-guarded stages
+//   * the tile's bias slice and the row-bias rows of a warpgroup's 64 rows are copied into that warpgroup's shared-memory
+//     buffer (cp.async) under the tile's main loop, so the epilogue reads them without a global round trip
 //   * A3D_A_CONV3: the A operand is an implicit 3x3 im2col of an NHWC image -- each k-block is one (tap, 64-channel)
 //     slice fetched with a rank-4 TMA box whose out-of-bounds rows/cols are zero-filled by the hardware (= padding 1);
 //     stride-2 convolutions use the tensor map's traversal strides
@@ -29,6 +31,8 @@ struct GemmDev {
   int bimg;       // images per tile
   int tpr;        // tiles per output row (> 1 when an output row is wider than the 128-row tile)
   int conv_pad;   // zero padding in front of row / column 0 (1, or 0 for the asymmetric (0,1,0,1) padding of the VAE downsampler)
+  int stages;     // operand ring depth
+  int rb_slots;   // row-bias rows a warpgroup's buffer holds (gemm_rb_slots)
   // epilogue
   const float* bias;
   const float* rowbias;
@@ -60,9 +64,10 @@ __device__ __forceinline__ float gelu_erf(float x) {
   return fmaf(fabsf(h), erf_abs, h);
 }
 
-__device__ __forceinline__ int64_t perm_row(int64_t m, int64_t a, int64_t b) {
+template <typename T>
+__device__ __forceinline__ T perm_row(T m, T a, T b) {
   if (a == 0) return m;
-  const int64_t ab = a * b;
+  const T ab = a * b;
   return (m / ab) * ab + (m % b) * a + (m / b) % a;
 }
 
@@ -70,16 +75,33 @@ constexpr int kBM = 128;
 constexpr int kBK = 64;
 constexpr int kGemmThreads = 288;   // 2 consumer warpgroups + 1 producer warp
 
+constexpr int kGemmSmemMax = 227 * 1024;
+constexpr int kMaxStages = 6;
+
+// Shared memory: the operand ring (stages x kStageBytes, 1024-aligned), its barriers, then one epilogue buffer per consumer
+// warpgroup: the tile's bias slice (row 0) and rb_slots row-bias rows, kEpiLd floats apart.  The epilogue reads 8 bytes per
+// lane; with kEpiLd = 8 mod 32 the four row groups of a half-warp land on 32 distinct banks even when each reads its own row.
 template <int BN>
 struct GemmCfg {
   static constexpr int kABytes = kBM * kBK * 2;
   static constexpr int kBBytes = BN * kBK * 2;
   static constexpr int kStageBytes = kABytes + kBBytes;
-  // as many stages as fit next to nothing else: the epilogue works from registers and needs no shared memory
-  static constexpr int kStages = (227 * 1024 - 1024 - 256) / kStageBytes > 6 ? 6 : (227 * 1024 - 1024 - 256) / kStageBytes;
-  static constexpr int kSmemBytes = kStages * kStageBytes + 1024 /*align slack*/ + 256 /*barriers*/;
-  static_assert(kSmemBytes <= 227 * 1024, "shared memory budget");
+  static constexpr int kEpiLd = BN + 8;
+  static constexpr int epi_bytes(int rb_slots) { return 2 * (1 + rb_slots) * kEpiLd * 4; }
+  // as many stages as fit next to the epilogue buffers, at most kMaxStages
+  static constexpr int stages(int rb_slots) {
+    return (kGemmSmemMax - 1024 - 256 - epi_bytes(rb_slots)) / kStageBytes > kMaxStages
+               ? kMaxStages
+               : (kGemmSmemMax - 1024 - 256 - epi_bytes(rb_slots)) / kStageBytes;
+  }
+  static constexpr int smem_bytes(int stages, int rb_slots) {
+    return stages * kStageBytes + 1024 /*align slack*/ + 256 /*barriers*/ + epi_bytes(rb_slots);
+  }
 };
+// a warpgroup's 64 rows use at most 64 row-bias rows; the 256-column tile falls back to 128 columns when they leave room for
+// fewer than two stages (gemm_rb_slots)
+static_assert(GemmCfg<128>::stages(64) >= 2 && GemmCfg<160>::stages(64) >= 2, "shared memory budget");
+static_assert(GemmCfg<256>::stages(16) >= 3, "shared memory budget");
 
 template <int BN>
 __device__ __forceinline__ void wgmma_tile(float (&d)[BN / 2], uint64_t adesc, uint64_t bdesc, uint32_t acc) {
@@ -91,20 +113,19 @@ __device__ __forceinline__ void wgmma_tile(float (&d)[BN / 2], uint64_t adesc, u
 // EPI: 0 = bias/row-bias only, 1 = + residuals / row permutation, 2 = GEGLU, 3 = fp32 output, 4 = GELU of the biased value
 enum { kEpiPlain = 0, kEpiRes = 1, kEpiGeglu = 2, kEpiF32 = 3, kEpiGelu = 4 };
 
-// The epilogue walks a thread's 8-column groups in chunks of G groups, both of its rows at once.  All global operands of a
-// chunk are requested together, and (kAhead) those of the next chunk before the current one is stored, so a thread waits for
-// memory once per chunk rather than once per group and row.  A GEGLU chunk holds G / 2 value groups and their gates.  The
-// operands sit in registers next to the accumulators, and a 288-thread CTA puts three warps on one SM sub-partition, which
-// caps a thread at 168 registers.  At BN = 256 the 128 accumulator registers leave room for one chunk's operands only, so
-// there the next chunk is requested after the current one is stored.  Residual rows are fetched into L2 ahead of the
-// epilogue at every BN (see the main loop).
+// The epilogue walks a thread's 8-column groups in chunks of G groups, both of its rows at once.  Bias and row-bias come
+// from the warpgroup's shared-memory buffer; the only global operands are the residuals (kEpiRes).  Those of a chunk are
+// requested together, and those of the next chunk before the current one is stored, so a thread waits for memory once per
+// chunk rather than once per group and row.  A GEGLU chunk holds G / 2 value groups and their gates.  The residuals sit in
+// registers next to the accumulators, and a 288-thread CTA puts three warps on one SM sub-partition, which caps a thread at
+// 168 registers.  At BN = 256 the 128 accumulator registers leave room for one group's residuals only, so there the next
+// group is requested after the current one is stored.  Residual rows are fetched into L2 ahead of the epilogue (see the
+// main loop).
 template <int BN, int EPI>
 struct EpiChunk {
-  static constexpr int G = BN == 256 ? 1 + (EPI == kEpiGeglu) : 2;
-  static constexpr bool kAhead = BN != 256;
-  float bias[G][2];
-  float rb[2][G][2];                  // [row][group][column]
-  uint32_t r1[2][G], r2[2][G];        // fp16x2 residuals (kEpiRes only)
+  static constexpr int G = BN == 256 && EPI == kEpiRes ? 1 : 2;
+  static constexpr bool kAhead = G == 2;
+  uint32_t r1[2][G], r2[2][G];        // [row][group] fp16x2 residuals (kEpiRes only)
 };
 
 // accumulator group (8 columns) of slot s of chunk c; GEGLU: slots < G / 2 hold values u of output group o, the others
@@ -121,19 +142,38 @@ __device__ __forceinline__ constexpr int epi_group(int c, int s) {
 
 __device__ __forceinline__ void prefetch_l2(const void* a) { asm volatile("prefetch.global.L2 [%0];" ::"l"(a)); }
 
+// 4-byte copies: the ABI guarantees bias / row-bias 4-byte alignment only
+__device__ __forceinline__ void cp_async_4(uint32_t smem_dst, const void* src) {
+  asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(smem_dst), "l"(src) : "memory");
+}
+// ordered with the epilogue's global stores like the global loads it replaces: a plain load would be hoisted over them,
+// and the loads of every chunk would then compete with the accumulators for registers
+__device__ __forceinline__ float2 lds_f32x2(uint32_t a) {
+  float2 v;
+  asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "r"(a) : "memory");
+  return v;
+}
+__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
+// barrier of one consumer warpgroup (ids 1, 2; 0 is __syncthreads)
+__device__ __forceinline__ void warpgroup_sync(int wg) {
+  if (wg == 0) asm volatile("bar.sync 1, 128;" ::: "memory");
+  else asm volatile("bar.sync 2, 128;" ::: "memory");
+}
+
 template <int BN, int EPI>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_tc_kernel(const GemmDev p, const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB) {
   static_assert(EPI != kEpiGeglu || BN % 64 == 0, "GEGLU pairs a value with its gate inside 64-column blocks");
   static_assert((BN / 8) % EpiChunk<BN, EPI>::G == 0, "the tile's column groups split into whole chunks");
   using Cfg = GemmCfg<BN>;
-  constexpr int kStages = Cfg::kStages;
+  const int num_stages = p.stages;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* smem_a = smem;
-  uint8_t* smem_b = smem + kStages * Cfg::kABytes;
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + kStages * Cfg::kStageBytes);   // [kStages]
-  uint64_t* empty_bar = full_bar + kStages;                                              // [kStages]
+  uint8_t* smem_b = smem + num_stages * Cfg::kABytes;
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + num_stages * Cfg::kStageBytes);   // [num_stages]
+  uint64_t* empty_bar = full_bar + num_stages;                                              // [num_stages]
+  float* epi_buf = reinterpret_cast<float*>(smem + num_stages * Cfg::kStageBytes + 256);    // [2][1 + rb_slots][kEpiLd]
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -142,7 +182,7 @@ gemm_tc_kernel(const GemmDev p, const __grid_constant__ CUtensorMap mapA, const 
   if (warp == 8 && lane == 0) {
     tma_prefetch_desc(&mapA);
     tma_prefetch_desc(&mapB);
-    for (int i = 0; i < kStages; ++i) {
+    for (int i = 0; i < num_stages; ++i) {
       mbar_init(&full_bar[i], 1);
       mbar_init(&empty_bar[i], 8);   // one arrive per consumer warp
     }
@@ -175,7 +215,7 @@ gemm_tc_kernel(const GemmDev p, const __grid_constant__ CUtensorMap mapA, const 
             tma_load_5d(smem_a + stage * Cfg::kABytes, &mapA, &full_bar[stage], kb * kBK, mt * kBM, 0, 0, 0);
           }
           tma_load_5d(smem_b + stage * Cfg::kBBytes, &mapB, &full_bar[stage], kb * kBK, nt * BN, 0, 0, 0);
-          if (++stage == kStages) { stage = 0; phase ^= 1; }
+          if (++stage == num_stages) { stage = 0; phase ^= 1; }
         }
       }
     }
@@ -185,23 +225,61 @@ gemm_tc_kernel(const GemmDev p, const __grid_constant__ CUtensorMap mapA, const 
   // -------------------------------------------------------------------- consumers: 2 warpgroups x 64 rows
   const int wg = warp >> 2;
   const int g = lane >> 2, t = lane & 3;
+  const uint32_t epi = smem_u32(epi_buf + wg * (1 + p.rb_slots) * Cfg::kEpiLd);
   int stage = 0;
   uint32_t phase = 0;
-  int tcount = 0;
   float acc[BN / 2];
-  for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++tcount) {
+  // one loop counter (tcount); the tile index is derived from it rather than kept live across the main loop
+  for (int tcount = 0; (int)(blockIdx.x + tcount * gridDim.x) < num_tiles; ++tcount) {
+    const int tile = blockIdx.x + tcount * gridDim.x;
     const int mt = tile / p.tiles_n, nt = tile % p.tiles_n;
     const bool tr = p.trace && blockIdx.x == 0 && threadIdx.x == 0 && tcount < 60;
     if (tr) p.trace[tcount * 16 + 0] = clock64();
     // epilogue rows of this thread: row[h] = 16 w + g + 8 h of the warpgroup's 64; group j = columns 8 j + 2 t, +1.
     // R2 and C are read / written at the same (orow, n) by the same thread, so R2 may be C.  R1 is read at (row, n), which
-    // another thread writes when the rows are permuted: R1 must not alias C then (see a3d.h).
-    const int64_t col_base = (int64_t)nt * BN + 2 * t;
-    int64_t row[2], orow[2];
+    // another thread writes when the rows are permuted: R1 must not alias C then (see a3d.h).  Row indices are divided in
+    // 32 bits (a3d_gemm checks that they fit): a 64-bit division is a subroutine call, and with the 128 accumulator
+    // registers of BN = 256 live, ptxas spills around it.
+    const int col_base = nt * BN + 2 * t;
+    uint32_t row[2], orow[2];
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
-      row[h] = (int64_t)mt * kBM + wg * 64 + (warp & 3) * 16 + g + 8 * h;
-      orow[h] = (EPI == kEpiRes) ? perm_row(row[h], p.perm_a, p.perm_b) : row[h];
+      row[h] = (uint32_t)mt * kBM + wg * 64 + (warp & 3) * 16 + g + 8 * h;
+      orow[h] = (EPI == kEpiRes) ? perm_row<uint32_t>(row[h], (uint32_t)p.perm_a, (uint32_t)p.perm_b) : row[h];
+    }
+    // ---- epilogue buffer, filled under the main loop once every thread of the warpgroup is done with the previous tile's.
+    // Row-bias rows m0 .. m1 (those < M) of the warpgroup use table rows q % rb_mod, q = q0 .. m1 / rb_div; slot s holds
+    // table row (q0 + s) % rb_mod and row m reads slot (m / rb_div - q0) % nslots: when the window wraps (nslots = rb_mod)
+    // the modulo keeps the slots distinct.  Columns past N are zero-filled, not read.  Bits 16 h .. 16 h + 15 of rb_off:
+    // the float offset in epi of this thread's columns 2 t, 2 t + 1 of row h's slot, 0xffff without a row-bias or past M
+    // (one register: it stays live across the main loop next to the accumulators).
+    uint32_t rb_off = 0xffffffffu;
+    {
+      const int64_t n0 = (int64_t)nt * BN;
+      const int ncols = p.N - n0 < BN ? (int)(p.N - n0) : BN;
+      const uint32_t m0 = (uint32_t)mt * kBM + wg * 64, M = (uint32_t)p.M;
+      const uint32_t rb_div = (uint32_t)p.rb_div, rb_mod = (uint32_t)p.rb_mod;
+      uint32_t nslots = 0, q = 0;
+      if (p.rowbias && m0 < M) {
+        const uint32_t m1 = m0 + 63 < M ? m0 + 63 : M - 1;
+        const uint32_t q0 = m0 / rb_div;
+        nslots = m1 / rb_div - q0 + 1 < rb_mod ? m1 / rb_div - q0 + 1 : rb_mod;
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+          if (row[h] < M)
+            rb_off ^= (0xffffu ^ ((1 + (row[h] / rb_div - q0) % nslots) * Cfg::kEpiLd + 2 * t)) << 16 * h;
+        q = q0 % rb_mod;
+      }
+      if (tcount > 0) warpgroup_sync(wg);
+      for (uint32_t r = p.bias ? 0 : 1; r <= nslots; ++r) {
+        const float* src = (r == 0 ? p.bias : p.rowbias + q * p.rb_ld) + n0;
+        const uint32_t dst = epi + 4 * r * Cfg::kEpiLd;
+        for (int c = threadIdx.x & 127; c < BN; c += 128) {
+          if (c < ncols) cp_async_4(dst + 4 * c, src + c);
+          else asm volatile("st.shared.f32 [%0], %1;" ::"r"(dst + 4 * c), "f"(0.f) : "memory");
+        }
+        if (r > 0 && ++q == rb_mod) q = 0;
+      }
     }
     // ---- main loop: one wgmma group in flight; the stage of k-block kb-1 is released once group kb-1 has retired
     int prev_stage = -1;
@@ -211,7 +289,7 @@ gemm_tc_kernel(const GemmDev p, const __grid_constant__ CUtensorMap mapA, const 
         // HBM miss, close enough that the operand stream of a long-K tile does not evict them first.  The four lanes of a
         // row take its 128-byte lines t, t + 4 (a row's BN halves span at most 2 BN / 128 + 1 lines).
         if (kb == (p.num_k_blocks > 2 ? p.num_k_blocks - 2 : 0)) {
-          const int64_t ncols = p.N - (int64_t)nt * BN < BN ? p.N - (int64_t)nt * BN : BN;
+          const int ncols = p.N - nt * BN < BN ? (int)p.N - nt * BN : BN;
           auto fetch = [&](const __half* a, bool ok) {
             const uintptr_t e = reinterpret_cast<uintptr_t>(a + ncols), l0 = reinterpret_cast<uintptr_t>(a) & ~uintptr_t(127);
 #pragma unroll
@@ -222,8 +300,8 @@ gemm_tc_kernel(const GemmDev p, const __grid_constant__ CUtensorMap mapA, const 
           };
 #pragma unroll
           for (int h = 0; h < 2; ++h) {
-            fetch(p.R1 + row[h] * p.ldr1 + (int64_t)nt * BN, p.R1 && row[h] < p.M);
-            fetch(p.R2 + orow[h] * p.ldr2 + (int64_t)nt * BN, p.R2 && row[h] < p.M);
+            fetch(p.R1 + row[h] * p.ldr1 + nt * BN, p.R1 && row[h] < p.M);
+            fetch(p.R2 + orow[h] * p.ldr2 + nt * BN, p.R2 && row[h] < p.M);
           }
         }
       }
@@ -239,47 +317,49 @@ gemm_tc_kernel(const GemmDev p, const __grid_constant__ CUtensorMap mapA, const 
       wgmma_wait<1>();
       if (prev_stage >= 0 && lane == 0) mbar_arrive(&empty_bar[prev_stage]);
       prev_stage = stage;
-      if (++stage == kStages) { stage = 0; phase ^= 1; }
+      if (++stage == num_stages) { stage = 0; phase ^= 1; }
     }
 
     // ---- epilogue from registers, chunk by chunk (EpiChunk): chunk c covers groups epi_group(c, 0 .. G - 1) of both rows
     using Chunk = EpiChunk<BN, EPI>;
     constexpr int G = Chunk::G;
     constexpr int kChunks = BN / 8 / G;
-    const float* rb[2];
-#pragma unroll
-    for (int h = 0; h < 2; ++h) rb[h] = p.rowbias ? p.rowbias + ((row[h] / p.rb_div) % p.rb_mod) * p.rb_ld : nullptr;
     Chunk op;
     auto load_chunk = [&](int c) {
+      if constexpr (EPI == kEpiRes) {
 #pragma unroll
-      for (int s = 0; s < G; ++s) {
-        const int64_t n = col_base + 8 * epi_group<EPI, G>(c, s);
-        const bool col_ok = n < p.N;
-        // coherent loads, unlike __ldg: they cannot be hoisted above the previous chunk's stores, which would hold the
-        // operands of every chunk in registers at once
-        op.bias[s][0] = (p.bias && col_ok) ? p.bias[n] : 0.f;
-        op.bias[s][1] = (p.bias && col_ok) ? p.bias[n + 1] : 0.f;
+        for (int s = 0; s < G; ++s) {
+          const int64_t n = col_base + 8 * epi_group<EPI, G>(c, s);
 #pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          const bool ok = col_ok && row[h] < p.M;
-          op.rb[h][s][0] = (rb[h] && ok) ? rb[h][n] : 0.f;
-          op.rb[h][s][1] = (rb[h] && ok) ? rb[h][n + 1] : 0.f;
-          if constexpr (EPI == kEpiRes) {
+          for (int h = 0; h < 2; ++h) {
+            const bool ok = n < p.N && row[h] < p.M;
+            // coherent loads, unlike __ldg: they cannot be hoisted above the previous chunk's stores, which would hold the
+            // operands of every chunk in registers at once
             op.r1[h][s] = (p.R1 && ok) ? *reinterpret_cast<const uint32_t*>(p.R1 + row[h] * p.ldr1 + n) : 0u;
             op.r2[h][s] = (p.R2 && ok) ? *reinterpret_cast<const uint32_t*>(p.R2 + orow[h] * p.ldr2 + n) : 0u;
           }
         }
       }
     };
-    // same order as the SIMT kernel: (acc + bias + row-bias) * acc_scale, then + r1_scale R1, + R2
-    auto finish = [&](float v, int h, int s, int e) {
-      if (p.bias) v += op.bias[s][e];
-      if (rb[h]) v += op.rb[h][s][e];
-      return v * p.acc_scale;
+    // same order as the SIMT kernel: (acc + bias + row-bias) * acc_scale, then + r1_scale R1, + R2; columns 8 j + 2 t, +1
+    // of row h
+    auto finish = [&](float v0, float v1, int h, int j) {
+      if (p.bias) {
+        const float2 b = lds_f32x2(epi + 4 * (2 * t + 8 * j));
+        v0 += b.x; v1 += b.y;
+      }
+      const uint32_t off = (rb_off >> 16 * h) & 0xffffu;
+      if (off != 0xffffu) {
+        const float2 r = lds_f32x2(epi + 4 * (off + 8 * j));
+        v0 += r.x; v1 += r.y;
+      }
+      return make_float2(v0 * p.acc_scale, v1 * p.acc_scale);
     };
     auto half2_float2 = [](uint32_t u) { return __half22float2(*reinterpret_cast<const __half2*>(&u)); };
 
     if constexpr (Chunk::kAhead) load_chunk(0);   // under the last MMA group
+    cp_async_wait_all();
+    warpgroup_sync(wg);
     wgmma_wait<0>();
     reg_fence(acc);
     if (lane == 0) mbar_arrive(&empty_bar[prev_stage]);
@@ -295,9 +375,9 @@ gemm_tc_kernel(const GemmDev p, const __grid_constant__ CUtensorMap mapA, const 
 #pragma unroll
           for (int s = 0; s < G / 2; ++s) {
             const int ju = epi_group<EPI, G>(c, s), jg = epi_group<EPI, G>(c, s + G / 2);
-            const float u0 = finish(acc[4 * ju + 2 * h], h, s, 0), u1 = finish(acc[4 * ju + 2 * h + 1], h, s, 1);
-            const float g0 = finish(acc[4 * jg + 2 * h], h, s + G / 2, 0), g1 = finish(acc[4 * jg + 2 * h + 1], h, s + G / 2, 1);
-            out[h][s] = pack_f16x2(u0 * gelu_erf(g0), u1 * gelu_erf(g1));
+            const float2 u = finish(acc[4 * ju + 2 * h], acc[4 * ju + 2 * h + 1], h, ju);
+            const float2 gt = finish(acc[4 * jg + 2 * h], acc[4 * jg + 2 * h + 1], h, jg);
+            out[h][s] = pack_f16x2(u.x * gelu_erf(gt.x), u.y * gelu_erf(gt.y));
           }
         if (Chunk::kAhead && c + 1 < kChunks) load_chunk(c + 1);
 #pragma unroll
@@ -312,13 +392,14 @@ gemm_tc_kernel(const GemmDev p, const __grid_constant__ CUtensorMap mapA, const 
           }
         }
       } else if constexpr (EPI == kEpiF32) {
-        float out[2][G][2];
+        float2 out[2][G];
 #pragma unroll
         for (int h = 0; h < 2; ++h)
 #pragma unroll
-          for (int s = 0; s < G; ++s)
-#pragma unroll
-            for (int e = 0; e < 2; ++e) out[h][s][e] = finish(acc[4 * (c * G + s) + 2 * h + e], h, s, e);
+          for (int s = 0; s < G; ++s) {
+            const int j = c * G + s;
+            out[h][s] = finish(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1], h, j);
+          }
         if (Chunk::kAhead && c + 1 < kChunks) load_chunk(c + 1);
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
@@ -328,8 +409,8 @@ gemm_tc_kernel(const GemmDev p, const __grid_constant__ CUtensorMap mapA, const 
           for (int s = 0; s < G; ++s) {
             const int64_t n = col_base + 8 * (c * G + s);
             if (n >= p.N) continue;
-            crow[n] = out[h][s][0];
-            crow[n + 1] = out[h][s][1];
+            crow[n] = out[h][s].x;
+            crow[n + 1] = out[h][s].y;
           }
         }
       } else {
@@ -339,7 +420,8 @@ gemm_tc_kernel(const GemmDev p, const __grid_constant__ CUtensorMap mapA, const 
 #pragma unroll
           for (int s = 0; s < G; ++s) {
             const int j = c * G + s;
-            float v0 = finish(acc[4 * j + 2 * h], h, s, 0), v1 = finish(acc[4 * j + 2 * h + 1], h, s, 1);
+            const float2 f = finish(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1], h, j);
+            float v0 = f.x, v1 = f.y;
             if constexpr (EPI == kEpiGelu) {
               v0 = gelu_erf(v0); v1 = gelu_erf(v1);
             }
@@ -429,15 +511,17 @@ __global__ void gemm_simt_kernel(const GemmDev p, const __half* __restrict__ A, 
 
 template <int BN, int EPI>
 static int launch_tc_epi(const GemmDev& dev, const CUtensorMap* mapA, const CUtensorMap* mapB, cudaStream_t st) {
-  using Cfg = GemmCfg<BN>;
   static bool attr_set = false;
   if (!attr_set) {
-    A3D_CUDA_CHECK(cudaFuncSetAttribute(gemm_tc_kernel<BN, EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
+    A3D_CUDA_CHECK(cudaFuncSetAttribute(gemm_tc_kernel<BN, EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, kGemmSmemMax));
     attr_set = true;
   }
+  const int smem = GemmCfg<BN>::smem_bytes(dev.stages, dev.rb_slots);
+  if (dev.stages < 2 || smem > kGemmSmemMax)
+    return fail(A3D_EINVAL, "a3d_gemm: %d row-bias rows per warpgroup leave no room for the operand ring", dev.rb_slots);
   const int tiles = dev.tiles_m * dev.tiles_n;
   const int grid = tiles < sm_count() ? tiles : sm_count();
-  gemm_tc_kernel<BN, EPI><<<grid, kGemmThreads, Cfg::kSmemBytes, st>>>(dev, *mapA, *mapB);
+  gemm_tc_kernel<BN, EPI><<<grid, kGemmThreads, smem, st>>>(dev, *mapA, *mapB);
   A3D_LAUNCH_CHECK();
   return A3D_OK;
 }
@@ -452,6 +536,14 @@ static int launch_tc(const GemmDev& dev, const CUtensorMap* mapA, const CUtensor
   if (dev.geglu == 2) return launch_tc_epi<BN, kEpiGelu>(dev, mapA, mapB, st);
   if (dev.R1 || dev.R2 || dev.perm_a) return launch_tc_epi<BN, kEpiRes>(dev, mapA, mapB, st);
   return launch_tc_epi<BN, kEpiPlain>(dev, mapA, mapB, st);
+}
+
+// Row-bias rows the 64 rows of one warpgroup use: their quotients m / rb_div span at most ceil(63 / rb_div) + 1 values,
+// and at most rb_mod of them are distinct table rows (rb_mod is at most the number of quotients of all M rows, see a3d_gemm).
+static int gemm_rb_slots(const GemmDev& d) {
+  if (!d.rowbias) return 0;
+  const int64_t s = 63 / d.rb_div + (63 % d.rb_div != 0) + 1;
+  return (int)(d.rb_mod < s ? d.rb_mod : s);
 }
 
 static long long* g_gemm_trace = nullptr;
@@ -476,6 +568,10 @@ extern "C" int a3d_gemm(const a3d_gemm_args* a, void* stream) {
   d.a_mode = a->a_mode;
   d.bias = a->bias; d.rowbias = a->rowbias; d.rb_ld = a->rb_ld;
   d.rb_div = a->rb_div > 0 ? a->rb_div : 1; d.rb_mod = a->rb_mod > 0 ? a->rb_mod : (int64_t)1 << 40;
+  // rows m < M only: a divisor above M leaves every quotient 0, and a modulus above the largest quotient changes none, so
+  // both are clamped to M's range (the tensor-core kernel divides in 32 bits)
+  if (d.rb_div > d.M) d.rb_div = d.M;
+  if (d.rb_mod > (d.M - 1) / d.rb_div + 1) d.rb_mod = (d.M - 1) / d.rb_div + 1;
   d.acc_scale = a->acc_scale;   // the caller passes 1.0 when unused; 0 is a legitimate blend weight, not a sentinel
   d.R1 = reinterpret_cast<const __half*>(a->R1); d.ldr1 = a->ldr1; d.r1_scale = a->r1_scale;
   d.R2 = reinterpret_cast<const __half*>(a->R2); d.ldr2 = a->ldr2;
@@ -509,6 +605,9 @@ extern "C" int a3d_gemm(const a3d_gemm_args* a, void* stream) {
                ((reinterpret_cast<uintptr_t>(a->B) & 15) == 0) && (a->ldc % 16 == 0) &&
                ((reinterpret_cast<uintptr_t>(a->C) & 31) == 0);
   if (a->a_mode == A3D_A_PLAIN) tc_ok = tc_ok && (a->lda % 8 == 0) && a->lda >= a->K;
+  // the kernel's row and column indices (up to M + 127, N + 255) and the permutation period perm_a * perm_b are 32-bit
+  tc_ok = tc_ok && a->M <= INT32_MAX - kBM && a->N <= INT32_MAX - 256 &&
+          (a->perm_a == 0 || (a->perm_a <= INT32_MAX && a->perm_b <= INT32_MAX / a->perm_a));
   int boh = 0, bimg = 1, tpi = 0, tpr = 1;
   if (a->a_mode == A3D_A_CONV3) {
     tc_ok = tc_ok && (cv.c % kBK == 0);
@@ -559,6 +658,12 @@ extern "C" int a3d_gemm(const a3d_gemm_args* a, void* stream) {
     if (force < 0) { const char* e = getenv("A3D_GEMM_BN"); force = e ? atoi(e) : 0; }
     if (!geglu && (force == 128 || force == 160 || force == 256)) BN = force;   // tuning override
   }
+  d.rb_slots = gemm_rb_slots(d);
+  // a table with up to 64 distinct rows per warpgroup (CLIP's position embeddings) leaves room for fewer than two stages
+  // of the 256-column tile
+  if (BN == 256 && GemmCfg<256>::stages(d.rb_slots) < 2) BN = 128;
+  d.stages = BN == 256 ? GemmCfg<256>::stages(d.rb_slots) : BN == 160 ? GemmCfg<160>::stages(d.rb_slots)
+                                                                      : GemmCfg<128>::stages(d.rb_slots);
   if (geglu && a->N % BN) return fail(A3D_EINVAL, "a3d_gemm: GEGLU needs N %% 128 == 0");
   d.num_k_blocks = (int)(a->K / kBK);
   d.tiles_m = (int)((a->M + kBM - 1) / kBM);

@@ -20,6 +20,8 @@ elif which == "geglu":
     kb.gemm_case("l0 geglu 320->2560 (traced)", M0, 2560, 320, geglu=True)
 elif which == "sqkv":
     kb.gemm_case("l0 sqkv+rowbias (traced)", M0, 1152, 320, rowbias=True)
+elif which == "tqkv":
+    kb.gemm_case("l0 tqkv+rowbias (traced)", M0, 960, 320, rowbias=True, rb=(1, 16))
 else:
     kb.gemm_case("l0 proj+res (traced)", M0, 320, 320, res=True)
 lib.a3d_debug_set_gemm_trace(C.c_void_p(None))
