@@ -14,6 +14,8 @@
 // Replaces xformers.ops.memory_efficient_attention at animatediff/models/attention_processor.py:103,233,268,405,416,656,691.
 #include <stdlib.h>
 
+#include <type_traits>
+
 #include "a3d_common.cuh"
 #include "a3d_host.cuh"
 #include "a3d_wgmma.cuh"
@@ -54,6 +56,14 @@ struct AttnCfg {
   static constexpr int kMinBlocks = (kSmemBytes <= 113 * 1024) ? 2 : 1;
   static_assert(kSmemBytes <= 227 * 1024, "shared memory budget");
 };
+
+// f(integral_constant<I>), f(integral_constant<I + 1>), ... up to N - 1, while f returns true
+template <int I, int N, class F>
+__device__ __forceinline__ void static_for(F&& f) {
+  if constexpr (I < N) {
+    if (f(std::integral_constant<int, I>{})) static_for<I + 1, N>(f);
+  }
+}
 
 template <int N>
 __device__ __forceinline__ void wgmma_pv(float (&o)[N / 2], const uint32_t (&a)[4], uint64_t bdesc, uint32_t acc) {
@@ -145,6 +155,10 @@ attn_tc_kernel(const AttnDev p, const __grid_constant__ CUtensorMap mapQ, const 
   // -------------------------------------------------------------------- consumers: warpgroup wg owns query rows [64 wg, 64 wg + 64)
   // thread (warp w, lane 4 g + t) holds rows r_lo = 16 (w % 4) + g and r_hi = r_lo + 8 of its warpgroup; score / output
   // columns 8 jj + 2 t, +1 (the wgmma accumulator layout)
+  //
+  // The key loop runs S steps per trip, so the stage of each step is a compile-time constant: every shared-memory
+  // descriptor is a base descriptor plus a constant and every barrier address a constant offset.  Only the barrier phase
+  // parity flips, once per trip.
   const int wg = warp >> 2;
   const int g = lane >> 2, t = lane & 3;
   float s[32];
@@ -152,77 +166,91 @@ attn_tc_kernel(const AttnDev p, const __grid_constant__ CUtensorMap mapQ, const 
 #pragma unroll
   for (int i = 0; i < Cfg::kDv / 2; ++i) o[i] = 0.f;
   float m_lo = -INFINITY, m_hi = -INFINITY;
-  const uint32_t q0 = smem_u32(sQ + wg * (64 * 128));
+  const uint64_t qdesc = make_smem_desc_sw128(smem_u32(sQ + wg * (64 * 128)), 16, 1024);
+  const uint64_t kdesc = make_smem_desc_sw128(smem_u32(sK), 16, 1024);
+  // V is MN-major: 16 keys = two 8-row swizzle atoms (SBO = 1024 B); the next 64 value columns live one TMA box further
+  const uint64_t vdesc = make_smem_desc_sw128(smem_u32(sV), Cfg::kKVBox, 1024);
+  // key columns at or past `valid` hold zero fill or the next tile's rows and are masked to -inf: in the last tile, and in
+  // every tile when a TMA box holds fewer than 64 keys
+  const int mask_from = rows_tile < 64 ? 0 : n - 1;
+  uint32_t ph = 0;   // barrier phase of this trip's stages
   mbar_wait(q_full, 0);
-  for (int j = 0; j < n; ++j) {
-    const int st = j % S;
-    const uint32_t ph = (j / S) & 1;
-    // ---- S = Q K^T
-    mbar_wait(&k_full[st], ph);
-    wgmma_fence();
+  for (int j0 = 0; j0 < n; j0 += S) {
+    static_for<0, S>([&](auto stc) {
+      constexpr int st = decltype(stc)::value;
+      const int j = j0 + st;
+      if (j >= n) return false;
+      // ---- S = Q K^T
+      mbar_wait(&k_full[st], ph);
+      wgmma_fence();
 #pragma unroll
-    for (int kk = 0; kk < Cfg::kDqk / 16; ++kk) {
-      const uint64_t qd = make_smem_desc_sw128(q0 + (kk / 4) * Cfg::kQBox + (kk % 4) * 32, 16, 1024);
-      const uint64_t kd = make_smem_desc_sw128(smem_u32(sK + (st * Cfg::kQB + kk / 4) * Cfg::kKVBox) + (kk % 4) * 32, 16, 1024);
-      wgmma_ss_n64<0>(s, qd, kd, kk ? 1u : 0u);
-    }
-    wgmma_commit();
-    wgmma_wait<0>();
-    reg_fence(s);
-    // ---- row maxima over the valid keys (a quad of lanes shares a row)
-    const int valid = (j == n - 1) ? p.rows_k : rows_tile;
-    float mx_lo = -INFINITY, mx_hi = -INFINITY;
+      for (int kk = 0; kk < Cfg::kDqk / 16; ++kk)
+        wgmma_ss_n64<0>(s, desc_add(qdesc, (kk / 4) * Cfg::kQBox + (kk % 4) * 32),
+                        desc_add(kdesc, (st * Cfg::kQB + kk / 4) * Cfg::kKVBox + (kk % 4) * 32), kk ? 1u : 0u);
+      wgmma_commit();
+      wgmma_wait<0>();
+      reg_fence(s);
+      // ---- row maxima over the valid keys (a quad of lanes shares a row)
+      if (j >= mask_from) {
+        const int valid = (j == n - 1) ? p.rows_k : rows_tile;
 #pragma unroll
-    for (int jj = 0; jj < 8; ++jj) {
+        for (int jj = 0; jj < 8; ++jj) {
 #pragma unroll
-      for (int e = 0; e < 2; ++e) {
-        if (8 * jj + 2 * t + e >= valid) { s[4 * jj + e] = -INFINITY; s[4 * jj + 2 + e] = -INFINITY; }
-        mx_lo = fmaxf(mx_lo, s[4 * jj + e]);
-        mx_hi = fmaxf(mx_hi, s[4 * jj + 2 + e]);
+          for (int e = 0; e < 2; ++e)
+            if (8 * jj + 2 * t + e >= valid) { s[4 * jj + e] = -INFINITY; s[4 * jj + 2 + e] = -INFINITY; }
+        }
       }
-    }
+      float mx_lo = -INFINITY, mx_hi = -INFINITY;
 #pragma unroll
-    for (int x = 1; x <= 2; x <<= 1) {
-      mx_lo = fmaxf(mx_lo, __shfl_xor_sync(0xffffffffu, mx_lo, x));
-      mx_hi = fmaxf(mx_hi, __shfl_xor_sync(0xffffffffu, mx_hi, x));
-    }
-    const float mn_lo = fmaxf(m_lo, mx_lo * p.scale_log2), mn_hi = fmaxf(m_hi, mx_hi * p.scale_log2);
-    if (j == 0) {
-      m_lo = mn_lo; m_hi = mn_hi;
-    } else if (__any_sync(0xffffffffu, mn_lo - m_lo > kRescaleLog2 || mn_hi - m_hi > kRescaleLog2)) {
-      if (p.dbg && lane == 0) atomicAdd(p.dbg, 1ull);
-      const float a_lo = ex2_approx(m_lo - mn_lo), a_hi = ex2_approx(m_hi - mn_hi);
+      for (int jj = 0; jj < 8; ++jj) {
 #pragma unroll
-      for (int c = 0; c < Cfg::kDv / 8; ++c) {
-        o[4 * c] *= a_lo; o[4 * c + 1] *= a_lo; o[4 * c + 2] *= a_hi; o[4 * c + 3] *= a_hi;
+        for (int e = 0; e < 2; ++e) {
+          mx_lo = fmaxf(mx_lo, s[4 * jj + e]);
+          mx_hi = fmaxf(mx_hi, s[4 * jj + 2 + e]);
+        }
       }
-      m_lo = mn_lo; m_hi = mn_hi;
-    }
-    // ---- P = exp2(s * scale_log2 - m) -> fp16 A fragments of the four 16-key k-steps
-    uint32_t pa[4][4];
 #pragma unroll
-    for (int kk = 0; kk < 4; ++kk) {
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const float* sb = s + 4 * (2 * kk + h);
-        pa[kk][2 * h] = pack_f16x2(ex2_approx(fmaf(sb[0], p.scale_log2, -m_lo)), ex2_approx(fmaf(sb[1], p.scale_log2, -m_lo)));
-        pa[kk][2 * h + 1] = pack_f16x2(ex2_approx(fmaf(sb[2], p.scale_log2, -m_hi)), ex2_approx(fmaf(sb[3], p.scale_log2, -m_hi)));
+      for (int x = 1; x <= 2; x <<= 1) {
+        mx_lo = fmaxf(mx_lo, __shfl_xor_sync(0xffffffffu, mx_lo, x));
+        mx_hi = fmaxf(mx_hi, __shfl_xor_sync(0xffffffffu, mx_hi, x));
       }
-    }
-    // ---- O += P V
-    mbar_wait(&v_full[st], ph);
-    wgmma_fence();
+      const float mn_lo = fmaxf(m_lo, mx_lo * p.scale_log2), mn_hi = fmaxf(m_hi, mx_hi * p.scale_log2);
+      if (st == 0 && j == 0) {
+        m_lo = mn_lo; m_hi = mn_hi;
+      } else if (__any_sync(0xffffffffu, mn_lo - m_lo > kRescaleLog2 || mn_hi - m_hi > kRescaleLog2)) {
+        if (p.dbg && lane == 0) atomicAdd(p.dbg, 1ull);
+        const float a_lo = ex2_approx(m_lo - mn_lo), a_hi = ex2_approx(m_hi - mn_hi);
 #pragma unroll
-    for (int kk = 0; kk < 4; ++kk) {
-      // V is MN-major: 16 keys = two 8-row swizzle atoms (SBO = 1024 B); the next 64 value columns live one TMA box further
-      const uint64_t vd = make_smem_desc_sw128(smem_u32(sV + st * Cfg::kVB * Cfg::kKVBox) + kk * 2048, Cfg::kKVBox, 1024);
-      wgmma_pv<Cfg::kDv>(o, pa[kk], vd, 1u);
-    }
-    wgmma_commit();
-    wgmma_wait<0>();
-    reg_fence(o);
-    __syncwarp();
-    if (lane == 0) mbar_arrive(&kv_empty[st]);
+        for (int c = 0; c < Cfg::kDv / 8; ++c) {
+          o[4 * c] *= a_lo; o[4 * c + 1] *= a_lo; o[4 * c + 2] *= a_hi; o[4 * c + 3] *= a_hi;
+        }
+        m_lo = mn_lo; m_hi = mn_hi;
+      }
+      // ---- P = exp2(s * scale_log2 - m) -> fp16 A fragments of the four 16-key k-steps
+      uint32_t pa[4][4];
+#pragma unroll
+      for (int kk = 0; kk < 4; ++kk) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const float* sb = s + 4 * (2 * kk + h);
+          pa[kk][2 * h] = pack_f16x2(ex2_approx(fmaf(sb[0], p.scale_log2, -m_lo)), ex2_approx(fmaf(sb[1], p.scale_log2, -m_lo)));
+          pa[kk][2 * h + 1] = pack_f16x2(ex2_approx(fmaf(sb[2], p.scale_log2, -m_hi)), ex2_approx(fmaf(sb[3], p.scale_log2, -m_hi)));
+        }
+      }
+      // ---- O += P V
+      mbar_wait(&v_full[st], ph);
+      wgmma_fence();
+#pragma unroll
+      for (int kk = 0; kk < 4; ++kk)
+        wgmma_pv<Cfg::kDv>(o, pa[kk], desc_add(vdesc, st * Cfg::kVB * Cfg::kKVBox + kk * 2048), 1u);
+      wgmma_commit();
+      wgmma_wait<0>();
+      reg_fence(o);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&kv_empty[st]);
+      return true;
+    });
+    ph ^= 1;
   }
   // ---- epilogue: O / O[:, D] -> fp16 -> global (through the query view geometry); column D sits in lane t = 0 of the quad
   const float l_lo = __shfl_sync(0xffffffffu, o[4 * (D / 8)], lane & ~3);

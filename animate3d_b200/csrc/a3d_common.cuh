@@ -117,6 +117,11 @@ __device__ __forceinline__ uint64_t make_smem_desc_sw128(uint32_t smem_addr, uin
   d |= (uint64_t)1 << 62;  // layout_type = SWIZZLE_128B
   return d;
 }
+// The same descriptor moved `bytes` (a multiple of 16) further into shared memory: the start-address field is the low
+// 14 bits and shared addresses stay below 2^18, so the add never carries out of the field or the low word.
+__device__ __forceinline__ uint64_t desc_add(uint64_t desc, uint32_t bytes) {
+  return (desc & 0xFFFFFFFF00000000ull) | (uint32_t)((uint32_t)desc + (bytes >> 4));
+}
 
 // warp-level MMA (fp16 x fp16 -> fp32), used where a problem is far below a 64-row warpgroup tile (16-frame temporal
 // attention, 77-key text cross-attention)
