@@ -276,57 +276,13 @@ attn_tc_kernel(const AttnDev p, const __grid_constant__ CUtensorMap mapQ, const 
   }
 }
 
-// ---------------------------------------------------------------------------------------------------------------
-// SIMT bring-up / reference kernel (one thread per (batch, head, query)); same view semantics, fp32 math
-// ---------------------------------------------------------------------------------------------------------------
+// A strided view as the thread-per-(row, head) kernels read it: element (col, i1, i2, i3, i4) at
+// base + col + i1*s1 + i2*s2 + i3*s3 + i4*s4 (a3d_view5 without the column extent)
 struct ViewDev {
   const __half* base;
   int64_t s1, s2, s3, s4;
   int e1, e2, e3, e4;
 };
-
-__global__ void attn_simt_kernel(ViewDev q, ViewDev k, ViewDev v, __half* out, int64_t os1, int64_t os2, int64_t os3,
-                                 int64_t os4, int heads, int d, int dqk, int dv, float scale, int kv_div, int kv_i3_zero,
-                                 int accumulate, float out_scale) {
-  const int Lq = q.e1 * q.e2, Lk = k.e1 * k.e2;
-  const int64_t total = (int64_t)q.e3 * q.e4 * heads * Lq;
-  const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (idx >= total) return;
-  const int l = (int)(idx % Lq);
-  const int h = (int)((idx / Lq) % heads);
-  const int qb = (int)(idx / ((int64_t)Lq * heads));
-  const int kb = qb / kv_div;
-  const __half* qp = q.base + (int64_t)(l % q.e1) * q.s1 + (int64_t)(l / q.e1) * q.s2 + (int64_t)(qb % q.e3) * q.s3 +
-                     (int64_t)(qb / q.e3) * q.s4 + h * dqk;
-  const int64_t koff = (int64_t)(kv_i3_zero ? 0 : kb % k.e3) * k.s3 + (int64_t)(kb / k.e3) * k.s4;
-  const int64_t voff = (int64_t)(kv_i3_zero ? 0 : kb % v.e3) * v.s3 + (int64_t)(kb / v.e3) * v.s4;
-  float m = -INFINITY;
-  for (int j = 0; j < Lk; ++j) {
-    const __half* kp = k.base + koff + (int64_t)(j % k.e1) * k.s1 + (int64_t)(j / k.e1) * k.s2 + h * dqk;
-    float s = 0.f;
-    for (int c = 0; c < d; ++c) s += __half2float(qp[c]) * __half2float(kp[c]);
-    m = fmaxf(m, s * scale);
-  }
-  float acc[160];
-  for (int c = 0; c < d; ++c) acc[c] = 0.f;
-  float sum = 0.f;
-  for (int j = 0; j < Lk; ++j) {
-    const __half* kp = k.base + koff + (int64_t)(j % k.e1) * k.s1 + (int64_t)(j / k.e1) * k.s2 + h * dqk;
-    const __half* vp = v.base + voff + (int64_t)(j % v.e1) * v.s1 + (int64_t)(j / v.e1) * v.s2 + h * dv;
-    float s = 0.f;
-    for (int c = 0; c < d; ++c) s += __half2float(qp[c]) * __half2float(kp[c]);
-    const float pj = expf(s * scale - m);
-    sum += pj;
-    for (int c = 0; c < d; ++c) acc[c] += pj * __half2float(vp[c]);
-  }
-  __half* op = out + (int64_t)(l % q.e1) * os1 + (int64_t)(l / q.e1) * os2 + (int64_t)(qb % q.e3) * os3 +
-               (int64_t)(qb / q.e3) * os4 + h * d;
-  for (int c = 0; c < d; ++c) {
-    float o = out_scale * acc[c] / sum;
-    if (accumulate) o += __half2float(op[c]);
-    op[c] = __float2half_rn(o);
-  }
-}
 
 // ---------------------------------------------------------------------------------------------------------------
 // Few-keys attention (IP-adapter image tokens: 4 keys per image group).  The tensor path would spend a whole CTA
@@ -573,27 +529,8 @@ attn_shortkeys_kernel(ViewDev q, ViewDev k, ViewDev v, __half* out, int64_t os1,
   }
 }
 
-template <int D>
-static int launch_shortkeys(const a3d_attn_args* a, int dqk, int dv, int kv_div, int batches, cudaStream_t st) {
-  using Cfg = ShortCfg<D>;
-  ViewDev q{reinterpret_cast<const __half*>(a->q.base), a->q.s1, a->q.s2, a->q.s3, a->q.s4, a->q.e1, a->q.e2, a->q.e3, a->q.e4};
-  ViewDev k{reinterpret_cast<const __half*>(a->k.base), a->k.s1, a->k.s2, a->k.s3, a->k.s4, a->k.e1, a->k.e2, a->k.e3, a->k.e4};
-  ViewDev v{reinterpret_cast<const __half*>(a->v.base), a->v.s1, a->v.s2, a->v.s3, a->v.s4, a->v.e1, a->v.e2, a->v.e3, a->v.e4};
-  static bool attr_set = false;
-  if (!attr_set && Cfg::kSmem > 48 * 1024) {
-    A3D_CUDA_CHECK(cudaFuncSetAttribute(attn_shortkeys_kernel<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmem));
-    attr_set = true;
-  }
-  const int Lq = a->q.e1 * a->q.e2;
-  int rows_per_block = 256;                       // 4 x 64-row rounds per block amortise the K/V staging
-  while (rows_per_block > 64 && (int64_t)((Lq + rows_per_block - 1) / rows_per_block) * a->heads * batches < 8 * sm_count())
-    rows_per_block /= 2;
-  dim3 grid((unsigned)((Lq + rows_per_block - 1) / rows_per_block), (unsigned)a->heads, (unsigned)batches);
-  attn_shortkeys_kernel<D><<<grid, 128, Cfg::kSmem, st>>>(q, k, v, reinterpret_cast<__half*>(a->out), a->os1, a->os2, a->os3, a->os4,
-                                                          dqk, dv, a->scale * 1.4426950408889634f, kv_div, a->kv_i3_zero,
-                                                          a->accumulate, a->out_scale, rows_per_block);
-  A3D_LAUNCH_CHECK();
-  return A3D_OK;
+static ViewDev view_dev(const a3d_view5& v) {
+  return ViewDev{reinterpret_cast<const __half*>(v.base), v.s1, v.s2, v.s3, v.s4, v.e1, v.e2, v.e3, v.e4};
 }
 
 static int tile_geom(const a3d_view5& v, int* box1, int* box2, int* t1, int* tiles, int* rows) {
@@ -634,85 +571,45 @@ static int tile_geom_k64(const a3d_view5& v, int* box1, int* box2, int* t1, int*
   return 0;
 }
 
-template <int D>
-static int launch_attn(AttnDev dev, const a3d_attn_args* a, const CUtensorMap* mq, dim3 grid, cudaStream_t st) {
-  using Cfg = AttnCfg<D>;
-  int kb1, kb2, kt1, ktiles, klast;
-  if (int r = tile_geom_k64(a->k, &kb1, &kb2, &kt1, &ktiles, &klast)) return r;
-  dev.kv_tiles = ktiles; dev.rows_k = klast; dev.k_t1 = kt1; dev.k_box1 = kb1; dev.k_box2 = kb2;
-  dev.k_box_bytes = 128u * (uint32_t)(kb1 * kb2);
-  const CUtensorMap *mk, *mv;
-  if (int r = view_map(a->k, kb1, kb2, &mk)) return r;
-  if (int r = view_map(a->v, kb1, kb2, &mv)) return r;
-  static bool attr_set = false;
-  if (!attr_set) {
-    A3D_CUDA_CHECK(cudaFuncSetAttribute(attn_tc_kernel<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
-    attr_set = true;
-  }
-  attn_tc_kernel<D><<<grid, kAttnThreads, Cfg::kSmemBytes, st>>>(dev, *mq, *mk, *mv);
-  A3D_LAUNCH_CHECK();
-  return A3D_OK;
-}
+enum { kAttnFewKeys = 0, kAttnShortKeys = 1, kAttnTc = 2 };
+static const char* const kAttnNames[] = {"fewkeys", "shortkeys", "tc"};   // indexed by kAttn*
 
-static unsigned long long* g_attn_dbg = nullptr;
+// What one a3d_attention call launches, decided from its arguments alone: a3d_attention launches exactly this, and
+// a3d_attention_kernel names it.
+struct AttnPlan {
+  int kernel;                         // kAttn*
+  int dqk, dv, kv_div, batches;
+  int qb1, qb2, qt1, qtiles, qrows;   // tensor-core kernel: 128-row query tiles (tile_geom)
+  int kb1, kb2, kt1, ktiles, klast;   // ... and 64-row key tiles (tile_geom_k64)
+};
 
-}  // namespace a3d
-
-extern "C" int a3d_attention(const a3d_attn_args* a, void* stream) {
-  using namespace a3d;
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+static int plan_attention(const a3d_attn_args* a, AttnPlan* p) {
   if (!a || !a->q.base || !a->k.base || !a->v.base || !a->out) return fail(A3D_EINVAL, "a3d_attention: null operand");
   const int d = a->d;
   if (d != 40 && d != 80 && d != 160) return fail(A3D_EINVAL, "a3d_attention: head dim %d not in {40,80,160}", d);
   if (a->k.e1 != a->v.e1 || a->k.e2 != a->v.e2 || a->k.e3 != a->v.e3 || a->k.e4 != a->v.e4)
     return fail(A3D_EINVAL, "a3d_attention: K and V extents differ");
-  const int dqk = (d + 15) / 16 * 16, dv = (d + 1 + 15) / 16 * 16;
-  const int kv_div = a->kv_div > 0 ? a->kv_div : 1;
-  const int batches = a->q.e3 * a->q.e4;
-  if ((batches + kv_div - 1) / kv_div > a->k.e3 * a->k.e4 && !a->kv_i3_zero)
+  memset(p, 0, sizeof(*p));
+  p->dqk = (d + 15) / 16 * 16;
+  p->dv = (d + 1 + 15) / 16 * 16;
+  p->kv_div = a->kv_div > 0 ? a->kv_div : 1;
+  const int batches = p->batches = a->q.e3 * a->q.e4;
+  if ((batches + p->kv_div - 1) / p->kv_div > a->k.e3 * a->k.e4 && !a->kv_i3_zero)
     return fail(A3D_EINVAL, "a3d_attention: key batches (%d) do not cover query batches (%d / %d)", a->k.e3 * a->k.e4,
-                batches, kv_div);
-
-  if (a->impl == A3D_GEMM_SIMT) {
-    ViewDev q{reinterpret_cast<const __half*>(a->q.base), a->q.s1, a->q.s2, a->q.s3, a->q.s4, a->q.e1, a->q.e2, a->q.e3, a->q.e4};
-    ViewDev k{reinterpret_cast<const __half*>(a->k.base), a->k.s1, a->k.s2, a->k.s3, a->k.s4, a->k.e1, a->k.e2, a->k.e3, a->k.e4};
-    ViewDev v{reinterpret_cast<const __half*>(a->v.base), a->v.s1, a->v.s2, a->v.s3, a->v.s4, a->v.e1, a->v.e2, a->v.e3, a->v.e4};
-    const int64_t total = (int64_t)batches * a->heads * a->q.e1 * a->q.e2;
-    attn_simt_kernel<<<(unsigned)((total + 63) / 64), 64, 0, st>>>(q, k, v, reinterpret_cast<__half*>(a->out), a->os1, a->os2,
-                                                                  a->os3, a->os4, a->heads, d, dqk, dv, a->scale, kv_div,
-                                                                  a->kv_i3_zero, a->accumulate,
-                                                                  a->out_scale);
-    A3D_LAUNCH_CHECK();
-    return A3D_OK;
-  }
-
+                batches, p->kv_div);
+  // AUTO picks the kernel by key count; A3D_GEMM_TC forces the tensor-core kernel (tests use it to keep its ragged-key paths
+  // covered)
+  if (a->impl != A3D_GEMM_AUTO && a->impl != A3D_GEMM_TC)
+    return fail(A3D_EINVAL, "a3d_attention: impl %d is not A3D_GEMM_AUTO or A3D_GEMM_TC", a->impl);
   if ((a->os1 | a->os2 | a->os3 | a->os4) % 8 || (reinterpret_cast<uintptr_t>(a->out) & 15))
     return fail(A3D_EINVAL, "a3d_attention: output rows must be 16-byte aligned");
-  // impl == AUTO picks the kernel by key count; an explicit A3D_GEMM_TCGEN05 forces the tensor-core kernel (tests use it to
-  // keep its ragged-key paths covered)
   const bool auto_impl = a->impl == A3D_GEMM_AUTO;
   if (auto_impl && a->k.e1 * a->k.e2 <= kFewKeysMax) {
     // a handful of keys (IP-adapter image tokens): HBM-bound thread-per-(row, head) kernel, see attn_fewkeys_kernel
     if ((a->q.s1 | a->q.s2 | a->q.s3 | a->q.s4 | a->k.s1 | a->k.s2 | a->k.s3 | a->k.s4 | a->v.s1 | a->v.s2 | a->v.s3 | a->v.s4) % 8 ||
         ((reinterpret_cast<uintptr_t>(a->q.base) | reinterpret_cast<uintptr_t>(a->k.base) | reinterpret_cast<uintptr_t>(a->v.base)) & 15))
       return fail(A3D_EINVAL, "a3d_attention: operand rows must be 16-byte aligned");
-    ViewDev q{reinterpret_cast<const __half*>(a->q.base), a->q.s1, a->q.s2, a->q.s3, a->q.s4, a->q.e1, a->q.e2, a->q.e3, a->q.e4};
-    ViewDev k{reinterpret_cast<const __half*>(a->k.base), a->k.s1, a->k.s2, a->k.s3, a->k.s4, a->k.e1, a->k.e2, a->k.e3, a->k.e4};
-    ViewDev v{reinterpret_cast<const __half*>(a->v.base), a->v.s1, a->v.s2, a->v.s3, a->v.s4, a->v.e1, a->v.e2, a->v.e3, a->v.e4};
-    const int64_t total = (int64_t)batches * a->heads * a->q.e1 * a->q.e2;
-    const unsigned blocks = (unsigned)((total + 255) / 256);
-    const float sl2 = a->scale * 1.4426950408889634f, osc = a->out_scale;
-    __half* o = reinterpret_cast<__half*>(a->out);
-    if (d == 40)
-      attn_fewkeys_kernel<40><<<blocks, 256, 0, st>>>(q, k, v, o, a->os1, a->os2, a->os3, a->os4, a->heads, dqk, dv, sl2, kv_div,
-                                                      a->kv_i3_zero, a->accumulate, osc);
-    else if (d == 80)
-      attn_fewkeys_kernel<80><<<blocks, 256, 0, st>>>(q, k, v, o, a->os1, a->os2, a->os3, a->os4, a->heads, dqk, dv, sl2, kv_div,
-                                                      a->kv_i3_zero, a->accumulate, osc);
-    else
-      attn_fewkeys_kernel<160><<<blocks, 256, 0, st>>>(q, k, v, o, a->os1, a->os2, a->os3, a->os4, a->heads, dqk, dv, sl2, kv_div,
-                                                       a->kv_i3_zero, a->accumulate, osc);
-    A3D_LAUNCH_CHECK();
+    p->kernel = kAttnFewKeys;
     return A3D_OK;
   }
   if (auto_impl && a->k.e1 * a->k.e2 <= kShortKeysPad && (a->os1 | a->os2) % 2 == 0 &&
@@ -721,37 +618,108 @@ extern "C" int a3d_attention(const a3d_attn_args* a, void* stream) {
       ((reinterpret_cast<uintptr_t>(a->k.base) | reinterpret_cast<uintptr_t>(a->v.base)) & 15) == 0 &&
       (reinterpret_cast<uintptr_t>(a->q.base) & 3) == 0 && batches <= 65535) {
     // 9..80 keys (text cross-attention): warp-level MMA kernel with the keys resident in shared memory
-    switch (d) {
-      case 40: return launch_shortkeys<40>(a, dqk, dv, kv_div, batches, st);
-      case 80: return launch_shortkeys<80>(a, dqk, dv, kv_div, batches, st);
-      default: return launch_shortkeys<160>(a, dqk, dv, kv_div, batches, st);
-    }
+    p->kernel = kAttnShortKeys;
+    return A3D_OK;
   }
+  p->kernel = kAttnTc;
+  if (int r = tile_geom(a->q, &p->qb1, &p->qb2, &p->qt1, &p->qtiles, &p->qrows)) return r;
+  if (batches > 65535 || a->heads > 65535) return fail(A3D_EINVAL, "a3d_attention: grid too large");
+  return tile_geom_k64(a->k, &p->kb1, &p->kb2, &p->kt1, &p->ktiles, &p->klast);
+}
 
+template <int D>
+static int launch_fewkeys(const a3d_attn_args* a, const AttnPlan& p, cudaStream_t st) {
+  const int64_t total = (int64_t)p.batches * a->heads * a->q.e1 * a->q.e2;
+  attn_fewkeys_kernel<D><<<(unsigned)((total + 255) / 256), 256, 0, st>>>(
+      view_dev(a->q), view_dev(a->k), view_dev(a->v), reinterpret_cast<__half*>(a->out), a->os1, a->os2, a->os3, a->os4,
+      a->heads, p.dqk, p.dv, a->scale * 1.4426950408889634f, p.kv_div, a->kv_i3_zero, a->accumulate, a->out_scale);
+  A3D_LAUNCH_CHECK();
+  return A3D_OK;
+}
+
+template <int D>
+static int launch_shortkeys(const a3d_attn_args* a, const AttnPlan& p, cudaStream_t st) {
+  using Cfg = ShortCfg<D>;
+  static bool attr_set = false;
+  if (!attr_set && Cfg::kSmem > 48 * 1024) {
+    A3D_CUDA_CHECK(cudaFuncSetAttribute(attn_shortkeys_kernel<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmem));
+    attr_set = true;
+  }
+  const int Lq = a->q.e1 * a->q.e2;
+  int rows_per_block = 256;                       // 4 x 64-row rounds per block amortise the K/V staging
+  while (rows_per_block > 64 && (int64_t)((Lq + rows_per_block - 1) / rows_per_block) * a->heads * p.batches < 8 * sm_count())
+    rows_per_block /= 2;
+  dim3 grid((unsigned)((Lq + rows_per_block - 1) / rows_per_block), (unsigned)a->heads, (unsigned)p.batches);
+  attn_shortkeys_kernel<D><<<grid, 128, Cfg::kSmem, st>>>(view_dev(a->q), view_dev(a->k), view_dev(a->v),
+                                                          reinterpret_cast<__half*>(a->out), a->os1, a->os2, a->os3, a->os4,
+                                                          p.dqk, p.dv, a->scale * 1.4426950408889634f, p.kv_div, a->kv_i3_zero,
+                                                          a->accumulate, a->out_scale, rows_per_block);
+  A3D_LAUNCH_CHECK();
+  return A3D_OK;
+}
+
+static unsigned long long* g_attn_dbg = nullptr;
+
+template <int D>
+static int launch_attn(const a3d_attn_args* a, const AttnPlan& p, cudaStream_t st) {
+  using Cfg = AttnCfg<D>;
   AttnDev dev;
   memset(&dev, 0, sizeof(dev));
-  int qb1, qb2, qt1, qtiles, qrows;
-  if (int r = tile_geom(a->q, &qb1, &qb2, &qt1, &qtiles, &qrows)) return r;
-  dev.q_tiles = qtiles; dev.rows_q = qrows;
+  dev.q_tiles = p.qtiles; dev.rows_q = p.qrows;
+  dev.kv_tiles = p.ktiles; dev.rows_k = p.klast;
   dev.heads = a->heads;
-  dev.q_t1 = qt1; dev.q_box1 = qb1; dev.q_box2 = qb2; dev.q_e1 = a->q.e1; dev.q_e3 = a->q.e3;
-  dev.k_e3 = a->k.e3;
-  dev.kv_div = kv_div; dev.kv_i3_zero = a->kv_i3_zero;
-  dev.q_box_bytes = 128u * qrows;
+  dev.q_t1 = p.qt1; dev.q_box1 = p.qb1; dev.q_box2 = p.qb2; dev.q_e1 = a->q.e1; dev.q_e3 = a->q.e3;
+  dev.k_t1 = p.kt1; dev.k_box1 = p.kb1; dev.k_box2 = p.kb2; dev.k_e3 = a->k.e3;
+  dev.kv_div = p.kv_div; dev.kv_i3_zero = a->kv_i3_zero;
+  dev.q_box_bytes = 128u * p.qrows;
+  dev.k_box_bytes = 128u * (uint32_t)(p.kb1 * p.kb2);
   dev.scale_log2 = a->scale * 1.4426950408889634f;
   dev.out = reinterpret_cast<__half*>(a->out);
   dev.os1 = a->os1; dev.os2 = a->os2; dev.os3 = a->os3; dev.os4 = a->os4;
   dev.accumulate = a->accumulate;
   dev.out_scale = a->out_scale;
   dev.dbg = g_attn_dbg;
-  const CUtensorMap* mq;
-  if (int r = view_map(a->q, qb1, qb2, &mq)) return r;
-  dim3 grid(qtiles, a->heads, batches);
-  if (batches > 65535 || a->heads > 65535) return fail(A3D_EINVAL, "a3d_attention: grid too large");
-  switch (d) {
-    case 40: return launch_attn<40>(dev, a, mq, grid, st);
-    case 80: return launch_attn<80>(dev, a, mq, grid, st);
-    default: return launch_attn<160>(dev, a, mq, grid, st);
+  const CUtensorMap *mq, *mk, *mv;
+  if (int r = view_map(a->q, p.qb1, p.qb2, &mq)) return r;
+  if (int r = view_map(a->k, p.kb1, p.kb2, &mk)) return r;
+  if (int r = view_map(a->v, p.kb1, p.kb2, &mv)) return r;
+  static bool attr_set = false;
+  if (!attr_set) {
+    A3D_CUDA_CHECK(cudaFuncSetAttribute(attn_tc_kernel<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
+    attr_set = true;
+  }
+  attn_tc_kernel<D><<<dim3(p.qtiles, a->heads, p.batches), kAttnThreads, Cfg::kSmemBytes, st>>>(dev, *mq, *mk, *mv);
+  A3D_LAUNCH_CHECK();
+  return A3D_OK;
+}
+
+template <int D>
+static int launch_planned(const a3d_attn_args* a, const AttnPlan& p, cudaStream_t st) {
+  switch (p.kernel) {
+    case kAttnFewKeys: return launch_fewkeys<D>(a, p, st);
+    case kAttnShortKeys: return launch_shortkeys<D>(a, p, st);
+    default: return launch_attn<D>(a, p, st);
+  }
+}
+
+}  // namespace a3d
+
+extern "C" int a3d_attention_kernel(const a3d_attn_args* a, char* name, size_t n) {
+  using namespace a3d;
+  AttnPlan p;
+  if (int r = plan_attention(a, &p)) return r;
+  return kernel_name(name, n, "%s", kAttnNames[p.kernel]);
+}
+
+extern "C" int a3d_attention(const a3d_attn_args* a, void* stream) {
+  using namespace a3d;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  AttnPlan p;
+  if (int r = plan_attention(a, &p)) return r;
+  switch (a->d) {
+    case 40: return launch_planned<40>(a, p, st);
+    case 80: return launch_planned<80>(a, p, st);
+    default: return launch_planned<160>(a, p, st);
   }
 }
 

@@ -509,61 +509,43 @@ __global__ void gemm_simt_kernel(const GemmDev p, const __half* __restrict__ A, 
   else reinterpret_cast<__half*>(p.C)[orow * p.ldc + j] = __float2half_rn(v);
 }
 
-template <int BN, int EPI>
-static int launch_tc_epi(const GemmDev& dev, const CUtensorMap* mapA, const CUtensorMap* mapB, cudaStream_t st) {
-  static bool attr_set = false;
-  if (!attr_set) {
-    A3D_CUDA_CHECK(cudaFuncSetAttribute(gemm_tc_kernel<BN, EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, kGemmSmemMax));
-    attr_set = true;
-  }
-  const int smem = GemmCfg<BN>::smem_bytes(dev.stages, dev.rb_slots);
-  if (dev.stages < 2 || smem > kGemmSmemMax)
-    return fail(A3D_EINVAL, "a3d_gemm: %d row-bias rows per warpgroup leave no room for the operand ring", dev.rb_slots);
-  const int tiles = dev.tiles_m * dev.tiles_n;
-  const int grid = tiles < sm_count() ? tiles : sm_count();
-  gemm_tc_kernel<BN, EPI><<<grid, kGemmThreads, smem, st>>>(dev, *mapA, *mapB);
-  A3D_LAUNCH_CHECK();
-  return A3D_OK;
-}
-
-template <int BN>
-static int launch_tc(const GemmDev& dev, const CUtensorMap* mapA, const CUtensorMap* mapB, cudaStream_t st) {
-  if (dev.out_f32) return launch_tc_epi<BN, kEpiF32>(dev, mapA, mapB, st);
-  if (dev.geglu == 1) {
-    if constexpr (BN % 64 == 0) return launch_tc_epi<BN, kEpiGeglu>(dev, mapA, mapB, st);
-    else return fail(A3D_EINVAL, "a3d_gemm: GEGLU needs a 128- or 256-column tile");
-  }
-  if (dev.geglu == 2) return launch_tc_epi<BN, kEpiGelu>(dev, mapA, mapB, st);
-  if (dev.R1 || dev.R2 || dev.perm_a) return launch_tc_epi<BN, kEpiRes>(dev, mapA, mapB, st);
-  return launch_tc_epi<BN, kEpiPlain>(dev, mapA, mapB, st);
-}
-
 // Row-bias rows the 64 rows of one warpgroup use: their quotients m / rb_div span at most ceil(63 / rb_div) + 1 values,
-// and at most rb_mod of them are distinct table rows (rb_mod is at most the number of quotients of all M rows, see a3d_gemm).
+// and at most rb_mod of them are distinct table rows (rb_mod is at most the number of quotients of all M rows, see plan_gemm).
 static int gemm_rb_slots(const GemmDev& d) {
   if (!d.rowbias) return 0;
   const int64_t s = 63 / d.rb_div + (63 % d.rb_div != 0) + 1;
   return (int)(d.rb_mod < s ? d.rb_mod : s);
 }
 
-static long long* g_gemm_trace = nullptr;
-
-}  // namespace a3d
-
-// debug hook (not part of the product path): per-tile clock64 timestamps of CTA 0 of the following tensor-core GEMM launches
-extern "C" int a3d_debug_set_gemm_trace(void* device_buffer_1024_int64) {
-  a3d::g_gemm_trace = reinterpret_cast<long long*>(device_buffer_1024_int64);
-  return A3D_OK;
+// GemmCfg<BN> at a run-time tile width
+static int gemm_stages(int bn, int rb_slots) {
+  return bn == 256 ? GemmCfg<256>::stages(rb_slots) : bn == 160 ? GemmCfg<160>::stages(rb_slots) : GemmCfg<128>::stages(rb_slots);
+}
+static int gemm_smem_bytes(int bn, int stages, int rb_slots) {
+  return bn == 256   ? GemmCfg<256>::smem_bytes(stages, rb_slots)
+         : bn == 160 ? GemmCfg<160>::smem_bytes(stages, rb_slots)
+                     : GemmCfg<128>::smem_bytes(stages, rb_slots);
 }
 
-extern "C" int a3d_gemm(const a3d_gemm_args* a, void* stream) {
-  using namespace a3d;
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+// What one a3d_gemm call launches, decided from its arguments alone: a3d_gemm launches exactly this, and a3d_gemm_kernel
+// names it.
+struct GemmPlan {
+  GemmDev dev;        // the kernel's arguments (trace excepted)
+  SimtConv cv;        // CONV3 geometry (SIMT kernel and the A tensor map)
+  bool simt;
+  int bn, epi;        // tensor-core tile width and epilogue instance (kEpi*)
+  int smem;           // dynamic shared memory of the tensor-core kernel
+  const char* geom;   // A operand tiling: plain, conv-wide-rows, conv-row-block or conv-image-block
+};
+
+static const char* const kEpiNames[] = {"plain", "res", "geglu", "f32", "gelu"};   // indexed by kEpi*
+
+static int plan_gemm(const a3d_gemm_args* a, GemmPlan* p) {
   if (!a || !a->A || !a->B || !a->C) return fail(A3D_EINVAL, "a3d_gemm: null operand");
   if (a->M <= 0 || a->N <= 0 || a->K <= 0) return fail(A3D_EINVAL, "a3d_gemm: empty problem M=%lld N=%lld K=%lld",
                                                         (long long)a->M, (long long)a->N, (long long)a->K);
-  GemmDev d;
-  memset(&d, 0, sizeof(d));
+  memset(p, 0, sizeof(*p));
+  GemmDev& d = p->dev;
   d.M = a->M; d.N = a->N; d.K = a->K;
   d.a_mode = a->a_mode;
   d.bias = a->bias; d.rowbias = a->rowbias; d.rb_ld = a->rb_ld;
@@ -577,7 +559,6 @@ extern "C" int a3d_gemm(const a3d_gemm_args* a, void* stream) {
   d.R2 = reinterpret_cast<const __half*>(a->R2); d.ldr2 = a->ldr2;
   d.C = a->C; d.ldc = a->ldc; d.geglu = a->geglu; d.out_f32 = a->out_f32;
   d.perm_a = a->perm_a; d.perm_b = a->perm_b;
-  d.trace = g_gemm_trace;
   if (a->geglu < 0 || a->geglu > 2) return fail(A3D_EINVAL, "a3d_gemm: geglu must be 0 (none), 1 (GEGLU) or 2 (GELU)");
   const bool geglu = a->geglu == 1;
   if (geglu && (a->out_f32 || a->R1 || a->R2 || a->perm_a || (a->N % 128)))
@@ -586,8 +567,11 @@ extern "C" int a3d_gemm(const a3d_gemm_args* a, void* stream) {
     return fail(A3D_EINVAL, "a3d_gemm: GELU epilogue takes bias / row-bias only, fp16 output");
   if (a->out_f32 && (a->R1 || a->R2 || a->perm_a))
     return fail(A3D_EINVAL, "a3d_gemm: fp32 output supports bias / row-bias only");
+  if (a->impl != A3D_GEMM_AUTO && a->impl != A3D_GEMM_TC && a->impl != A3D_GEMM_SIMT)
+    return fail(A3D_EINVAL, "a3d_gemm: impl %d is not A3D_GEMM_AUTO, _TC or _SIMT", a->impl);
 
-  SimtConv cv{0, 0, 0, 0, 1, 0, 0};
+  SimtConv& cv = p->cv;
+  cv = SimtConv{0, 0, 0, 0, 1, 0, 0};
   if (a->a_mode == A3D_A_CONV3) {
     const int s = a->conv_stride;
     if (s != 1 && s != 2) return fail(A3D_EINVAL, "a3d_gemm: conv stride must be 1 or 2");
@@ -608,38 +592,35 @@ extern "C" int a3d_gemm(const a3d_gemm_args* a, void* stream) {
   // the kernel's row and column indices (up to M + 127, N + 255) and the permutation period perm_a * perm_b are 32-bit
   tc_ok = tc_ok && a->M <= INT32_MAX - kBM && a->N <= INT32_MAX - 256 &&
           (a->perm_a == 0 || (a->perm_a <= INT32_MAX && a->perm_b <= INT32_MAX / a->perm_a));
-  int boh = 0, bimg = 1, tpi = 0, tpr = 1;
+  p->geom = "plain";
+  d.bimg = 1; d.tpr = 1;
   if (a->a_mode == A3D_A_CONV3) {
     tc_ok = tc_ok && (cv.c % kBK == 0);
     const int opix = cv.oh * cv.ow;
     if (cv.ow > kBM) {           // wide images (VAE at 256^2): a tile is a 128-pixel piece of one output row
       tc_ok = tc_ok && (cv.ow % kBM == 0);
-      boh = 1; tpr = cv.ow / kBM; tpi = cv.oh * tpr; bimg = 1;
+      d.boh = 1; d.tpr = cv.ow / kBM; d.tpi = cv.oh * d.tpr;
+      p->geom = "conv-wide-rows";
     } else if (opix >= kBM) {
       tc_ok = tc_ok && (opix % kBM == 0) && (kBM % cv.ow == 0);
-      boh = kBM / cv.ow; tpi = opix / kBM; bimg = 1;
+      d.boh = kBM / cv.ow; d.tpi = opix / kBM;
+      p->geom = "conv-row-block";
     } else {
       tc_ok = tc_ok && (kBM % opix == 0);
-      boh = cv.oh; tpi = 0; bimg = kBM / (opix > 0 ? opix : 1);
+      d.boh = cv.oh; d.bimg = kBM / (opix > 0 ? opix : 1);
+      p->geom = "conv-image-block";
     }
-    tc_ok = tc_ok && (tpr > 1 ? kBM : cv.ow) * cv.s <= 256 && boh * cv.s <= 256;
+    tc_ok = tc_ok && (d.tpr > 1 ? kBM : cv.ow) * cv.s <= 256 && d.boh * cv.s <= 256;
+    d.cpb = cv.c / kBK;
+    d.conv_pad = cv.pad;
   }
   if (a->R1) tc_ok = tc_ok && (a->ldr1 % 16 == 0) && ((reinterpret_cast<uintptr_t>(a->R1) & 31) == 0);
   if (a->R2) tc_ok = tc_ok && (a->ldr2 % 16 == 0) && ((reinterpret_cast<uintptr_t>(a->R2) & 31) == 0);
-  int impl = a->impl;
-  if (impl == A3D_GEMM_AUTO) impl = tc_ok ? A3D_GEMM_TCGEN05 : A3D_GEMM_SIMT;
-  if (impl == A3D_GEMM_TCGEN05 && !tc_ok)
+  if (a->impl == A3D_GEMM_TC && !tc_ok)
     return fail(A3D_EINVAL, "a3d_gemm: shape/alignment not supported by the tensor-core path (M=%lld N=%lld K=%lld)",
                 (long long)a->M, (long long)a->N, (long long)a->K);
-
-  if (impl == A3D_GEMM_SIMT) {
-    const int64_t n_out = geglu ? a->N / 2 : a->N;
-    const int64_t total = a->M * n_out;
-    const int threads = 128;
-    const int64_t blocks = (total + threads - 1) / threads;
-    gemm_simt_kernel<<<(unsigned)blocks, threads, 0, st>>>(d, reinterpret_cast<const __half*>(a->A), a->lda,
-                                                           reinterpret_cast<const __half*>(a->B), cv);
-    A3D_LAUNCH_CHECK();
+  if (a->impl == A3D_GEMM_SIMT || !tc_ok) {
+    p->simt = true;
     return A3D_OK;
   }
 
@@ -653,30 +634,92 @@ extern "C" int a3d_gemm(const a3d_gemm_args* a, void* stream) {
     BN = 256;
   } else if (a->N % 160 == 0) BN = 160;
   else BN = 128;
-  {
-    static int force = -1;
-    if (force < 0) { const char* e = getenv("A3D_GEMM_BN"); force = e ? atoi(e) : 0; }
-    if (!geglu && (force == 128 || force == 160 || force == 256)) BN = force;   // tuning override
-  }
   d.rb_slots = gemm_rb_slots(d);
   // a table with up to 64 distinct rows per warpgroup (CLIP's position embeddings) leaves room for fewer than two stages
   // of the 256-column tile
   if (BN == 256 && GemmCfg<256>::stages(d.rb_slots) < 2) BN = 128;
-  d.stages = BN == 256 ? GemmCfg<256>::stages(d.rb_slots) : BN == 160 ? GemmCfg<160>::stages(d.rb_slots)
-                                                                      : GemmCfg<128>::stages(d.rb_slots);
+  d.stages = gemm_stages(BN, d.rb_slots);
+  p->smem = gemm_smem_bytes(BN, d.stages, d.rb_slots);
+  if (d.stages < 2 || p->smem > kGemmSmemMax)
+    return fail(A3D_EINVAL, "a3d_gemm: %d row-bias rows per warpgroup leave no room for the operand ring", d.rb_slots);
   if (geglu && a->N % BN) return fail(A3D_EINVAL, "a3d_gemm: GEGLU needs N %% 128 == 0");
   d.num_k_blocks = (int)(a->K / kBK);
   d.tiles_m = (int)((a->M + kBM - 1) / kBM);
   d.tiles_n = (int)((a->N + BN - 1) / BN);
-  d.cpb = a->a_mode == A3D_A_CONV3 ? cv.c / kBK : 0;
-  d.tpi = tpi; d.boh = boh; d.bimg = bimg; d.tpr = tpr; d.conv_pad = cv.pad;
+  p->bn = BN;
+  p->epi = a->out_f32 ? kEpiF32 : geglu ? kEpiGeglu : a->geglu == 2 ? kEpiGelu : (a->R1 || a->R2 || a->perm_a) ? kEpiRes : kEpiPlain;
+  return A3D_OK;
+}
+
+template <int BN, int EPI>
+static int launch_tc_epi(const GemmPlan& p, const CUtensorMap* mapA, const CUtensorMap* mapB, cudaStream_t st) {
+  static bool attr_set = false;
+  if (!attr_set) {
+    A3D_CUDA_CHECK(cudaFuncSetAttribute(gemm_tc_kernel<BN, EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, kGemmSmemMax));
+    attr_set = true;
+  }
+  const int tiles = p.dev.tiles_m * p.dev.tiles_n;
+  const int grid = tiles < sm_count() ? tiles : sm_count();
+  gemm_tc_kernel<BN, EPI><<<grid, kGemmThreads, p.smem, st>>>(p.dev, *mapA, *mapB);
+  A3D_LAUNCH_CHECK();
+  return A3D_OK;
+}
+
+template <int BN>
+static int launch_tc(const GemmPlan& p, const CUtensorMap* mapA, const CUtensorMap* mapB, cudaStream_t st) {
+  switch (p.epi) {
+    case kEpiF32: return launch_tc_epi<BN, kEpiF32>(p, mapA, mapB, st);
+    case kEpiGeglu:
+      if constexpr (BN % 64 == 0) return launch_tc_epi<BN, kEpiGeglu>(p, mapA, mapB, st);
+      else return fail(A3D_EINVAL, "a3d_gemm: GEGLU needs a 128- or 256-column tile");
+    case kEpiGelu: return launch_tc_epi<BN, kEpiGelu>(p, mapA, mapB, st);
+    case kEpiRes: return launch_tc_epi<BN, kEpiRes>(p, mapA, mapB, st);
+    default: return launch_tc_epi<BN, kEpiPlain>(p, mapA, mapB, st);
+  }
+}
+
+static long long* g_gemm_trace = nullptr;
+
+}  // namespace a3d
+
+// debug hook (not part of the product path): per-tile clock64 timestamps of CTA 0 of the following tensor-core GEMM launches
+extern "C" int a3d_debug_set_gemm_trace(void* device_buffer_1024_int64) {
+  a3d::g_gemm_trace = reinterpret_cast<long long*>(device_buffer_1024_int64);
+  return A3D_OK;
+}
+
+extern "C" int a3d_gemm_kernel(const a3d_gemm_args* a, char* name, size_t n) {
+  using namespace a3d;
+  GemmPlan p;
+  if (int r = plan_gemm(a, &p)) return r;
+  if (p.simt) return kernel_name(name, n, "simt");
+  return kernel_name(name, n, "tc BN%d %s %s", p.bn, kEpiNames[p.epi], p.geom);
+}
+
+extern "C" int a3d_gemm(const a3d_gemm_args* a, void* stream) {
+  using namespace a3d;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  GemmPlan p;
+  if (int r = plan_gemm(a, &p)) return r;
+  p.dev.trace = g_gemm_trace;
+  const SimtConv& cv = p.cv;
+  if (p.simt) {
+    const int64_t n_out = a->geglu == 1 ? a->N / 2 : a->N;
+    const int64_t total = a->M * n_out;
+    const int threads = 128;
+    const int64_t blocks = (total + threads - 1) / threads;
+    gemm_simt_kernel<<<(unsigned)blocks, threads, 0, st>>>(p.dev, reinterpret_cast<const __half*>(a->A), a->lda,
+                                                           reinterpret_cast<const __half*>(a->B), cv);
+    A3D_LAUNCH_CHECK();
+    return A3D_OK;
+  }
+
   const CUtensorMap *mapA = nullptr, *mapB = nullptr;
   {
-    MapKey kb;
     const uint64_t dims[5] = {(uint64_t)a->K, (uint64_t)a->N, 1, 1, 1};
     const uint64_t str[4] = {(uint64_t)a->K, (uint64_t)a->K * a->N, (uint64_t)a->K * a->N, (uint64_t)a->K * a->N};
-    const uint32_t box[5] = {kBK, (uint32_t)BN, 1, 1, 1};
-    kb = make_key(a->B, dims, str, box);
+    const uint32_t box[5] = {kBK, (uint32_t)p.bn, 1, 1, 1};
+    MapKey kb = make_key(a->B, dims, str, box);
     if (int r = get_tensor_map(kb, &mapB)) return r;
   }
   if (a->a_mode == A3D_A_PLAIN) {
@@ -686,17 +729,18 @@ extern "C" int a3d_gemm(const a3d_gemm_args* a, void* stream) {
     MapKey ka = make_key(a->A, dims, str, box);
     if (int r = get_tensor_map(ka, &mapA)) return r;
   } else {
+    const GemmDev& d = p.dev;
     const uint64_t img = (uint64_t)cv.h * cv.w * cv.c;
     const uint64_t dims[5] = {(uint64_t)cv.c, (uint64_t)cv.w, (uint64_t)cv.h, (uint64_t)cv.n, 1};
     const uint64_t str[4] = {(uint64_t)cv.c, (uint64_t)cv.w * cv.c, img, img * cv.n};
-    const uint32_t box[5] = {kBK, (uint32_t)((tpr > 1 ? kBM : cv.ow) * cv.s), (uint32_t)(boh * cv.s), (uint32_t)bimg, 1};
+    const uint32_t box[5] = {kBK, (uint32_t)((d.tpr > 1 ? kBM : cv.ow) * cv.s), (uint32_t)(d.boh * cv.s), (uint32_t)d.bimg, 1};
     MapKey ka = make_key(a->A, dims, str, box);
     ka.estr[1] = cv.s; ka.estr[2] = cv.s;
     if (int r = get_tensor_map(ka, &mapA)) return r;
   }
-  switch (BN) {
-    case 256: return launch_tc<256>(d, mapA, mapB, st);
-    case 160: return launch_tc<160>(d, mapA, mapB, st);
-    default: return launch_tc<128>(d, mapA, mapB, st);
+  switch (p.bn) {
+    case 256: return launch_tc<256>(p, mapA, mapB, st);
+    case 160: return launch_tc<160>(p, mapA, mapB, st);
+    default: return launch_tc<128>(p, mapA, mapB, st);
   }
 }

@@ -25,6 +25,17 @@ inline int fail(int code, const char* fmt, ...) {
   return code;
 }
 
+// The a3d_*_kernel queries: the kernel name into a caller buffer of n bytes, NUL-terminated; one that does not fit is an error.
+inline int kernel_name(char* name, size_t n, const char* fmt, ...) {
+  if (!name) return fail(A3D_EINVAL, "kernel name: null buffer");
+  va_list ap;
+  va_start(ap, fmt);
+  const int len = vsnprintf(name, n, fmt, ap);
+  va_end(ap);
+  if (len < 0 || (size_t)len >= n) return fail(A3D_EINVAL, "kernel name: %zu bytes do not hold the name", n);
+  return A3D_OK;
+}
+
 #define A3D_CUDA_CHECK(expr)                                                                          \
   do {                                                                                                \
     cudaError_t _e = (expr);                                                                          \

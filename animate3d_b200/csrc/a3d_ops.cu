@@ -899,11 +899,25 @@ extern "C" int a3d_layer_norm(const void* x, const float* gamma, const float* be
   return A3D_OK;
 }
 
+// The checks of a3d_temporal_attn and its kernel: temporal_attn16_kernel (16 frames, HB = 320 / d heads per block) or the
+// generic one.  *ldo: the output row stride, 0 resolved to heads * d.
+static int plan_temporal(const void* out, int frames, int heads, int d, int64_t* ldo, bool* frames16) {
+  if (frames > 32 || frames * heads > 1024) return fail(A3D_EINVAL, "a3d_temporal_attn: frames=%d heads=%d", frames, heads);
+  if (*ldo == 0) *ldo = (int64_t)heads * d;
+  if (*ldo < (int64_t)heads * d || *ldo % 8 || (reinterpret_cast<uintptr_t>(out) & 15))
+    return fail(A3D_EINVAL, "a3d_temporal_attn: output row stride %lld must be >= C, a multiple of 8, 16-byte aligned base",
+                (long long)*ldo);
+  if (d != 40 && d != 80 && d != 160) return fail(A3D_EINVAL, "a3d_temporal_attn: head dim %d not in {40,80,160}", d);
+  const int hb = 320 / d;
+  *frames16 = frames == 16 && heads % hb == 0 && heads / hb <= 65535;
+  return A3D_OK;
+}
+
 template <int D>
 static int launch_temporal(const void* qkv, void* out, int64_t pixels, int frames, int heads, float scale, int64_t ldo,
-                           cudaStream_t st) {
+                           bool frames16, cudaStream_t st) {
   constexpr int HB = 320 / D;   // 8 / 4 / 2 heads per block
-  if (frames == 16 && heads % HB == 0 && heads / HB <= 65535) {
+  if (frames16) {
     const size_t smem16 = (size_t)16 * (3 * HB * D + 8) * 2;   // 31 KB
     temporal_attn16_kernel<D, HB><<<dim3((unsigned)pixels, (unsigned)(heads / HB)), HB * 32, smem16, st>>>(
         reinterpret_cast<const __half*>(qkv), reinterpret_cast<__half*>(out), heads, scale * 1.4426950408889634f, ldo);
@@ -923,18 +937,22 @@ static int launch_temporal(const void* qkv, void* out, int64_t pixels, int frame
   return A3D_OK;
 }
 
+extern "C" int a3d_temporal_attn_kernel(const void* out, int64_t pixels, int frames, int heads, int d, int64_t ldo, char* name,
+                                        size_t n) {
+  bool frames16;
+  if (int r = plan_temporal(out, frames, heads, d, &ldo, &frames16)) return r;
+  return kernel_name(name, n, "%s", frames16 ? "frames16" : "generic");
+}
+
 extern "C" int a3d_temporal_attn(const void* qkv, void* out, int64_t pixels, int frames, int heads, int d, float scale,
                                  int64_t ldo, void* stream) {
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  if (frames > 32 || frames * heads > 1024) return fail(A3D_EINVAL, "a3d_temporal_attn: frames=%d heads=%d", frames, heads);
-  if (ldo == 0) ldo = (int64_t)heads * d;
-  if (ldo < (int64_t)heads * d || ldo % 8 || (reinterpret_cast<uintptr_t>(out) & 15))
-    return fail(A3D_EINVAL, "a3d_temporal_attn: output row stride %lld must be >= C, a multiple of 8, 16-byte aligned base", (long long)ldo);
+  bool frames16;
+  if (int r = plan_temporal(out, frames, heads, d, &ldo, &frames16)) return r;
   switch (d) {
-    case 40: return launch_temporal<40>(qkv, out, pixels, frames, heads, scale, ldo, st);
-    case 80: return launch_temporal<80>(qkv, out, pixels, frames, heads, scale, ldo, st);
-    case 160: return launch_temporal<160>(qkv, out, pixels, frames, heads, scale, ldo, st);
-    default: return fail(A3D_EINVAL, "a3d_temporal_attn: head dim %d not in {40,80,160}", d);
+    case 40: return launch_temporal<40>(qkv, out, pixels, frames, heads, scale, ldo, frames16, st);
+    case 80: return launch_temporal<80>(qkv, out, pixels, frames, heads, scale, ldo, frames16, st);
+    default: return launch_temporal<160>(qkv, out, pixels, frames, heads, scale, ldo, frames16, st);
   }
 }
 

@@ -26,16 +26,13 @@ def _chk16(*ts):
             assert t.is_cuda and t.dtype == HALF and t.is_contiguous(), (t.dtype, t.shape, t.is_contiguous())
 
 
-def gemm(A: torch.Tensor, B: torch.Tensor, out: torch.Tensor, *, M: int, N: int, K: int, lda: int = 0, ldc: int = 0,
-         conv: Optional[Tuple[int, int, int, int, int]] = None, bias=None, rowbias=None, rb_div: int = 1, rb_mod: int = 0,
-         rb_ld: int = 0,
-         acc_scale: float = 1.0, R1=None, ldr1: int = 0, r1_scale: float = 1.0, R2=None, ldr2: int = 0, geglu: bool = False,
-         out_f32: bool = False, perm: Tuple[int, int] = (0, 0), impl: int = L.IMPL_AUTO, conv_nopad_lo: bool = False,
-         gelu: bool = False) -> torch.Tensor:
-    """out = epilogue(A @ B^T); see a3d_gemm in include/a3d.h.  `conv` = (n_img, H, W, C, stride) selects the implicit
-    3x3 convolution A operand; `gelu` applies the erf GELU to the biased value (CLIP's MLP)."""
+def _gemm_args(A, B, out, *, M: int, N: int, K: int, lda: int = 0, ldc: int = 0,
+               conv: Optional[Tuple[int, int, int, int, int]] = None, bias=None, rowbias=None, rb_div: int = 1, rb_mod: int = 0,
+               rb_ld: int = 0,
+               acc_scale: float = 1.0, R1=None, ldr1: int = 0, r1_scale: float = 1.0, R2=None, ldr2: int = 0, geglu: bool = False,
+               out_f32: bool = False, perm: Tuple[int, int] = (0, 0), impl: int = L.IMPL_AUTO, conv_nopad_lo: bool = False,
+               gelu: bool = False) -> L.GemmArgs:
     assert not (geglu and gelu)
-    lib = L.load()
     a = L.GemmArgs()
     a.A, a.B, a.C = A.data_ptr(), B.data_ptr(), out.data_ptr()
     a.M, a.N, a.K = M, N, K
@@ -59,8 +56,26 @@ def gemm(A: torch.Tensor, B: torch.Tensor, out: torch.Tensor, *, M: int, N: int,
     a.out_f32 = int(out_f32)
     a.perm_a, a.perm_b = perm
     a.impl = impl
-    _enqueued(lib.a3d_gemm(C.byref(a), L.stream_ptr()))
+    return a
+
+
+def _kernel_name(query, *args) -> str:
+    name = C.create_string_buffer(48)
+    L.check(query(*args, name, C.c_size_t(len(name))))
+    return name.value.decode()
+
+
+def gemm(A: torch.Tensor, B: torch.Tensor, out: torch.Tensor, **kw) -> torch.Tensor:
+    """out = epilogue(A @ B^T); see a3d_gemm in include/a3d.h and the keywords of `_gemm_args`.  `conv` = (n_img, H, W, C,
+    stride) selects the implicit 3x3 convolution A operand; `gelu` applies the erf GELU to the biased value (CLIP's MLP)."""
+    lib = L.load()
+    _enqueued(lib.a3d_gemm(C.byref(_gemm_args(A, B, out, **kw)), L.stream_ptr()))
     return out
+
+
+def gemm_kernel(A, B, out, **kw) -> str:
+    """The kernel `gemm` launches for the same arguments (a3d_gemm_kernel), e.g. "tc BN256 res plain"; launches nothing."""
+    return _kernel_name(L.load(require_gpu=False).a3d_gemm_kernel, C.byref(_gemm_args(A, B, out, **kw)))
 
 
 def view5(base: torch.Tensor, col_offset: int, cols: int, strides, extents) -> L.View5:
@@ -72,10 +87,9 @@ def view5(base: torch.Tensor, col_offset: int, cols: int, strides, extents) -> L
     return v
 
 
-def attention(q: L.View5, k: L.View5, v: L.View5, out: torch.Tensor, ostrides, *, heads: int, d: int, scale: float,
-              kv_div: int = 1, kv_i3_zero: bool = False, accumulate: bool = False, out_scale: float = 1.0,
-              impl: int = L.IMPL_AUTO, out_col_offset: int = 0) -> None:
-    lib = L.load()
+def _attn_args(q: L.View5, k: L.View5, v: L.View5, out, ostrides, *, heads: int, d: int, scale: float, kv_div: int = 1,
+               kv_i3_zero: bool = False, accumulate: bool = False, out_scale: float = 1.0, impl: int = L.IMPL_AUTO,
+               out_col_offset: int = 0) -> L.AttnArgs:
     a = L.AttnArgs()
     a.q, a.k, a.v = q, k, v
     a.out = out.data_ptr() + 2 * out_col_offset
@@ -83,15 +97,37 @@ def attention(q: L.View5, k: L.View5, v: L.View5, out: torch.Tensor, ostrides, *
     a.heads, a.d, a.scale = heads, d, scale
     a.kv_div, a.kv_i3_zero = kv_div, int(kv_i3_zero)
     a.accumulate, a.out_scale, a.impl = int(accumulate), out_scale, impl
-    _enqueued(lib.a3d_attention(C.byref(a), L.stream_ptr()))
+    return a
 
 
-def temporal_attn(qkv: torch.Tensor, out: torch.Tensor, pixels: int, frames: int, heads: int, d: int, scale: float,
-                  ldo: int = 0, out_col_offset: int = 0):
-    """out rows have stride `ldo` halves (0 = heads*d) and start at column `out_col_offset` of `out`."""
+def attention(q: L.View5, k: L.View5, v: L.View5, out: torch.Tensor, ostrides, **kw) -> None:
+    """a3d_attention; the keywords are those of `_attn_args`."""
     lib = L.load()
-    _enqueued(lib.a3d_temporal_attn(C.c_void_p(qkv.data_ptr()), C.c_void_p(out.data_ptr() + 2 * out_col_offset), C.c_int64(pixels),
-                                  frames, heads, d, C.c_float(scale), C.c_int64(ldo), L.stream_ptr()))
+    _enqueued(lib.a3d_attention(C.byref(_attn_args(q, k, v, out, ostrides, **kw)), L.stream_ptr()))
+
+
+def attention_kernel(q: L.View5, k: L.View5, v: L.View5, out, ostrides, **kw) -> str:
+    """The kernel `attention` launches for the same arguments (a3d_attention_kernel): fewkeys, shortkeys or tc."""
+    return _kernel_name(L.load(require_gpu=False).a3d_attention_kernel, C.byref(_attn_args(q, k, v, out, ostrides, **kw)))
+
+
+def _temporal_args(qkv, out, pixels: int, frames: int, heads: int, d: int, scale: float, ldo: int = 0, out_col_offset: int = 0):
+    """(qkv, out, pixels, frames, heads, d, scale, ldo) as the C arguments of a3d_temporal_attn."""
+    return (C.c_void_p(qkv.data_ptr()), C.c_void_p(out.data_ptr() + 2 * out_col_offset), C.c_int64(pixels), frames, heads, d,
+            C.c_float(scale), C.c_int64(ldo))
+
+
+def temporal_attn(qkv: torch.Tensor, out: torch.Tensor, *args, **kw):
+    """a3d_temporal_attn; the arguments are those of `_temporal_args`: out rows have stride `ldo` halves (0 = heads*d) and
+    start at column `out_col_offset` of `out`."""
+    lib = L.load()
+    _enqueued(lib.a3d_temporal_attn(*_temporal_args(qkv, out, *args, **kw), L.stream_ptr()))
+
+
+def temporal_attn_kernel(qkv, out, *args, **kw) -> str:
+    """The kernel `temporal_attn` launches for the same arguments (a3d_temporal_attn_kernel): frames16 or generic."""
+    _, o, pixels, frames, heads, d, _, ldo = _temporal_args(qkv, out, *args, **kw)
+    return _kernel_name(L.load(require_gpu=False).a3d_temporal_attn_kernel, o, pixels, frames, heads, d, ldo)
 
 
 def group_norm_ws_floats(samples: int, rows_per_sample: int, c: int, groups: int) -> int:

@@ -53,8 +53,10 @@ int a3d_init(void);
  * Row permutation (perm_a, perm_b > 0): om = (m / (a*b))*(a*b) + (m % b)*a + (m / b) % a   ("(x a b) -> (x b a)").
  */
 enum { A3D_A_PLAIN = 0, A3D_A_CONV3 = 1 };
-/* A3D_GEMM_TCGEN05 selects the tensor-core (wgmma) kernels; the name is kept for ABI compatibility. */
-enum { A3D_GEMM_AUTO = 0, A3D_GEMM_TCGEN05 = 1, A3D_GEMM_SIMT = 2 };
+/* impl: A3D_GEMM_AUTO lets the library pick the kernel from the arguments; A3D_GEMM_TC forces the tensor-core (wgmma)
+ * kernels and fails with A3D_EINVAL where they cannot run; A3D_GEMM_SIMT forces a3d_gemm's one-thread-per-element kernel,
+ * which AUTO also picks for shapes and alignments the tensor cores cannot take. */
+enum { A3D_GEMM_AUTO = 0, A3D_GEMM_TC = 1, A3D_GEMM_SIMT = 2 };
 
 typedef struct a3d_gemm_args {
   const void* A;      /* fp16 */
@@ -77,7 +79,7 @@ typedef struct a3d_gemm_args {
   int geglu;                  /* 0 = none, 1 = GEGLU, 2 = GELU */
   int out_f32;
   int64_t perm_a, perm_b;     /* 0,0 = identity */
-  int impl;                   /* A3D_GEMM_* */
+  int impl;                   /* A3D_GEMM_AUTO / _TC / _SIMT */
 } a3d_gemm_args;
 
 /* Replaces every Linear / Conv2d(3x3) the reference's forward issues through torch: ResnetBlock2D conv1/conv2/
@@ -86,6 +88,16 @@ typedef struct a3d_gemm_args {
  * to_q/to_k/to_v/to_out + *_i2v / *_ip / *_sp projections (animatediff/models/attention_processor.py:211-231, 383-403,
  * 425-441, 600-655, 686-717), with their bias, residual, positional-table and layout epilogues fused. */
 int a3d_gemm(const a3d_gemm_args* args, void* stream);
+
+/* Kernel queries: the kernel the matching call would launch for the same arguments, as a NUL-terminated name in name[n]
+ * (names are shorter than 48 bytes; a buffer too small for the name is A3D_EINVAL).  They launch nothing, never touch the
+ * device or dereference an operand pointer, need no a3d_init, and fail with the same A3D_EINVAL and a3d_last_error() as
+ * the call.  A failure to encode a tensor map is reported by the call alone.
+ *   a3d_gemm_kernel           "simt", or "tc BN{128|160|256} {plain|res|geglu|gelu|f32} {plain|conv-wide-rows|conv-row-block|
+ *                             conv-image-block}": tile width, epilogue instance, A operand tiling
+ *   a3d_attention_kernel      "fewkeys" (<= 8 keys), "shortkeys" (9..80 keys, operand rows aligned for it) or "tc"
+ *   a3d_temporal_attn_kernel  "frames16" or "generic" */
+int a3d_gemm_kernel(const a3d_gemm_args* args, char* name, size_t n);
 
 /* ---------------------------------------------------------------- fused attention (wgmma) -------------------- */
 /* O = softmax(scale * Q K^T) V per (batch, head); Q/K/V are read in place from projection outputs through rank-5
@@ -115,7 +127,8 @@ typedef struct a3d_attn_args {
   float scale;
   int kv_div, kv_i3_zero;
   int accumulate; float out_scale;  /* MUST be set (1.0 if unused; 0.0 is honoured, not remapped: accumulate leaves out as is) */
-  int impl;                 /* A3D_GEMM_AUTO / _TCGEN05 / _SIMT */
+  int impl;                 /* A3D_GEMM_AUTO: by key count (few-keys, short-keys or tensor-core kernel); A3D_GEMM_TC: the
+                               tensor-core kernel at any key count.  Anything else is A3D_EINVAL. */
 } a3d_attn_args;
 
 /* Replaces the xformers.ops.memory_efficient_attention calls of the processors together with the einops regroups around
@@ -123,6 +136,7 @@ typedef struct a3d_attn_args {
  * `scale`), 405 (cross-view self-attention) and 416 (I2V branch, frame-0 keys: kv_i3_zero), 656 and 691 (spatio-temporal
  * processor's cross-view / image branches). */
 int a3d_attention(const a3d_attn_args* args, void* stream);
+int a3d_attention_kernel(const a3d_attn_args* args, char* name, size_t n);
 
 /* Temporal attention over F frames for every (pixel, head): qkv [P, F, 3*C] fp16 (q | k | v), out [P, F, C].
  * Replaces the attention of the motion modules' temporal transformer blocks (diffusers TransformerTemporalModel reached
@@ -130,6 +144,7 @@ int a3d_attention(const a3d_attn_args* args, void* stream);
 int a3d_temporal_attn(const void* qkv, void* out, int64_t pixels, int frames, int heads, int d, float scale, int64_t ldo,
                       void* stream);   /* ldo: output row stride in halves (0 = C): lets the result land in a column block of a
                                           wider buffer, e.g. next to the cross-view branch for the merged output projection */
+int a3d_temporal_attn_kernel(const void* out, int64_t pixels, int frames, int heads, int d, int64_t ldo, char* name, size_t n);
 
 /* ---------------------------------------------------------------- normalisation / elementwise ---------------- */
 /* Replaces nn.GroupNorm (+ SiLU) of ResnetBlock2D.norm1/norm2, Transformer2DModel.norm, TransformerTemporalModel.norm

@@ -35,73 +35,15 @@ def _snap(t, n):
     return O.flat(t, n).clone()
 
 
-# ------------------------------------------------------------------------------------------------ kernel path (mirrors the host dispatch)
-def gemm_path(A, B, out, kw):
-    M, N, K = kw["M"], kw["N"], kw["K"]
-    geglu, f32 = kw.get("geglu", False), kw.get("out_f32", False)
-    n_out = N // 2 if geglu else N
-    lda, ldc = kw.get("lda", 0) or K, kw.get("ldc", 0) or n_out
-    conv = kw.get("conv")
-    R1, R2 = kw.get("R1"), kw.get("R2")
-    perm = kw.get("perm", (0, 0))
-    ok = K % 64 == 0 and N % (16 if geglu else 8) == 0 and A.data_ptr() % 16 == 0 and B.data_ptr() % 16 == 0 and ldc % 16 == 0 \
-        and out.data_ptr() % 32 == 0
-    geom = "plain"
-    if conv is None:
-        ok = ok and lda % 8 == 0 and lda >= K
-    else:
-        n, h, w, c, s = conv
-        oh, ow = h // s, w // s
-        ok = ok and c % 64 == 0
-        if ow > 128:
-            geom, tpr, boh = "conv-wide-rows", ow // 128, 1
-            ok = ok and ow % 128 == 0
-        elif oh * ow >= 128:
-            geom, tpr, boh = "conv-row-block", 1, 128 // ow
-            ok = ok and (oh * ow) % 128 == 0 and 128 % ow == 0
-        else:
-            geom, tpr, boh = "conv-image-block", 1, oh
-            ok = ok and 128 % (oh * ow) == 0
-        ok = ok and (128 if tpr > 1 else ow) * s <= 256 and boh * s <= 256
-    for R, ld in ((R1, kw.get("ldr1", 0) or N), (R2, kw.get("ldr2", 0) or N)):
-        if R is not None:
-            ok = ok and ld % 16 == 0 and R.data_ptr() % 32 == 0
-    impl = kw.get("impl", 0)
-    if impl == 2 or (impl == 0 and not ok):
-        return "simt"
-    if geglu:
-        bn = 256 if N % 256 == 0 else 128
-    elif N % 256 == 0:
-        bn = 256
-    elif K <= 640 and N > 512 and (256 * ((N + 255) // 256) - N) * 8 <= N:
-        bn = 256
-    elif N % 160 == 0:
-        bn = 160
-    else:
-        bn = 128
-    epi = "f32" if f32 else "geglu" if geglu else "res" if (R1 is not None or R2 is not None or perm[0]) else "plain"
-    return f"tc BN{bn} {epi} {geom}"
-
-
-def attention_path(q, k, kw):
-    impl = kw.get("impl", 0)
-    lk = k.e1 * k.e2
-    if impl == 2:
-        return "simt"
-    if impl == 0 and lk <= 8:
-        return "fewkeys"
-    if impl == 0 and lk <= 80:
-        return "shortkeys"
-    return "tc"
-
-
 # ------------------------------------------------------------------------------------------------ the wrappers
 def _v5(v):
     return O.V5(v._t, v._off, v.cols, (v.s1, v.s2, v.s3, v.s4), (v.e1, v.e2, v.e3, v.e4))
 
 
 def _prepare(op, a, kw):
-    """-> (oracle thunk to run after the call, output tensor, output span, kernel path, geometry)."""
+    """-> (oracle thunk to run after the call, output tensor, output span, kernel path, geometry).  The kernel path is the
+    library's own answer for these arguments (ops.*_kernel)."""
+    from animate3d_b200 import ops
     if op == "gemm":
         A, B, out = a
         M, N, K = kw["M"], kw["N"], kw["K"]
@@ -117,7 +59,7 @@ def _prepare(op, a, kw):
                 k2[r] = _snap(kw[r], O.span_of(M, N, k2[ld]))
         if kw.get("rowbias") is not None:
             k2["rb_ld"] = kw.get("rb_ld", 0) or kw["rowbias"].stride(0)
-        path = gemm_path(A, B, out, kw)
+        path = ops.gemm_kernel(*a, **kw)
         geo = f"M={M} N={N} K={K}" + (f" conv={kw['conv']}" if kw.get("conv") else "") + \
             "".join(f" {f}" for f in ("bias", "rowbias", "R1", "R2") if kw.get(f) is not None) + \
             (f" perm={kw['perm']}" if kw.get("perm", (0, 0))[0] else "") + (" geglu" if geglu else "")
@@ -129,7 +71,7 @@ def _prepare(op, a, kw):
         span = O.out_span((q.e1, q.e2, q.e3, q.e4), ostr, heads * d, off)
         snap = _snap(out, span)
         k2 = dict(kw)
-        path = attention_path(q, k, kw)
+        path = ops.attention_kernel(*a, **kw)
         geo = f"Lq={q.e1 * q.e2} Lk={k.e1 * k.e2} batches={q.e3 * q.e4} d={d}" + \
             "".join(f" {f}={kw[f]}" for f in ("kv_div", "kv_i3_zero", "accumulate", "out_scale", "out_col_offset") if kw.get(f))
         return (lambda: O.attention(_v5(q), _v5(k), _v5(v), snap, ostr, **k2)), out, span, path, geo
@@ -139,8 +81,7 @@ def _prepare(op, a, kw):
         off = kw.get("out_col_offset", 0)
         span = off + O.span_of(pixels * frames, heads * d, ldo)
         snap = _snap(out, span)
-        hb = 320 // d
-        path = "frames16" if frames == 16 and heads % hb == 0 else "generic"
+        path = ops.temporal_attn_kernel(*a, **kw)
         return (lambda: O.temporal_attn(qkv, snap, pixels, frames, heads, d, scale, ldo=ldo, out_col_offset=off)), out, span, \
             path, f"P={pixels} F={frames} d={d} ldo={ldo} off={off}"
     if op == "ddim_cfg_step":

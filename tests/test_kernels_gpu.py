@@ -202,7 +202,7 @@ ATTN_CASES = [
 
 
 @pytest.mark.parametrize("layout", ["spatial_tf", "motion"])
-@pytest.mark.parametrize("impl", ["tc", "simt"])
+@pytest.mark.parametrize("impl", ["tc"])
 @pytest.mark.parametrize("case", ATTN_CASES, ids=lambda c: c[0])
 def test_cross_view_attention(case, impl, layout):
     """MV attention ("(b n f) l c -> (b f) (n l) c") + the I2V branch (frame-0 keys) through the strided views."""
@@ -232,7 +232,7 @@ def test_cross_view_attention(case, impl, layout):
     ext = (hw, Nv, Fr, B)
     qoff, q2off, koff, voff = 0, heads * dqk, 2 * heads * dqk, 3 * heads * dqk
     scale = d ** -0.5
-    im = L.IMPL_TC if impl == "tc" else L.IMPL_SIMT
+    im = L.IMPL_TC
     out = torch.zeros(rows, C, device=DEV, dtype=torch.float16)
     vq = ops.view5(buf, qoff, ld - qoff, strides, ext)
     vk = ops.view5(buf, koff, ld - koff, strides, ext)
@@ -253,7 +253,7 @@ def test_cross_view_attention(case, impl, layout):
     close(out, ref2, what=f"i2v attention {name} {impl} {layout}")
 
 
-@pytest.mark.parametrize("impl", ["tc", "auto", "simt"])
+@pytest.mark.parametrize("impl", ["tc", "auto"])
 @pytest.mark.parametrize("case", [(2, 3, 1024, 40, 77), (2, 2, 256, 80, 77), (3, 2, 64, 160, 4), (2, 2, 16, 160, 77),
                                   (2, 3, 1024, 40, 4), (3, 2, 256, 80, 4), (2, 2, 64, 160, 8), (2, 2, 256, 40, 16)],
                          ids=lambda c: "bn%d_f%d_hw%d_d%d_k%d" % c)
@@ -274,7 +274,7 @@ def test_cross_attention_text_keys(case, impl):
     vv = ops.view5(kvbuf, 2 * heads * dqk, ldk - 2 * heads * dqk, (ldk, Lk * ldk, Lk * ldk, Lk * ldk), (Lk, 1, 1, BN))
     out = torch.zeros(rows, C, device=DEV, dtype=torch.float16)
     scale = d ** -0.5
-    im = {"tc": L.IMPL_TC, "auto": L.IMPL_AUTO, "simt": L.IMPL_SIMT}[impl]   # auto = few-keys / short-keys kernels
+    im = {"tc": L.IMPL_TC, "auto": L.IMPL_AUTO}[impl]   # auto = few-keys / short-keys kernels
     ops.attention(vq, vk, vv, out, (C, hw * C, hw * C, Fr * hw * C), heads=heads, d=d, scale=scale, kv_div=Fr, impl=im)
     qq = q[:, 0].reshape(BN, Fr, hw, heads, d).permute(0, 1, 3, 2, 4)                  # [BN, F, H, hw, d]
     kk = k.reshape(BN, 1, Lk, heads, d).permute(0, 1, 3, 2, 4).expand(BN, Fr, heads, Lk, d)
