@@ -778,8 +778,11 @@ conv_out_kernel(const __half* __restrict__ x, const float* __restrict__ w, const
   }
 }
 
-__global__ void ddim_cfg_step_kernel(float* __restrict__ lat, const float* __restrict__ eps2, const float* __restrict__ first,
-                                     int bn, int c, int f, int hw, float g, float a_t, float a_prev, int uncond_first) {
+// cfg_mode: 0 = noise_pred holds bn samples (no guidance); 1 = (uncond, cond) halves; 2 = (cond, uncond) halves.
+// z (variance noise) is read only when non-null.  Both a3d_ddim_step and a3d_ddim_cfg_step launch this kernel.
+__global__ void ddim_step_kernel(float* __restrict__ lat, const float* __restrict__ eps_in, const float* __restrict__ first,
+                                 const float* __restrict__ z, int bn, int c, int f, int hw, int cfg_mode, float g, float a_t,
+                                 float a_prev, float dir_coef, float std_dev) {
   const int64_t n = (int64_t)bn * c * f * hw;
   const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= n) return;
@@ -789,11 +792,18 @@ __global__ void ddim_cfg_step_kernel(float* __restrict__ lat, const float* __res
     lat[idx] = first[sc * hw + idx % hw];
     return;
   }
-  const float e0 = eps2[idx], e1 = eps2[n + idx];
-  const float eps = uncond_first ? (e0 + g * (e1 - e0)) : (e0 + g * (e0 - e1));
+  float eps;
+  if (cfg_mode == 0) {
+    eps = eps_in[idx];
+  } else {
+    const float e0 = eps_in[idx], e1 = eps_in[n + idx];
+    eps = cfg_mode == 1 ? (e0 + g * (e1 - e0)) : (e0 + g * (e0 - e1));
+  }
   const float x = lat[idx];
   const float x0 = (x - sqrtf(1.f - a_t) * eps) / sqrtf(a_t);
-  lat[idx] = sqrtf(a_prev) * x0 + sqrtf(1.f - a_prev) * eps;
+  float v = sqrtf(a_prev) * x0 + dir_coef * eps;
+  if (z) v += std_dev * z[idx];
+  lat[idx] = v;
 }
 
 }  // namespace a3d
@@ -1027,12 +1037,21 @@ extern "C" int a3d_cast_f32_f16(const float* x, void* y, int64_t n, void* stream
   return A3D_OK;
 }
 
-extern "C" int a3d_ddim_cfg_step(float* latents, const float* noise_pred, const float* first_frame, int bn, int c, int f,
-                                 int hw, float guidance, float alpha_t, float alpha_prev, int uncond_first, void* stream) {
+extern "C" int a3d_ddim_step(float* latents, const float* noise_pred, const float* first_frame, const float* variance_noise,
+                             int bn, int c, int f, int hw, int cfg_mode, float guidance, float alpha_t, float alpha_prev,
+                             float dir_coef, float std_dev, void* stream) {
+  if (cfg_mode < 0 || cfg_mode > 2) return fail(A3D_EINVAL, "a3d_ddim_step: cfg_mode %d is not 0, 1 or 2", cfg_mode);
+  if (std_dev != 0.f && !variance_noise) return fail(A3D_EINVAL, "a3d_ddim_step: std_dev %g needs variance_noise", std_dev);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   const int64_t n = (int64_t)bn * c * f * hw;
-  ddim_cfg_step_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(latents, noise_pred, first_frame, bn, c, f, hw, guidance,
-                                                                   alpha_t, alpha_prev, uncond_first);
+  ddim_step_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(latents, noise_pred, first_frame, variance_noise, bn, c, f, hw,
+                                                               cfg_mode, guidance, alpha_t, alpha_prev, dir_coef, std_dev);
   A3D_LAUNCH_CHECK();
   return A3D_OK;
+}
+
+extern "C" int a3d_ddim_cfg_step(float* latents, const float* noise_pred, const float* first_frame, int bn, int c, int f,
+                                 int hw, float guidance, float alpha_t, float alpha_prev, int uncond_first, void* stream) {
+  return a3d_ddim_step(latents, noise_pred, first_frame, nullptr, bn, c, f, hw, uncond_first ? 1 : 2, guidance, alpha_t,
+                       alpha_prev, sqrtf(1.f - alpha_prev), 0.f, stream);
 }

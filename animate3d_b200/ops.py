@@ -215,6 +215,18 @@ def ddim_cfg_step(latents, noise_pred, first_frame, bn, c, f, hw, guidance, alph
     return latents
 
 
+def ddim_step(latents, noise_pred, first_frame, variance_noise, bn, c, f, hw, cfg_mode, guidance, alpha_t, alpha_prev, dir_coef,
+              std_dev):
+    """a3d_ddim_step: cfg_mode 0 = no guidance, 1 = (uncond, cond) halves, 2 = (cond, uncond) halves; `variance_noise` may be
+    None when std_dev == 0."""
+    lib = L.load()
+    _enqueued(lib.a3d_ddim_step(C.c_void_p(latents.data_ptr()), C.c_void_p(noise_pred.data_ptr()), C.c_void_p(L.ptr(first_frame)),
+                              C.c_void_p(L.ptr(variance_noise)), bn, c, f, hw, int(cfg_mode), C.c_float(guidance),
+                              C.c_float(alpha_t), C.c_float(alpha_prev), C.c_float(dir_coef), C.c_float(std_dev),
+                              L.stream_ptr()))
+    return latents
+
+
 def clip_resize_tables(h: int, w: int):
     """Host-built Pillow bicubic tables of the CLIP resize of an h x w image: (resize_h, resize_w, (bounds_y, coeffs_y,
     ksize_y), (bounds_x, coeffs_x, ksize_x)) with int32 CPU tensors."""

@@ -83,6 +83,30 @@ def _butterworth_lpf(shape, order=4, d_s=0.25, d_t=0.25, device="cpu"):
     return 1.0 / (1.0 + (d2 / d_s ** 2) ** order)
 
 
+def randn_tensor(shape, generator: Optional[torch.Generator], device) -> torch.Tensor:
+    """diffusers' randn_tensor for one generator: fp32 normal noise drawn on the generator's device (so a CPU generator
+    gives the same stream whatever `device` is), then moved to `device`."""
+    rand_device = generator.device if generator is not None else device
+    return torch.randn(shape, generator=generator, device=rand_device, dtype=torch.float32).to(device)
+
+
+def similarity_init_latents(first_frame_latents: torch.Tensor, num_frames: int, t_first: int, origin_prob: float,
+                            scheduler: DDIMScheduler, generator: Optional[torch.Generator]) -> torch.Tensor:
+    """`i2v_similarity_init` latents of frames 1.. (reference prepare_latents, pipeline.py:707-724): each pixel of each
+    frame is the first-frame latent with probability `origin_prob`, else that latent noised to the first timestep.  Draws
+    the mask (uniform, [Nv, 1, num_frames, h, w]) and then the noise ([Nv, C, num_frames, h, w]) with `generator`, on its
+    device.  No init_noise_sigma scaling (pipeline.py:727-729; it is 1)."""
+    nv, c, _, h, w = first_frame_latents.shape
+    dev = first_frame_latents.device
+    rand_device = generator.device if generator is not None else dev
+    mask = torch.rand((nv, 1, num_frames, h, w), generator=generator, device=rand_device, dtype=torch.float32).to(dev)
+    mask = (mask < origin_prob).float()
+    noise = randn_tensor((nv, c, num_frames, h, w), generator, dev)
+    cond = first_frame_latents.repeat_interleave(num_frames, dim=2)
+    noised = scheduler.add_noise(cond, noise, torch.full((nv,), int(t_first), dtype=torch.long))
+    return mask * cond + (1 - mask) * noised
+
+
 class AnimateDiffMVI2VPipeline:
     """`AnimationPipeline` of north_star == this class (alias below).  Constructor keeps the reference's argument names
     (pipeline.py:308-325); everything except `unet` and `scheduler` is optional."""
@@ -190,16 +214,32 @@ class AnimateDiffMVI2VPipeline:
     # -------------------------------------------------------------------------------------------- one denoise step
     def denoise_step(self, latents: torch.Tensor, t: int, prompt_embeds: torch.Tensor, camera: torch.Tensor,
                      image_embeds: torch.Tensor, first_frame_latents: torch.Tensor, guidance_scale: float,
-                     i2v_cond_time_zero: bool = False, num_views: int = 4) -> torch.Tensor:
+                     i2v_cond_time_zero: bool = False, num_views: int = 4, do_classifier_free_guidance: bool = True,
+                     eta: float = 0.0, generator: Optional[torch.Generator] = None,
+                     variance_noise: Optional[torch.Tensor] = None) -> torch.Tensor:
         """Body of the loop at pipeline.py:1006-1031, in place on `latents` [Nv, 4, F, h, w] (fp32, device).
-        prompt_embeds / camera / image_embeds already carry the (uncond, cond) CFG duplication."""
-        x2 = torch.cat([latents, latents], 0)
-        noise_pred = self.unet(x2, t, prompt_embeds, camera=camera, added_cond_kwargs={"image_embeds": image_embeds},
+        With guidance, prompt_embeds / camera / image_embeds carry the (uncond, cond) CFG duplication; without it
+        (guidance_scale <= 1 in `__call__`) they are the conditional ones only and the UNet batch is `latents` itself.
+        eta > 0 adds std_dev * variance_noise (DDIMScheduler.step); unless given, the noise is drawn with `generator`, one
+        draw of the latents' full shape per step, after the UNet call, as diffusers does."""
+        if variance_noise is not None and generator is not None:
+            raise ValueError("pass either `generator` or `variance_noise`, not both (DDIMScheduler.step)")
+        x = torch.cat([latents, latents], 0) if do_classifier_free_guidance else latents
+        noise_pred = self.unet(x, t, prompt_embeds, camera=camera, added_cond_kwargs={"image_embeds": image_embeds},
                                num_views=num_views, i2v_cond_time_zero=i2v_cond_time_zero).sample
-        a_t, a_p = self.scheduler.alphas_for(int(t))
         bn, c, f, h, w = latents.shape
-        ops.ddim_cfg_step(latents, noise_pred.contiguous(), first_frame_latents.contiguous(), bn, c, f, h * w, guidance_scale,
-                          a_t, a_p, uncond_first=True)
+        if do_classifier_free_guidance and eta == 0:
+            # the released sampler: a3d_ddim_cfg_step runs the same kernel as a3d_ddim_step with std_dev 0
+            a_t, a_p = self.scheduler.alphas_for(int(t))
+            ops.ddim_cfg_step(latents, noise_pred.contiguous(), first_frame_latents.contiguous(), bn, c, f, h * w, guidance_scale,
+                              a_t, a_p, uncond_first=True)
+            return latents
+        a_t, a_p, dir_coef, std_dev = self.scheduler.step_coefficients(int(t), eta)
+        if eta > 0 and variance_noise is None:
+            variance_noise = randn_tensor(latents.shape, generator, latents.device)
+        z = variance_noise.to(latents.device, torch.float32).contiguous() if eta > 0 else None
+        ops.ddim_step(latents, noise_pred.contiguous(), first_frame_latents.contiguous(), z, bn, c, f, h * w,
+                      1 if do_classifier_free_guidance else 0, guidance_scale, a_t, a_p, dir_coef, std_dev if eta > 0 else 0.0)
         return latents
 
     def denoise_step_host(self, latents_host: torch.Tensor, t: int, prompt_embeds_host, camera_host, image_embeds_host,
@@ -279,39 +319,48 @@ class AnimateDiffMVI2VPipeline:
         """Argument names follow pipeline.py:760-786.  `num_videos_per_prompt` is the number of views.  Text / image
         encoders are only invoked if they were injected; otherwise prompt_embeds / negative_prompt_embeds [Nv,77,768],
         ip_adapter_image_embeds [Nv,1024] and first_frame_latents [Nv,4,1,h,w] must be given."""
-        if eta != 0.0 or i2v_similarity_init is not None:
-            raise NotImplementedError("eta != 0 / i2v_similarity_init are unused by the released configuration")
+        if i2v_similarity_init is not None and self.free_init_enabled:
+            # the reference reads an undefined `strength` on this path (pipeline.py:997): it has no defined meaning
+            raise ValueError("i2v_similarity_init cannot be combined with FreeInit: the reference raises NameError there "
+                             "(pipeline.py:997); call disable_free_init() or drop i2v_similarity_init")
         dev = self.device
         nv = num_videos_per_prompt
-        if prompt_embeds is None or negative_prompt_embeds is None:
-            prompt_embeds, negative_prompt_embeds = self.encode_prompt(prompt, dev, nv, True, negative_prompt, prompt_embeds=prompt_embeds,
+        do_cfg = guidance_scale > 1.0                                                  # pipeline.py:746-748
+        if prompt_embeds is None or (do_cfg and negative_prompt_embeds is None):
+            prompt_embeds, negative_prompt_embeds = self.encode_prompt(prompt, dev, nv, do_cfg, negative_prompt, prompt_embeds=prompt_embeds,
                                                                        negative_prompt_embeds=negative_prompt_embeds, clip_skip=clip_skip)
         if ip_adapter_image_embeds is None:
             ip_adapter_image_embeds, _ = self.encode_image(ip_adapter_image, dev)
         if first_frame_latents is None:
             first_frame_latents = self.encode_latents((height, width), ip_adapter_image)
-        do_cfg = guidance_scale > 1.0
-        if not do_cfg:
-            raise NotImplementedError("the released sampler always runs with classifier-free guidance (guidance_scale 7.5)")
-        pe = torch.cat([negative_prompt_embeds, prompt_embeds]).to(dev, torch.float32)            # (uncond, cond): line 932
-        ie = torch.cat([torch.zeros_like(ip_adapter_image_embeds), ip_adapter_image_embeds]).to(dev, torch.float32)  # 537
+        cam = get_camera(nv).to(dev)
+        if do_cfg:
+            pe = torch.cat([negative_prompt_embeds, prompt_embeds]).to(dev, torch.float32)            # (uncond, cond): line 932
+            ie = torch.cat([torch.zeros_like(ip_adapter_image_embeds), ip_adapter_image_embeds]).to(dev, torch.float32)  # 537
+            cam = torch.cat([cam, cam])
+        else:                                                                          # pipeline.py:929-937, 1008-1018
+            pe = prompt_embeds.to(dev, torch.float32)
+            ie = ip_adapter_image_embeds.to(dev, torch.float32)
         first = first_frame_latents.to(dev, torch.float32).reshape(nv, -1, 1, height // 8, width // 8).contiguous()
         c = self.unet.config.in_channels
+        if i2v_similarity_init is not None:                                            # pipeline.py:940-946, 700-733
+            timesteps = self.scheduler.get_timesteps(num_inference_steps, i2v_similarity_init["strength"])
+            if latents is None:
+                latents = similarity_init_latents(first, num_frames - 1, int(timesteps[0]), i2v_similarity_init["origin_prob"],
+                                                  self.scheduler, generator)
         if latents is None:
-            latents = torch.randn(nv, c, num_frames - 1, height // 8, width // 8, generator=generator, device=dev, dtype=torch.float32)
+            latents = randn_tensor((nv, c, num_frames - 1, height // 8, width // 8), generator, dev)
         rest = latents.to(dev, torch.float32)
-        cam = get_camera(nv).to(dev)
-        cam2 = torch.cat([cam, cam])
         iters = self._free_init_num_iters if self.free_init_enabled else 1
         lat = torch.cat([first, rest], dim=2).contiguous()
         for it in range(iters):
             if self.free_init_enabled:
                 rest, timesteps = self._apply_free_init(lat[:, :, 1:].contiguous(), it, num_inference_steps, generator)
                 lat = torch.cat([first, rest], dim=2).contiguous()
-            else:
+            elif i2v_similarity_init is None:
                 timesteps = self.scheduler.set_timesteps(num_inference_steps)
             for i, t in enumerate(timesteps):
-                self.denoise_step(lat, int(t), pe, cam2, ie, first, guidance_scale, i2v_cond_time_zero, nv)
+                self.denoise_step(lat, int(t), pe, cam, ie, first, guidance_scale, i2v_cond_time_zero, nv, do_cfg, eta, generator)
                 if callback_on_step_end is not None:
                     res = callback_on_step_end(self, i, int(t), {"latents": lat})
                     lat = res.pop("latents", lat)

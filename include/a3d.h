@@ -15,6 +15,7 @@
  *   a3d_layer_norm      torch LayerNorm in BasicTransformerBlock
  *   a3d_conv_in/out     unet_motion_mv_model.py:767-768 (permute + conv_in) and 859-862 (conv_out + permute back)
  *   a3d_ddim_cfg_step   animatediff/pipelines/pipeline.py:1023-1031 (CFG combine + DDIMScheduler.step + frame-0 re-injection)
+ *   a3d_ddim_step       the same with eta > 0 (variance noise) and with guidance off (pipeline.py:580-590, 1008-1028)
  *   a3d_clip_preprocess .cpu() -> PIL -> CLIPImageProcessor -> patch embedding of the IP-Adapter image encoder at
  *                       custom/threestudio-animate3d/guidance/animatemv_guidance.py:546-555
  *   a3d_raster_*        diff_gaussian_rasterization._C.rasterize_gaussians / rasterize_gaussians_backward, called at
@@ -198,6 +199,19 @@ int a3d_cast_f32_f16(const float* x, void* y, int64_t n, void* stream);
  * latents/noise_pred: fp32 [BN(,x2), C, F, H, W]. */
 int a3d_ddim_cfg_step(float* latents, const float* noise_pred, const float* first_frame, int bn, int c, int f, int hw,
                       float guidance, float alpha_t, float alpha_prev, int uncond_first, void* stream);
+/* One DDIM update with eta (diffusers 0.28.0 DDIMScheduler.step(..., eta, variance_noise), reached through
+ * prepare_extra_step_kwargs at pipeline.py:580-590, 975, 1028), the optional CFG combine and frame-0 re-injection:
+ *   eps = noise_pred                       cfg_mode 0 (no guidance: noise_pred holds bn samples)
+ *   eps = e_u + g (e_c - e_u)              cfg_mode 1 ((uncond, cond) halves, pipeline.py:1023-1025)
+ *   eps = e_c + g (e_c - e_u)              cfg_mode 2 ((cond, uncond) halves, the SDS guidance order)
+ *   x0 = (x - sqrt(1-a_t) eps)/sqrt(a_t);  x' = sqrt(a_prev) x0 + dir_coef eps + std_dev z;  frame 0 of x' := first_frame.
+ * The caller computes dir_coef = sqrt(1 - a_prev - std_dev^2) and std_dev = eta sqrt((1-a_prev)/(1-a_t) (1 - a_t/a_prev))
+ * in fp32 (scheduler.py DDIMScheduler.step_coefficients).  variance_noise z: fp32 with the latents' shape [BN, C, F, H, W]
+ * (frame 0 included and ignored); it may be NULL only when std_dev == 0.  first_frame may be NULL (no re-injection).
+ * a3d_ddim_cfg_step(..., uncond_first) is this call with cfg_mode 1 / 2, dir_coef = sqrtf(1 - alpha_prev), std_dev 0. */
+int a3d_ddim_step(float* latents, const float* noise_pred, const float* first_frame, const float* variance_noise, int bn, int c,
+                  int f, int hw, int cfg_mode, float guidance, float alpha_t, float alpha_prev, float dir_coef, float std_dev,
+                  void* stream);
 
 /* ---------------------------------------------------------------- 4D-Gaussian rasterizer --------------------- */
 typedef struct a3d_raster_cam {
