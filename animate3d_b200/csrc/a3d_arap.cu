@@ -9,8 +9,9 @@
 
 namespace a3d {
 
-// K+1 nearest (squared distance ascending, ties by index) of every point among all points; the first one (the point itself)
-// is dropped -- pytorch3d.ops.knn_points(points, points, K=K+1)[..., 1:] as the reference uses it (util.py:79-82).
+// K+1 nearest (squared distance ascending, ties by index) of every point among all points; the first one is dropped -- the
+// lowest-index point coincident with i, i itself unless a lower-index copy exists (include/a3d.h) --
+// pytorch3d.ops.knn_points(points, points, K=K+1)[..., 1:] as the reference uses it (util.py:79-82).
 __global__ void __launch_bounds__(128) knn_kernel(const float* __restrict__ pts, int n, int K, int* __restrict__ nbr,
                                                   float* __restrict__ dist2) {
   __shared__ float sp[128 * 3];

@@ -340,21 +340,24 @@ int a3d_deform_backward(const a3d_deform_args* args, const float* dL_dmeans, con
                         void* scratch, size_t scratch_bytes, void* stream);
 
 /* ---------------------------------------------------------------- ARAP regulariser (SURVEY 8f-3) -------------- */
-/* K nearest neighbours of every point among the same points, self excluded, squared distances ascending, ties by index:
+/* Row i is positions 1..K of the order of all n points by (fp32 squared distance to point i, index), ascending:
  * pytorch3d.ops.knn_points(p, p, K=K+1)[..., 1:] as used by cal_connectivity_from_points
- * (custom/threestudio-animate3d/systems/util.py:79-82).  nbr [n,K] int32, dist2 [n,K]; K <= 12. */
+ * (custom/threestudio-animate3d/systems/util.py:79-82).  Position 0, the one dropped, is the lowest-index point coincident
+ * with i: that is i itself unless a lower-index point shares its position, in which case that point is dropped and i appears
+ * in its own row (after any other lower-index copies).  nbr [n,K] int32, dist2 [n,K]; 1 <= K <= 12, K < n. */
 int a3d_knn_graph(const float* points, int n, int K, int32_t* nbr, float* dist2, void* stream);
 /* cal_arap_error (util.py:183-215) with estimate_rotation (138-173) fused, all frames at once:
  *   err = sum_{t>=1} sum_{i in sample} sum_n w[i,n] | e_in(t) - R_i(t) e_in(0) |^2,   e_in(t) = x_t[i] - x_t[nbr[i,n]],
  * R_i(t) = the weighted Procrustes rotation of the node's frame-0 edges onto its frame-t edges (no gradient through R).
  * nodes [Nt,Nv,3]; nbr [Nv,K] (-1 = no edge); weight [Nv,K] or NULL (1 on existing edges, the reference's call);
- * sample [Ns] node indices or NULL (all nodes).  err: device scalar; grad [Nt,Nv,3] = d err / d nodes or NULL; both are
+ * sample [Ns] node indices or NULL (all nodes); an entry outside [0, Nv) contributes nothing (no energy, no gradient), and a
+ * repeated entry contributes once per occurrence.  err: device scalar; grad [Nt,Nv,3] = d err / d nodes or NULL; both are
  * overwritten.  scratch: caller-owned, of a3d_arap_scratch_bytes (NULL when that returned 0).  With deterministic 0 one
  * kernel accumulates energy and gradient with float atomics.  With deterministic 1 every sum runs in a fixed order: the
  * energy from per-(frame, sample) partials reduced by one CTA; the gradient from per-(frame, sample, edge) 3-vector records
  * gathered per node after a stable sort of the (target node, record) pairs, so repeated samples add in sample order and the
  * frame-0 gradient adds frames in order.  Checked on the CPU (tests/test_arap_cpu.py) and on the GPU against the reference
- * goldens (tests/test_arap_gpu.py). */
+ * goldens (tests/test_arap_gpu.py), and per element against the float64 oracle (tests/test_arap_abi_oracle_gpu.py). */
 int a3d_arap(const float* nodes, int Nt, int Nv, const int32_t* nbr, int K, const float* weight, const int32_t* sample, int Ns,
              int deterministic, float* err, float* grad, void* scratch, size_t scratch_bytes, void* stream);
 /* Scratch bytes a3d_arap needs for the same sizes (Ns of a NULL sample = Nv): 0 when deterministic is 0. */

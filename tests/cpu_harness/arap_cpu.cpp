@@ -7,13 +7,15 @@ using namespace a3d;
 
 extern "C" {
 
-// nodes [Nt,Nv,3]; nbr [Nv,K] (-1 = absent); weight [Nv,K] or NULL (1 on existing edges); sample [Ns] node indices.  grad [Nt,Nv,3] must be zeroed.
+// nodes [Nt,Nv,3]; nbr [Nv,K] (-1 = absent); weight [Nv,K] or NULL (1 on existing edges); sample [Ns] node indices (entries
+// outside [0, Nv) are skipped, like the kernels).  grad [Nt,Nv,3] must be zeroed.
 double arap_cpu(const float* nodes, int Nt, int Nv, const int* nbr, int K, const float* weight, const int* sample, int Ns,
                 float* grad) {
   double total = 0.0;
   for (int t = 1; t < Nt; ++t)
     for (int si = 0; si < Ns; ++si) {
       const int i = sample[si];
+      if (i < 0 || i >= Nv) continue;             // out-of-range sample entries contribute nothing (a3d.h)
       float e0[kArapMaxK][3], et[kArapMaxK][3], g0[kArapMaxK][3], gt[kArapMaxK][3], w[kArapMaxK];
       bool valid[kArapMaxK];
       arap_gather(nodes, Nv, nbr, K, weight, i, t, e0, et, w, valid);
