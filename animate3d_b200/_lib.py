@@ -67,6 +67,16 @@ class RasterArgs(C.Structure):
                 ("per_cam_geometry", C.c_int), ("scale_modifier", C.c_float), ("bg", C.c_float * 3), ("deterministic", C.c_int)]
 
 
+class SamplerStepArgs(C.Structure):
+    _fields_ = [("latents", C.c_void_p), ("noise_pred", C.c_void_p), ("first_frame", C.c_void_p), ("noise", C.c_void_p),
+                ("history_out", C.c_void_p), ("history_in", C.c_void_p),
+                ("bn", C.c_int), ("c", C.c_int), ("f", C.c_int), ("hw", C.c_int),
+                ("cfg_mode", C.c_int), ("guidance", C.c_float), ("kind", C.c_int), ("order", C.c_int),
+                ("alpha_s0", C.c_float), ("sigma_s0", C.c_float), ("c_x", C.c_float), ("c_m0", C.c_float),
+                ("inv_r0", C.c_float), ("c_d1", C.c_float),
+                ("sigma", C.c_float), ("dt", C.c_float), ("sigma_up", C.c_float)]
+
+
 _lib: Optional[C.CDLL] = None
 _inited = False
 

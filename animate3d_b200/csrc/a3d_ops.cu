@@ -806,6 +806,39 @@ __global__ void ddim_step_kernel(float* __restrict__ lat, const float* __restric
   lat[idx] = v;
 }
 
+// a3d_sampler_step: the per-element order of operations is written above the declaration in include/a3d.h.
+__global__ void sampler_step_kernel(a3d_sampler_step_args a) {
+  const int64_t n = (int64_t)a.bn * a.c * a.f * a.hw;
+  const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= n) return;
+  if (a.first_frame && (int)((idx / a.hw) % a.f) == 0) {
+    const int64_t sc = idx / ((int64_t)a.f * a.hw);  // (bn c)
+    a.latents[idx] = a.first_frame[sc * a.hw + idx % a.hw];
+    return;
+  }
+  float eps;
+  if (a.cfg_mode == 0) {
+    eps = a.noise_pred[idx];
+  } else {
+    const float e0 = a.noise_pred[idx], e1 = a.noise_pred[n + idx];
+    eps = a.cfg_mode == 1 ? (e0 + a.guidance * (e1 - e0)) : (e0 + a.guidance * (e0 - e1));
+  }
+  const float x = a.latents[idx];
+  float v;
+  if (a.kind == A3D_SAMPLER_DPMPP) {
+    const float m0 = (x - a.sigma_s0 * eps) / a.alpha_s0;
+    if (a.history_out) a.history_out[idx] = m0;
+    v = a.c_x * x - a.c_m0 * m0;
+    if (a.order == 2) v += a.c_d1 * (a.inv_r0 * (m0 - a.history_in[idx]));
+  } else {
+    const float x0 = x - a.sigma * eps;
+    const float d = (x - x0) / a.sigma;
+    v = x + d * a.dt;
+    if (a.sigma_up != 0.f) v += a.noise[idx] * a.sigma_up;
+  }
+  a.latents[idx] = v;
+}
+
 }  // namespace a3d
 
 using namespace a3d;
@@ -1054,4 +1087,25 @@ extern "C" int a3d_ddim_cfg_step(float* latents, const float* noise_pred, const 
                                  int hw, float guidance, float alpha_t, float alpha_prev, int uncond_first, void* stream) {
   return a3d_ddim_step(latents, noise_pred, first_frame, nullptr, bn, c, f, hw, uncond_first ? 1 : 2, guidance, alpha_t,
                        alpha_prev, sqrtf(1.f - alpha_prev), 0.f, stream);
+}
+
+extern "C" int a3d_sampler_step(const a3d_sampler_step_args* args, void* stream) {
+  if (!args) return fail(A3D_EINVAL, "a3d_sampler_step: args is NULL");
+  const a3d_sampler_step_args& a = *args;
+  if (a.kind != A3D_SAMPLER_DPMPP && a.kind != A3D_SAMPLER_EULER)
+    return fail(A3D_EINVAL, "a3d_sampler_step: kind %d is not A3D_SAMPLER_DPMPP (0) or A3D_SAMPLER_EULER (1)", a.kind);
+  if (a.cfg_mode < 0 || a.cfg_mode > 2) return fail(A3D_EINVAL, "a3d_sampler_step: cfg_mode %d is not 0, 1 or 2", a.cfg_mode);
+  if (a.kind == A3D_SAMPLER_DPMPP && a.order != 1 && a.order != 2)
+    return fail(A3D_EINVAL, "a3d_sampler_step: DPM-Solver++ order %d is not 1 or 2", a.order);
+  if (a.kind == A3D_SAMPLER_DPMPP && a.order == 2 && !a.history_in)
+    return fail(A3D_EINVAL, "a3d_sampler_step: order 2 needs history_in (the previous step's m0)");
+  if (a.kind == A3D_SAMPLER_EULER && a.sigma_up != 0.f && !a.noise)
+    return fail(A3D_EINVAL, "a3d_sampler_step: sigma_up %g needs noise", a.sigma_up);
+  if (!a.latents || !a.noise_pred) return fail(A3D_EINVAL, "a3d_sampler_step: latents and noise_pred are required");
+  const int64_t n = (int64_t)a.bn * a.c * a.f * a.hw;
+  if (n <= 0) return A3D_OK;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  sampler_step_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(a);
+  A3D_LAUNCH_CHECK();
+  return A3D_OK;
 }

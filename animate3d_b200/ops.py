@@ -227,6 +227,24 @@ def ddim_step(latents, noise_pred, first_frame, variance_noise, bn, c, f, hw, cf
     return latents
 
 
+def sampler_step(latents, noise_pred, first_frame, bn, c, f, hw, cfg_mode, guidance, step, noise=None, history_out=None,
+                 history_in=None):
+    """a3d_sampler_step with the scalars of `step` (scheduler.SolverStep): DPM-Solver++ writes m0 into `history_out` and reads
+    the previous m0 from `history_in` at order 2; Euler-ancestral reads `noise` (sigma_up != 0).  cfg_mode as ddim_step."""
+    lib = L.load()
+    a = L.SamplerStepArgs()
+    a.latents, a.noise_pred, a.first_frame = latents.data_ptr(), noise_pred.data_ptr(), L.ptr(first_frame)
+    a.noise, a.history_out, a.history_in = L.ptr(noise), L.ptr(history_out), L.ptr(history_in)
+    a.bn, a.c, a.f, a.hw = bn, c, f, hw
+    a.cfg_mode, a.guidance = int(cfg_mode), guidance
+    a.kind, a.order = step.kind, step.order
+    a.alpha_s0, a.sigma_s0, a.c_x, a.c_m0, a.inv_r0, a.c_d1 = (step.alpha_s0, step.sigma_s0, step.c_x, step.c_m0, step.inv_r0,
+                                                            step.c_d1)
+    a.sigma, a.dt, a.sigma_up = step.sigma, step.dt, step.sigma_up
+    _enqueued(lib.a3d_sampler_step(C.byref(a), L.stream_ptr()))
+    return latents
+
+
 def clip_resize_tables(h: int, w: int):
     """Host-built Pillow bicubic tables of the CLIP resize of an h x w image: (resize_h, resize_w, (bounds_y, coeffs_y,
     ksize_y), (bounds_x, coeffs_x, ksize_x)) with int32 CPU tensors."""

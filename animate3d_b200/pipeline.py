@@ -15,7 +15,7 @@ from typing import Callable, List, Optional
 import torch
 
 from . import ops
-from .scheduler import DDIMScheduler
+from .scheduler import SOLVER_SCHEDULERS, DDIMScheduler, DPMSolverMultistepScheduler, as_engine_scheduler
 from .unet import MVUNetMotionModel
 
 
@@ -90,12 +90,13 @@ def randn_tensor(shape, generator: Optional[torch.Generator], device) -> torch.T
     return torch.randn(shape, generator=generator, device=rand_device, dtype=torch.float32).to(device)
 
 
-def similarity_init_latents(first_frame_latents: torch.Tensor, num_frames: int, t_first: int, origin_prob: float,
-                            scheduler: DDIMScheduler, generator: Optional[torch.Generator]) -> torch.Tensor:
+def similarity_init_latents(first_frame_latents: torch.Tensor, num_frames: int, t_first, origin_prob: float,
+                            scheduler, generator: Optional[torch.Generator]) -> torch.Tensor:
     """`i2v_similarity_init` latents of frames 1.. (reference prepare_latents, pipeline.py:707-724): each pixel of each
     frame is the first-frame latent with probability `origin_prob`, else that latent noised to the first timestep.  Draws
     the mask (uniform, [Nv, 1, num_frames, h, w]) and then the noise ([Nv, C, num_frames, h, w]) with `generator`, on its
-    device.  No init_noise_sigma scaling (pipeline.py:727-729; it is 1)."""
+    device.  `t_first` is a schedule entry (an int, or a 0-dim tensor of the scheduler's timesteps).  No init_noise_sigma
+    scaling (pipeline.py:727-729)."""
     nv, c, _, h, w = first_frame_latents.shape
     dev = first_frame_latents.device
     rand_device = generator.device if generator is not None else dev
@@ -103,13 +104,16 @@ def similarity_init_latents(first_frame_latents: torch.Tensor, num_frames: int, 
     mask = (mask < origin_prob).float()
     noise = randn_tensor((nv, c, num_frames, h, w), generator, dev)
     cond = first_frame_latents.repeat_interleave(num_frames, dim=2)
-    noised = scheduler.add_noise(cond, noise, torch.full((nv,), int(t_first), dtype=torch.long))
+    noised = scheduler.add_noise(cond, noise, torch.as_tensor(t_first).reshape(1).repeat(nv))
     return mask * cond + (1 - mask) * noised
 
 
 class AnimateDiffMVI2VPipeline:
     """`AnimationPipeline` of north_star == this class (alias below).  Constructor keeps the reference's argument names
-    (pipeline.py:308-325); everything except `unet` and `scheduler` is optional."""
+    (pipeline.py:308-325); everything except `unet` and `scheduler` is optional.  `scheduler` is a DDIMScheduler (the
+    default), DPMSolverMultistepScheduler, EulerDiscreteScheduler or EulerAncestralDiscreteScheduler of scheduler.py, or
+    diffusers' class of one of those names (rebuilt from its config); it may be replaced at any time, as with the reference:
+    `pipe.scheduler = DPMSolverMultistepScheduler.from_config(pipe.scheduler.config)`."""
 
     def __init__(self, vae=None, text_encoder=None, tokenizer=None, unet: MVUNetMotionModel = None, motion_adapter=None,
                  scheduler: DDIMScheduler = None, feature_extractor=None, image_encoder=None):
@@ -121,6 +125,14 @@ class AnimateDiffMVI2VPipeline:
         self.free_init_enabled = False
         self._free_init_num_iters = 1
         self.device = unet.device
+
+    @property
+    def scheduler(self):
+        return self._scheduler
+
+    @scheduler.setter
+    def scheduler(self, scheduler):
+        self._scheduler = as_engine_scheduler(scheduler)
 
     def to(self, device):
         return self
@@ -296,9 +308,16 @@ class AnimateDiffMVI2VPipeline:
             self._free_init_initial_noise = latents.detach().clone()
         else:
             order, ds, dt = self._fi
-            a = float(self.scheduler.alphas_cumprod[self.scheduler.num_train_timesteps - 1])
-            z_T = math.sqrt(a) * latents + math.sqrt(1 - a) * self._free_init_initial_noise
-            z_rand = torch.randn(latents.shape, generator=generator, device=latents.device, dtype=torch.float32)
+            if isinstance(self.scheduler, SOLVER_SCHEDULERS):
+                # the scheduler's own add_noise at t = 999, on the schedule of the previous iteration; draws on the
+                # generator's device (diffusers' randn_tensor)
+                t_T = torch.full((latents.shape[0],), self.scheduler.num_train_timesteps - 1, dtype=torch.long)
+                z_T = self.scheduler.add_noise(latents, self._free_init_initial_noise, t_T)
+                z_rand = randn_tensor(latents.shape, generator, latents.device)
+            else:
+                a = float(self.scheduler.alphas_cumprod[self.scheduler.num_train_timesteps - 1])
+                z_T = math.sqrt(a) * latents + math.sqrt(1 - a) * self._free_init_initial_noise
+                z_rand = torch.randn(latents.shape, generator=generator, device=latents.device, dtype=torch.float32)
             lpf = _butterworth_lpf(latents.shape, order, ds, dt, latents.device)
             dims = (-3, -2, -1)
             zf = torch.fft.fftshift(torch.fft.fftn(z_T, dim=dims), dim=dims)
@@ -343,6 +362,10 @@ class AnimateDiffMVI2VPipeline:
             ie = ip_adapter_image_embeds.to(dev, torch.float32)
         first = first_frame_latents.to(dev, torch.float32).reshape(nv, -1, 1, height // 8, width // 8).contiguous()
         c = self.unet.config.in_channels
+        if isinstance(self.scheduler, SOLVER_SCHEDULERS):
+            lat = self._solver_loop(first, latents, num_frames, num_inference_steps, pe, cam, ie, guidance_scale,
+                                    i2v_cond_time_zero, nv, do_cfg, generator, i2v_similarity_init, callback_on_step_end)
+            return self._output(lat, output_type, return_dict)
         if i2v_similarity_init is not None:                                            # pipeline.py:940-946, 700-733
             timesteps = self.scheduler.get_timesteps(num_inference_steps, i2v_similarity_init["strength"])
             if latents is None:
@@ -364,6 +387,9 @@ class AnimateDiffMVI2VPipeline:
                 if callback_on_step_end is not None:
                     res = callback_on_step_end(self, i, int(t), {"latents": lat})
                     lat = res.pop("latents", lat)
+        return self._output(lat, output_type, return_dict)
+
+    def _output(self, lat, output_type, return_dict):
         if output_type == "latent":
             video = lat
         else:
@@ -372,6 +398,47 @@ class AnimateDiffMVI2VPipeline:
                                  "(pipeline.py:1049-1056)")
             video = tensor2vid(self.decode_latents(lat), getattr(self, "image_processor", None), output_type=output_type)
         return AnimateDiffMVI2VPipelineOutput(frames=video) if return_dict else (video,)
+
+    def _solver_loop(self, first, latents, num_frames, num_inference_steps, pe, cam, ie, guidance_scale, i2v_cond_time_zero,
+                     nv, do_cfg, generator, similarity, callback_on_step_end):
+        """The sampling loop of pipeline.py:939-1047 for DPM-Solver++ and the Euler schedulers: scale_model_input on the UNet
+        input, the schedule's float timestep into the UNet, then one a3d_sampler_step (CFG combine, solver update,
+        frame-0 re-injection).  The Euler schedulers draw one normal sample of the latents' shape per step after the UNet
+        call, as diffusers' step does; DPM-Solver++ keeps each step's m0 in one of two device buffers that swap roles."""
+        sched, dev = self.scheduler, self.device
+        c, h, w = first.shape[1], first.shape[3], first.shape[4]
+        if similarity is not None:                                                     # pipeline.py:943-946, 707-729
+            timesteps = sched.get_timesteps(num_inference_steps, similarity["strength"])
+            if latents is None:
+                latents = similarity_init_latents(first, num_frames - 1, timesteps[0], similarity["origin_prob"], sched,
+                                                  generator)
+            rest = latents.to(dev, torch.float32)
+        else:                                                                          # pipeline.py:941, 700-732
+            timesteps = sched.set_timesteps(num_inference_steps)
+            if latents is None:
+                latents = randn_tensor((nv, c, num_frames - 1, h, w), generator, dev)
+            rest = latents.to(dev, torch.float32) * sched.init_noise_sigma
+        lat = torch.cat([first, rest], dim=2).contiguous()
+        dpm = isinstance(sched, DPMSolverMultistepScheduler)
+        hist = (torch.empty_like(lat), torch.empty_like(lat)) if dpm else (None, None)
+        for it in range(self._free_init_num_iters if self.free_init_enabled else 1):
+            if self.free_init_enabled:
+                rest, timesteps = self._apply_free_init(lat[:, :, 1:].contiguous(), it, num_inference_steps, generator)
+                lat = torch.cat([first, rest], dim=2).contiguous()
+            for i, t in enumerate(timesteps):
+                x = torch.cat([lat, lat], 0) if do_cfg else lat
+                x = sched.scale_model_input(x, t)
+                noise_pred = self.unet(x, float(t), pe, camera=cam, added_cond_kwargs={"image_embeds": ie}, num_views=nv,
+                                       i2v_cond_time_zero=i2v_cond_time_zero).sample
+                step = sched.next_step(t)
+                z = None if dpm else randn_tensor(lat.shape, generator, dev)
+                ops.sampler_step(lat, noise_pred.contiguous(), first, nv, c, num_frames, h * w, 1 if do_cfg else 0,
+                                 guidance_scale, step, noise=z if step.sigma_up != 0.0 else None, history_out=hist[i % 2],
+                                 history_in=hist[(i + 1) % 2] if step.order == 2 else None)
+                if callback_on_step_end is not None:
+                    res = callback_on_step_end(self, i, t.item(), {"latents": lat})
+                    lat = res.pop("latents", lat)
+        return lat
 
 
 AnimationPipeline = AnimateDiffMVI2VPipeline   # name used by BASELINE.json's north_star

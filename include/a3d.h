@@ -213,6 +213,44 @@ int a3d_ddim_step(float* latents, const float* noise_pred, const float* first_fr
                   int f, int hw, int cfg_mode, float guidance, float alpha_t, float alpha_prev, float dir_coef, float std_dev,
                   void* stream);
 
+/* One step of the DPM-Solver++ (orders 1 and 2) or Euler / Euler-ancestral scheduler (diffusers 0.28.0
+ * DPMSolverMultistepScheduler / EulerDiscreteScheduler / EulerAncestralDiscreteScheduler .step, epsilon prediction) with the
+ * CFG combine of a3d_ddim_step (`cfg_mode` 0 / 1 / 2) and the frame-0 re-injection.  One thread per latent element; the
+ * caller computes every scalar in fp32 in diffusers' order (scheduler.py `next_step`).  Per element, in this fp32 order:
+ *   eps = cfg(noise_pred)                                  as a3d_ddim_step
+ *   A3D_SAMPLER_DPMPP:
+ *     m0 = (x - sigma_s0 * eps) / alpha_s0                 sigma_s0 = sigma~ = sigma alpha of the current sigma
+ *     history_out[i] = m0                                  when history_out is non-NULL
+ *     x' = c_x * x - c_m0 * m0                             c_x = sigma~_t / sigma~_s0, c_m0 = alpha_t (e^-h - 1)
+ *     order 2: x' = x' + c_d1 * (inv_r0 * (m0 - m1))       m1 = history_in[i], the previous step's m0;
+ *                                                          c_d1 = -0.5 alpha_t (e^-h - 1) (midpoint) or
+ *                                                          alpha_t ((e^-h - 1)/h + 1) (heun)
+ *     (sigma_t = 0 on the last step gives c_x = 0, c_m0 = -1: x' = m0 exactly)
+ *   A3D_SAMPLER_EULER:
+ *     x0 = x - sigma * eps;  d = (x - x0) / sigma;  x' = x + d * dt
+ *     x' = x' + noise[i] * sigma_up                        when sigma_up != 0 (ancestral: dt = sigma_down - sigma)
+ *   frame 0 of x' := first_frame when first_frame is non-NULL (nothing else is read or written for frame 0).
+ * latents, history_out, history_in, noise: fp32 [BN, C, F, H, W]; noise_pred [BN(,x2), C, F, H, W].  The history buffers are
+ * caller-owned and must not alias each other: the caller swaps them between steps.  A3D_EINVAL: a bad kind or cfg_mode,
+ * order not 1 or 2, order 2 without history_in, or sigma_up != 0 without noise. */
+typedef struct a3d_sampler_step_args {
+  float* latents;
+  const float* noise_pred;
+  const float* first_frame;   /* [BN, C, 1, H, W] or NULL */
+  const float* noise;         /* Euler-ancestral z, or NULL */
+  float* history_out;         /* DPM-Solver++: m0 of this step, or NULL */
+  const float* history_in;    /* DPM-Solver++ order 2: m1 */
+  int bn, c, f, hw;
+  int cfg_mode;
+  float guidance;
+  int kind;                   /* A3D_SAMPLER_DPMPP or A3D_SAMPLER_EULER */
+  int order;                  /* DPM-Solver++: 1 or 2 */
+  float alpha_s0, sigma_s0, c_x, c_m0, inv_r0, c_d1;   /* DPM-Solver++ */
+  float sigma, dt, sigma_up;                           /* Euler */
+} a3d_sampler_step_args;
+enum { A3D_SAMPLER_DPMPP = 0, A3D_SAMPLER_EULER = 1 };
+int a3d_sampler_step(const a3d_sampler_step_args* args, void* stream);
+
 /* ---------------------------------------------------------------- 4D-Gaussian rasterizer --------------------- */
 typedef struct a3d_raster_cam {
   float viewmatrix[16];   /* row-vector convention, as passed by threestudio/utils/ops.py:344-359 */
