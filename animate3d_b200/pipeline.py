@@ -84,9 +84,48 @@ def _butterworth_lpf(shape, order=4, d_s=0.25, d_t=0.25, device="cpu"):
     return 1.0 / (1.0 + (d2 / d_s ** 2) ** order)
 
 
-def randn_tensor(shape, generator: Optional[torch.Generator], device) -> torch.Tensor:
-    """diffusers' randn_tensor for one generator: fp32 normal noise drawn on the generator's device (so a CPU generator
-    gives the same stream whatever `device` is), then moved to `device`."""
+FREE_INIT_METHODS = ("butterworth", "gaussian", "ideal")
+
+
+def free_init_filter(shape, method="butterworth", order=4, d_s=0.25, d_t=0.25, device="cpu") -> torch.Tensor:
+    """FreeInit's low-pass filter over the last three dimensions (T, H, W) of `shape`, as a float32 [T, H, W] tensor
+    (diffusers 0.28.0 FreeInitMixin._get_free_init_freq_filter, which loops over the entries).  With
+    d² = ((d_s/d_t)(2t/T − 1))² + (2h/H − 1)² + (2w/W − 1)²: butterworth 1 / (1 + (d²/d_s²)^order), gaussian
+    exp(−d² / (2 d_s²)), ideal 1 where d² <= 2 d_s (diffusers compares d² with 2 d_s, not d_s²) and 0 elsewhere; all
+    zeros when d_s or d_t is 0.  diffusers evaluates every entry in Python floats and stores it in float32: the gaussian
+    and ideal filters are evaluated the same way, in float64 rounded once, while the butterworth filter keeps its float32
+    arithmetic (`_butterworth_lpf`), a few ulps from diffusers'."""
+    if method not in FREE_INIT_METHODS:
+        raise NotImplementedError("`filter_type` must be one of gaussian, butterworth or ideal")
+    T, H, W = shape[-3], shape[-2], shape[-1]
+    if d_s == 0 or d_t == 0:
+        return torch.zeros((T, H, W), device=device)
+    if method == "butterworth":
+        return _butterworth_lpf(shape, order, d_s, d_t, device)
+    t = torch.arange(T, device=device, dtype=torch.float64)[:, None, None]
+    h = torch.arange(H, device=device, dtype=torch.float64)[None, :, None]
+    w = torch.arange(W, device=device, dtype=torch.float64)[None, None, :]
+    d2 = ((d_s / d_t) * (2 * t / T - 1)) ** 2 + (2 * h / H - 1) ** 2 + (2 * w / W - 1) ** 2
+    mask = torch.exp(-1 / (2 * d_s ** 2) * d2) if method == "gaussian" else (d2 <= d_s * 2).double()
+    return mask.float()
+
+
+def randn_tensor(shape, generator, device) -> torch.Tensor:
+    """diffusers' randn_tensor: fp32 normal noise of `shape` on `device`.  `generator` is None, one torch.Generator, or a
+    list of them, one per item along dim 0 (a list of one is that one generator).  Every draw runs on its generator's
+    device, so a CPU generator gives the same stream whatever `device` is, and the result moves to `device`; a CUDA
+    generator cannot fill a tensor on another device type (ValueError, as diffusers raises)."""
+    device = torch.device(device)
+    gens = generator if isinstance(generator, list) else [generator]
+    for g in gens:
+        if g is not None and g.device.type == "cuda" and device.type != "cuda":
+            raise ValueError(f"cannot draw a {device} tensor from a {g.device} generator")
+    if isinstance(generator, list) and len(generator) == 1:
+        generator = generator[0]
+    if isinstance(generator, list):
+        item = (1,) + tuple(shape[1:])
+        return torch.cat([torch.randn(item, generator=generator[i], device=generator[i].device,
+                                      dtype=torch.float32).to(device) for i in range(shape[0])], 0)
     rand_device = generator.device if generator is not None else device
     return torch.randn(shape, generator=generator, device=rand_device, dtype=torch.float32).to(device)
 
@@ -97,7 +136,11 @@ def similarity_init_latents(first_frame_latents: torch.Tensor, num_frames: int, 
     frame is the first-frame latent with probability `origin_prob`, else that latent noised to the first timestep.  Draws
     the mask (uniform, [Nv, 1, num_frames, h, w]) and then the noise ([Nv, C, num_frames, h, w]) with `generator`, on its
     device.  `t_first` is a schedule entry (an int, or a 0-dim tensor of the scheduler's timesteps).  No init_noise_sigma
-    scaling (pipeline.py:727-729)."""
+    scaling (pipeline.py:727-729).  A list of generators raises ValueError: the reference draws the mask with torch.rand,
+    which takes one generator, and fails there with TypeError."""
+    if isinstance(generator, list):
+        raise ValueError("i2v_similarity_init draws its mask with one generator (torch.rand): pass a single "
+                         "torch.Generator, not a list")
     nv, c, _, h, w = first_frame_latents.shape
     dev = first_frame_latents.device
     rand_device = generator.device if generator is not None else dev
@@ -116,6 +159,10 @@ class AnimateDiffMVI2VPipeline:
     LMSDiscreteScheduler of scheduler.py, or diffusers' class of one of those names (rebuilt from its config); it may be
     replaced at any time, as with the reference:
     `pipe.scheduler = DPMSolverMultistepScheduler.from_config(pipe.scheduler.config)`."""
+
+    _free_init_method = "butterworth"
+    _free_init_use_fast_sampling = False
+    _free_init_filter = None                    # (key, filter) of the last filter built: one per (shape, options, device)
 
     def __init__(self, vae=None, text_encoder=None, tokenizer=None, unet: MVUNetMotionModel = None, motion_adapter=None,
                  scheduler: DDIMScheduler = None, feature_extractor=None, image_encoder=None):
@@ -141,9 +188,15 @@ class AnimateDiffMVI2VPipeline:
 
     def enable_free_init(self, num_iters: int = 3, use_fast_sampling: bool = False, method: str = "butterworth", order: int = 4,
                          spatial_stop_frequency: float = 0.25, temporal_stop_frequency: float = 0.25):
-        if method != "butterworth" or use_fast_sampling:
-            raise NotImplementedError("released configuration only: butterworth, no fast sampling (inference.py:244-245)")
+        """diffusers' FreeInitMixin.enable_free_init: `num_iters` sampling passes, each after the first restarting from
+        the low frequencies of the previous result (filter `method`: butterworth, gaussian or ideal, see
+        `free_init_filter`) and the high frequencies of fresh noise.  With `use_fast_sampling` (coarse-to-fine), pass i
+        of n runs max(1, int(num_inference_steps / n * (i + 1))) steps.  An unknown `method` raises NotImplementedError
+        here; diffusers raises it at the second pass."""
+        if method not in FREE_INIT_METHODS:
+            raise NotImplementedError("`filter_type` must be one of gaussian, butterworth or ideal")
         self.free_init_enabled, self._free_init_num_iters = True, num_iters
+        self._free_init_use_fast_sampling, self._free_init_method = bool(use_fast_sampling), method
         self._fi = (order, spatial_stop_frequency, temporal_stop_frequency)
 
     def disable_free_init(self):
@@ -304,28 +357,38 @@ class AnimateDiffMVI2VPipeline:
         return latents_local
 
     # -------------------------------------------------------------------------------------------- full sampler
+    def _free_init_steps(self, it: int, num_inference_steps: int) -> int:
+        """Steps of FreeInit pass `it`: all of them, or with coarse-to-fine sampling diffusers' share of them."""
+        if not self._free_init_use_fast_sampling:
+            return num_inference_steps
+        return max(1, int(num_inference_steps / self._free_init_num_iters * (it + 1)))
+
     def _apply_free_init(self, latents, it, num_inference_steps, generator):
-        """FreeInitMixin._apply_free_init on frames 1.. (pipeline.py:990-992; SURVEY Appendix B.11)."""
+        """FreeInitMixin._apply_free_init on frames 1.. (pipeline.py:990-992; SURVEY Appendix B.11): keep the first pass's
+        noise, or mix the previous result noised to t = 999 with fresh noise through the low-pass filter; then set this
+        pass's schedule, which restarts the scheduler's step counter and history."""
         if it == 0:
             self._free_init_initial_noise = latents.detach().clone()
         else:
             order, ds, dt = self._fi
             if isinstance(self.scheduler, SOLVER_SCHEDULERS):
-                # the scheduler's own add_noise at t = 999, on the schedule of the previous iteration; draws on the
-                # generator's device (diffusers' randn_tensor)
+                # the scheduler's own add_noise at t = 999, on the schedule of the previous iteration
                 t_T = torch.full((latents.shape[0],), self.scheduler.num_train_timesteps - 1, dtype=torch.long)
                 z_T = self.scheduler.add_noise(latents, self._free_init_initial_noise, t_T)
-                z_rand = randn_tensor(latents.shape, generator, latents.device)
             else:
                 a = float(self.scheduler.alphas_cumprod[self.scheduler.num_train_timesteps - 1])
                 z_T = math.sqrt(a) * latents + math.sqrt(1 - a) * self._free_init_initial_noise
-                z_rand = torch.randn(latents.shape, generator=generator, device=latents.device, dtype=torch.float32)
-            lpf = _butterworth_lpf(latents.shape, order, ds, dt, latents.device)
+            z_rand = randn_tensor(latents.shape, generator, latents.device)
+            key = (tuple(latents.shape[-3:]), self._free_init_method, order, ds, dt, latents.device)
+            if self._free_init_filter is None or self._free_init_filter[0] != key:
+                self._free_init_filter = (key, free_init_filter(latents.shape, self._free_init_method, order, ds, dt,
+                                                                latents.device))
+            lpf = self._free_init_filter[1]
             dims = (-3, -2, -1)
             zf = torch.fft.fftshift(torch.fft.fftn(z_T, dim=dims), dim=dims)
             rf = torch.fft.fftshift(torch.fft.fftn(z_rand, dim=dims), dim=dims)
             latents = torch.fft.ifftn(torch.fft.ifftshift(zf * lpf + rf * (1 - lpf), dim=dims), dim=dims).real.contiguous()
-        self.scheduler.set_timesteps(num_inference_steps)
+        self.scheduler.set_timesteps(self._free_init_steps(it, num_inference_steps))
         return latents, self.scheduler.timesteps
 
     @torch.no_grad()
@@ -339,7 +402,11 @@ class AnimateDiffMVI2VPipeline:
                  i2v_similarity_init=None, first_frame_latents: Optional[torch.Tensor] = None):
         """Argument names follow pipeline.py:760-786.  `num_videos_per_prompt` is the number of views.  Text / image
         encoders are only invoked if they were injected; otherwise prompt_embeds / negative_prompt_embeds [Nv,77,768],
-        ip_adapter_image_embeds [Nv,1024] and first_frame_latents [Nv,4,1,h,w] must be given."""
+        ip_adapter_image_embeds [Nv,1024] and first_frame_latents [Nv,4,1,h,w] must be given.  `generator` is one
+        torch.Generator or a list of one per view, from which every draw of that view comes (`randn_tensor`)."""
+        if isinstance(generator, list) and len(generator) != num_videos_per_prompt:     # prepare_latents, 699-703
+            raise ValueError(f"generator is a list of {len(generator)} generators, but the call samples "
+                             f"{num_videos_per_prompt} views (num_videos_per_prompt): pass one generator per view")
         if i2v_similarity_init is not None and self.free_init_enabled:
             # the reference reads an undefined `strength` on this path (pipeline.py:997): it has no defined meaning
             raise ValueError("i2v_similarity_init cannot be combined with FreeInit: the reference raises NameError there "

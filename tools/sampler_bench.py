@@ -1,7 +1,8 @@
 """Sampling time per scheduler: one full latent-output `__call__` at 4 views x 16 frames x 32^2 latents with CFG, random
 weights and FreeInit off, for DDIM 25 steps, DPM-Solver++ 25 and 15 steps, Euler 25 steps, PNDM 25 steps with and without
-its PRK steps and LMS 25 steps (wall clock ending on a device synchronise, after one untimed warm-up call of each; each
-leg also reports how many times the last call ran the UNet); then the step kernels alone, a3d_sampler_step (DPM-Solver++
+its PRK steps and LMS 25 steps, then DDIM 25 steps with three butterworth FreeInit iterations, with and without
+coarse-to-fine sampling (wall clock ending on a device synchronise, after one untimed warm-up call of each; each leg also
+reports how many times the last call ran the UNet); then the step kernels alone, a3d_sampler_step (DPM-Solver++
 order 2 and Euler-ancestral) and a3d_multistep_step (four-term PLMS and LMS, and a PRK sub-step) against a3d_ddim_step,
 timed with CUDA events over many launches.  Prints one JSON line with the card's name and power limit.
 `python tools/sampler_bench.py [--reps 3] [--out DIR]`."""
@@ -34,8 +35,10 @@ def card():
     return q
 
 
-def time_calls(pipe, sched, steps, reps, cond):
+def time_calls(pipe, sched, steps, reps, cond, free_init=None):
     pipe.scheduler = sched
+    if free_init is not None:
+        pipe.enable_free_init(**free_init)
     forward, unet_calls = pipe.unet.forward, [0]
 
     def counted(*a, **k):
@@ -56,6 +59,7 @@ def time_calls(pipe, sched, steps, reps, cond):
         torch.cuda.synchronize()
         out.append(time.perf_counter() - t0)
     del pipe.unet.forward
+    pipe.disable_free_init()
     return out, unet_calls[0]
 
 
@@ -92,10 +96,12 @@ def main():
             ("Euler", 25, lambda: S.EulerDiscreteScheduler.from_config(ddim_cfg)),
             ("PNDM (PLMS only)", 25, lambda: S.PNDMScheduler.from_config(ddim_cfg, skip_prk_steps=True)),
             ("PNDM (PRK + PLMS)", 25, lambda: S.PNDMScheduler.from_config(ddim_cfg)),
-            ("LMS", 25, lambda: S.LMSDiscreteScheduler.from_config(ddim_cfg))]
+            ("LMS", 25, lambda: S.LMSDiscreteScheduler.from_config(ddim_cfg)),
+            ("DDIM, FreeInit 3", 25, lambda: S.DDIMScheduler(), dict(num_iters=3)),
+            ("DDIM, FreeInit 3, coarse-to-fine", 25, lambda: S.DDIMScheduler(), dict(num_iters=3, use_fast_sampling=True))]
     calls = []
-    for name, steps, make in runs:
-        secs, unet_calls = time_calls(pipe, make(), steps, args.reps, cond)
+    for name, steps, make, *free_init in runs:
+        secs, unet_calls = time_calls(pipe, make(), steps, args.reps, cond, *free_init)
         med = sorted(secs)[len(secs) // 2]
         calls.append(dict(scheduler=name, steps=steps, unet_calls=unet_calls, seconds=[round(s, 3) for s in secs],
                           median_s=round(med, 3), ms_per_step=round(1e3 * med / steps, 1),
@@ -133,7 +139,7 @@ def main():
         "a3d_multistep_step prk sub-step 2": time_kernel(multistep(prk2)),
         "a3d_multistep_step lms 4 terms": time_kernel(multistep(lms4)),
     }
-    result = dict(card=card(), workload=f"{NV} views x {NF} frames x {LAT}^2 latents, CFG 7.5, FreeInit off, random weights",
+    result = dict(card=card(), workload=f"{NV} views x {NF} frames x {LAT}^2 latents, CFG 7.5, random weights",
                   calls=calls, kernel_us={k: round(v, 2) for k, v in kernels.items()})
     print(json.dumps(result), flush=True)
     if args.out:
