@@ -490,3 +490,26 @@ extern "C" int a3d_raster_binning_tap(const void* workspace, int P, int H, int W
   if (ranges_out) A3D_CUDA_CHECK(cudaMemcpyAsync(ranges_out, ws.ranges, (size_t)l.total_tiles * 8, cudaMemcpyDeviceToDevice, st));
   return A3D_OK;
 }
+
+extern "C" int a3d_raster_state_tap(const void* workspace, int P, int H, int W, int num_cams, int64_t max_rendered, int cam,
+                                    float* xy_out, float* conic_opac_out, float* rgb_depth_out, uint8_t* clamped_out,
+                                    uint32_t* n_contrib_out, float* final_T_out, void* stream) {
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  if (!workspace || P <= 0 || H <= 0 || W <= 0 || num_cams <= 0 || cam < 0 || cam >= num_cams)
+    return fail(A3D_EINVAL, "a3d_raster_state_tap: bad arguments");
+  const RasterLayout l = raster_layout(const_cast<void*>(workspace), P, H, W, num_cams, max_rendered);
+  const RasterLayout lr = raster_layout(const_cast<void*>(workspace), P, H, W, num_cams, max_rendered, true);
+  // the per-(camera, gaussian) records are carved before anything the RGBA8 layout leaves out, so one tap serves both
+  if (l.ws.xy != lr.ws.xy || l.ws.conic_opac != lr.ws.conic_opac || l.ws.rgb_depth != lr.ws.rgb_depth || l.ws.clamped != lr.ws.clamped)
+    return fail(A3D_EINVAL, "a3d_raster_state_tap: record offsets differ between the forward and RGBA8 workspaces");
+  const RasterWs& ws = l.ws;
+  const size_t n = (size_t)P, c0 = (size_t)cam * P, hw = (size_t)H * W;
+  if (xy_out) A3D_CUDA_CHECK(cudaMemcpyAsync(xy_out, ws.xy + c0, n * sizeof(float2), cudaMemcpyDeviceToDevice, st));
+  if (conic_opac_out) A3D_CUDA_CHECK(cudaMemcpyAsync(conic_opac_out, ws.conic_opac + c0, n * sizeof(float4), cudaMemcpyDeviceToDevice, st));
+  if (rgb_depth_out) A3D_CUDA_CHECK(cudaMemcpyAsync(rgb_depth_out, ws.rgb_depth + c0, n * sizeof(float4), cudaMemcpyDeviceToDevice, st));
+  if (clamped_out) A3D_CUDA_CHECK(cudaMemcpyAsync(clamped_out, ws.clamped + c0, n, cudaMemcpyDeviceToDevice, st));
+  if (n_contrib_out)
+    A3D_CUDA_CHECK(cudaMemcpyAsync(n_contrib_out, ws.n_contrib + (size_t)cam * hw, hw * 4, cudaMemcpyDeviceToDevice, st));
+  if (final_T_out) A3D_CUDA_CHECK(cudaMemcpyAsync(final_T_out, ws.final_T + (size_t)cam * hw, hw * 4, cudaMemcpyDeviceToDevice, st));
+  return A3D_OK;
+}

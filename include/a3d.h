@@ -376,6 +376,16 @@ int a3d_raster_backward(const a3d_raster_args* args, const float* dL_dcolor, con
 /* debug/parity taps of the binning stage for one camera: sorted keys [n] uint64, point_list [n] uint32, ranges [tiles] uint2 */
 int a3d_raster_binning_tap(const void* workspace, int P, int H, int W, int num_cams, int64_t max_rendered, int cam,
                            uint64_t* keys_out, uint32_t* point_list_out, uint32_t* ranges_out, void* stream);
+/* debug/parity tap of the render state of camera `cam` (same leading arguments as a3d_raster_binning_tap): the per-(camera,
+ * gaussian) records the tile render consumes -- xy [P,2] pixel centre, conic_opac [P,4] (conic a, b, c, opacity),
+ * rgb_depth [P,4], clamped [P] (bit ch: SH colour channel ch clamped at 0) -- and the per-pixel backward state
+ * n_contrib [H,W] (1-based list position of the last contributor, 0 for none) and final_T [H,W].  Records of gaussians with
+ * radius 0 are not written by the forward and hold whatever the workspace held.  The records sit at the same offsets in
+ * the workspaces of a3d_raster_forward and a3d_raster_forward_rgba8 (checked here); n_contrib / final_T exist only in
+ * a3d_raster_forward's workspace, so with an RGBA8 workspace they must be NULL.  Any NULL output is skipped. */
+int a3d_raster_state_tap(const void* workspace, int P, int H, int W, int num_cams, int64_t max_rendered, int cam, float* xy_out,
+                         float* conic_opac_out, float* rgb_depth_out, uint8_t* clamped_out, uint32_t* n_contrib_out,
+                         float* final_T_out, void* stream);
 
 /* ---------------------------------------------------------------- 4D deformation field (k-planes + MLPs) --------- */
 /* Per (frame, gaussian): 32 k-planes features (num_scales x 16 channels, product over the 6 coordinate planes of

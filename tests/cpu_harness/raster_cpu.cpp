@@ -24,17 +24,22 @@ static std::vector<float> gaussian_colours(int P, const float* means, const floa
 
 extern "C" {
 
-// colors: precomputed rgb [P,3], or nullptr for SH colours (shs, sh_degree, sh_coeffs, campos).  Returns number of
-// (tile, gaussian) pairs.
+// colors: precomputed rgb [P,3], or nullptr for SH colours (shs, sh_degree, sh_coeffs, campos).  Optional outputs: the
+// records the kernel's render reads (pre_dump [P,8]: depth, px, py, conic a, b, c, tiles, radius; rgb_out [P,3];
+// clamped_out [P]) and the RGBA8 bytes of a3d_raster_forward_rgba8 (rgba_out [H,W,4]).  Returns number of (tile, gaussian)
+// pairs.
 long raster_cpu_forward(int P, const float* means, const float* scales, const float* rots, const float* opac, const float* colors,
                         const float* shs, int sh_degree, int sh_coeffs, const float* campos,
                         const float* vm, const float* pm, float tanfovx, float tanfovy, int H, int W, const float* bg, float mod,
                         float* out_color, float* out_depth, float* out_alpha, int* radii, int* n_contrib, float* final_T,
-                        unsigned long long* keys, unsigned int* vals, long cap, long long* ranges, float* pre_dump) {
+                        unsigned long long* keys, unsigned int* vals, long cap, long long* ranges, float* pre_dump,
+                        float* rgb_out, unsigned char* clamped_out, unsigned char* rgba_out) {
   const int gx = (W + kTile - 1) / kTile, gy = (H + kTile - 1) / kTile;
   std::vector<uint32_t> clamped;
   const std::vector<float> col = gaussian_colours(P, means, colors, shs, sh_degree, sh_coeffs, campos, clamped);
   colors = col.data();
+  if (rgb_out) std::memcpy(rgb_out, col.data(), col.size() * sizeof(float));
+  if (clamped_out) for (int i = 0; i < P; ++i) clamped_out[i] = (unsigned char)clamped[i];
   std::vector<PreGauss> pre(P);
   std::vector<std::pair<unsigned long long, unsigned int>> kv;
   for (int i = 0; i < P; ++i) {
@@ -84,6 +89,10 @@ long raster_cpu_forward(int P, const float* means, const float* scales, const fl
       const long pix = (long)py * W + px;
       for (int ch = 0; ch < 3; ++ch) out_color[(long)ch * H * W + pix] = C[ch] + T * bg[ch];
       out_depth[pix] = D; out_alpha[pix] = A; n_contrib[pix] = last; final_T[pix] = T;
+      if (rgba_out) {
+        for (int ch = 0; ch < 3; ++ch) rgba_out[4 * pix + ch] = quantise_u8(clamp01(C[ch] + T * bg[ch]));
+        rgba_out[4 * pix + 3] = quantise_u8(A);
+      }
     }
   return R;
 }

@@ -212,16 +212,24 @@ def cuda_run(geo, o, sh, col, deg, per_cam, cams, H, W, bg, mod, grads, determin
         else:
             leaves["colors"] = col.cuda().requires_grad_(True)
         leaves["means2D"] = torch.zeros(len(cams), o.shape[0], 3, device="cuda", requires_grad=True)
+        settings = _settings(cams, H, W, bg, deg, mod)
         color, radii, depth, alpha = RZ.rasterize_batch(leaves["means3D"], leaves["scales"], leaves["rotations"], leaves["opacity"],
-                                                        leaves.get("shs"), leaves.get("colors"), _settings(cams, H, W, bg, deg, mod),
+                                                        leaves.get("shs"), leaves.get("colors"), settings,
                                                         per_cam_geometry=per_cam, means2D=leaves["means2D"])
+        # the forward, element by element, from the workspace the backward is about to read
+        from test_raster_forward_oracle_gpu import check_saved
+        node = color.grad_fn
+        forward = check_saved(node.saved_tensors[-1], node.meta[1],
+                              [leaves[k] if k in leaves else None for k in ("means3D", "scales", "rotations", "opacity", "shs", "colors")],
+                              deg, per_cam, settings, dict(color=color.detach(), depth=depth.detach(), alpha=alpha.detach()), radii,
+                              mod, name=f"deterministic={int(deterministic)}")
         dC, dD, dA = grads
         ((color * dC.cuda()).sum() + (depth * dD.cuda()).sum() + (alpha * dA.cuda()).sum()).backward()
         torch.cuda.synchronize()
     finally:
         torch.use_deterministic_algorithms(prev)
     return dict(grads={k: t.grad.cpu() for k, t in leaves.items()}, radii=radii.cpu(), color=color.detach().cpu(),
-                depth=depth.detach().cpu(), alpha=alpha.detach().cpu())
+                depth=depth.detach().cpu(), alpha=alpha.detach().cpu(), forward=forward)
 
 
 # ------------------------------------------------------------------------------------------------ comparison
@@ -264,13 +272,9 @@ def compare_grads(name, mine, ora, per_cam, tau=TAU):
 
 
 def compare_images(name, mine, ora):
+    """radii equal to the fp32 oracle's; the images were checked element by element in cuda_run (check_saved)"""
     assert torch.equal(mine["radii"], ora["radii"]), f"{name}: radii"
-    for k in ("color", "depth", "alpha"):
-        for c in range(len(ora[k])):
-            got, ref = mine[k][c], ora[k][c]
-            bad = ((got - ref).abs() > 3e-5 + 1e-4 * ref.abs())
-            assert bad.sum().item() <= 8, f"{name} cam {c} {k}: {bad.sum().item()} pixels off"
-            assert (got - ref).abs().max().item() < 5e-3, f"{name} cam {c} {k}: max err {(got - ref).abs().max().item()}"
+    assert mine["forward"]["color"] <= 1.0 and mine["forward"]["n_contrib"] == 0.0
 
 
 def loss_grads(ncam, H, W, seed):

@@ -47,10 +47,16 @@ def run_harness(lib, xyz, s, q, o, col, wv, full, tf, H, W, bg, grads=None, sh=N
     cap = P * gx * gy
     keys = np.zeros(cap, np.uint64); vals = np.zeros(cap, np.uint32); ranges = np.zeros((gx * gy, 2), np.int64)
     pre = np.zeros((P, 8), np.float32)
+    rgb = np.zeros((P, 3), np.float32); clamped = np.zeros(P, np.uint8); rgba = np.zeros((H, W, 4), np.uint8)
     n = lib.raster_cpu_forward(P, fp(xyz_), fp(s_), fp(q_), fp(o_), opt(col_), opt(sh_), deg, K, opt(cp_), fp(wv_), fp(full_),
                                C.c_float(tf), C.c_float(tf), H, W, fp(bg_), C.c_float(mod), fp(color), fp(depth), fp(alpha), fp(radii), fp(ncon), fp(fT), fp(keys),
-                               fp(vals), C.c_long(cap), fp(ranges), fp(pre))
-    res = dict(color=color, depth=depth, alpha=alpha, radii=radii, ncon=ncon, fT=fT, keys=keys[:n], vals=vals[:n], ranges=ranges, pre=pre)
+                               fp(vals), C.c_long(cap), fp(ranges), fp(pre), fp(rgb), fp(clamped), fp(rgba))
+    res = dict(color=color, depth=depth, alpha=alpha, radii=radii, ncon=ncon, fT=fT, keys=keys[:n], vals=vals[:n], ranges=ranges, pre=pre,
+               rgba=rgba)
+    t = torch.from_numpy
+    # the records the render reads, laid out as a3d_raster_state_tap returns them (one camera)
+    res["rec"] = dict(xy=t(pre[None, :, 1:3].copy()), conic_opac=t(np.concatenate([pre[:, 3:6], o_.reshape(P, 1)], 1)[None]),
+                      rgb_depth=t(np.concatenate([rgb, pre[:, 0:1]], 1)[None]), clamped=t(clamped[None]))
     if grads is not None:
         dC, dD, dA = [np.ascontiguousarray(g.numpy().astype(np.float32)) for g in grads]
         gm = np.zeros((P, 3), np.float32); gs = np.zeros((P, 3), np.float32); gr = np.zeros((P, 4), np.float32)
@@ -78,10 +84,26 @@ def test_forward_indices_bit_exact_and_image_close(harness, P, H, W, seed):
     assert np.array_equal(got["vals"].astype(np.int64), ora["point_list"])
     assert np.array_equal(got["ranges"], ora["ranges"])
     assert len(got["keys"]) > P // 2
-    np.testing.assert_allclose(got["color"], ora["color"].numpy(), rtol=1e-4, atol=2e-5)
-    np.testing.assert_allclose(got["depth"], ora["depth"][0].numpy(), rtol=1e-4, atol=2e-5)
-    np.testing.assert_allclose(got["alpha"], ora["alpha"][0].numpy(), rtol=1e-4, atol=2e-5)
     assert np.array_equal(got["ncon"], ora["n_contrib"].numpy().astype(np.int32))
+    # every record, plane and byte within the float64 oracle's per-element bound
+    check_harness(got, (xyz, s, q, o, None, col, 0), (wv, full, cp, tf), H, W, bg)
+
+
+def check_harness(got, scene, cam, H, W, bg, mod=1.0, max_excluded=None):
+    """The harness's records, planes, n_contrib, final_T and bytes against oracle/raster_abi_oracle.py."""
+    from oracle import raster_abi_oracle as RA
+    xyz, s, q, o, sh, col, deg = scene
+    wv, full, cp, tf = cam
+    spec = [RA.CamSpec(wv, full, cp, RA.f32c(tf), RA.f32c(tf))]
+    rep = RA.check_records(xyz, s, q, o, sh, col, deg, False, spec, H, W, mod, got["rec"], torch.from_numpy(got["radii"])[None])
+    ora = RA.render(got["rec"], got["vals"], got["ranges"], H, W, bg)
+    planes = dict(color=torch.from_numpy(got["color"])[None], depth=torch.from_numpy(got["depth"])[None],
+                  alpha=torch.from_numpy(got["alpha"])[None], n_contrib=torch.from_numpy(got["ncon"])[None],
+                  final_T=torch.from_numpy(got["fT"])[None])
+    rep.update(RA.compare_forward(planes, ora, RA.MAX_EXCLUDED if max_excluded is None else max_excluded, "harness",
+                                  rgba=torch.from_numpy(got["rgba"])[None]))
+    rep.update(ora["stats"])
+    return rep
 
 
 @pytest.mark.parametrize("P,H,W,seed", [(200, 32, 48, 3), (600, 48, 48, 4)])
