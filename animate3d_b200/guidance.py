@@ -13,10 +13,12 @@ remaining arithmetic is a handful of elementwise/reduction ops on [B*Nv*F, 4, 32
 autograd tape (the loss's gradient flows to `latents` and from there through the VAE encoder to the rasterizer), so they
 are torch ops.
 
-Differences from the reference class, all at construction time (there are no Hugging Face checkpoints to load here):
-`configure()` accepts the already-built components (`unet`, `vae`, `ip_image_processor`, `scheduler`) as keyword arguments;
-with none given it builds the engine UNet from `cfg.model_config` and loads `cfg.pretrained_unet_path` through
-`weights.load_unet_checkpoint` (inference.py:213-223 semantics)."""
+Differences from the reference class, all at construction time: `configure()` accepts the already-built components
+(`unet`, `vae`, `ip_image_processor`, `scheduler`) as keyword arguments.  Those not given are built on the engine from
+`cfg.pretrained_model_name_or_path`, `motion_adapter_path`, `ip_adapter_path` and `pretrained_unet_path` as
+animatemv_guidance.py:115-160 does, from local files only (directories or the hub cache, `pretrained.resolve`).  With no
+`pretrained_model_name_or_path` the UNet is built from `cfg.model_config` and `cfg.pretrained_unet_path` is loaded through
+`weights.load_unet_checkpoint` (inference.py:213-223 semantics); that file alone does not hold the base weights."""
 from __future__ import annotations
 
 import os
@@ -117,6 +119,8 @@ class AnimateMVDiffusionGuidance(BaseObject):
         if not cfg.recon_loss:
             raise NotImplementedError("only the x0-reconstruction loss path exists in the reference (recon_loss=True)")
         self.weights_dtype = torch.float16 if cfg.half_precision_weights else torch.float32
+        if cfg.pretrained_model_name_or_path:
+            unet, vae, ip_image_processor = self._load_pretrained(unet, vae, ip_image_processor)
         if unet is None:
             from .unet import MVUNetMotionModel
             from .unet_config import UNetConfig
@@ -138,6 +142,28 @@ class AnimateMVDiffusionGuidance(BaseObject):
         self.alphas = torch.from_numpy(self.scheduler.alphas_cumprod).to(self.device)
         self.set_min_max_steps()                                            # defaults (0.02, 0.98) until update_step
         self.grad_clip_val: Optional[float] = None
+
+    def _load_pretrained(self, unet, vae, ip_image_processor):
+        """animatemv_guidance.py:121-146 on the engine, for whichever of the three components was not injected: the UNet
+        through `MVUNetMotionModel.from_pretrained` (the three path fields, `pretrained_unet_path`, `model_config`,
+        n_view x n_frame wiring), the VAE from `<pretrained_model_name_or_path>/vae`, and the IP-Adapter image processor
+        over the engine's CLIP tower from `<ip_adapter_path>/models/image_encoder`.  Local files only."""
+        cfg = self.cfg
+        if unet is None:
+            from .unet import MVUNetMotionModel
+            unet = MVUNetMotionModel.from_pretrained(cfg.pretrained_model_name_or_path, cfg.motion_adapter_path,
+                                                     cfg.ip_adapter_path, cfg.pretrained_unet_path, cfg.model_config,
+                                                     device=self.device, num_views=cfg.n_view, num_frames=cfg.n_frame)
+        if vae is None:
+            from .vae import AutoencoderKL
+            vae = AutoencoderKL.from_pretrained(cfg.pretrained_model_name_or_path, subfolder="vae", device=self.device)
+        if ip_image_processor is None and cfg.ip_adapter_path:
+            from . import pretrained as PT
+            from .clip import CLIPImageProcessor, CLIPVisionModelWithProjection, IPAdapterImageProcessor
+            tower = CLIPVisionModelWithProjection.from_pretrained(PT.resolve(cfg.ip_adapter_path, "models/image_encoder"),
+                                                                  device=self.device)
+            ip_image_processor = IPAdapterImageProcessor(CLIPImageProcessor(device=self.device), tower)
+        return unet, vae, ip_image_processor
 
     # ---------------------------------------------------------------------------------------------- small helpers
     def set_min_max_steps(self, min_step_percent: float = 0.02, max_step_percent: float = 0.98):

@@ -521,3 +521,47 @@ class AnimateDiffMVI2VPipeline:
 
 
 AnimationPipeline = AnimateDiffMVI2VPipeline   # name used by BASELINE.json's north_star
+
+
+def read_yaml(config) -> dict:
+    """A parsed config (returned as a plain dict) or the path of a YAML file, read with PyYAML (the inference configs use
+    no OmegaConf interpolation)."""
+    if isinstance(config, dict):
+        return dict(config)
+    import yaml
+    with open(config) as f:
+        return yaml.safe_load(f)
+
+
+def load_pipeline(config, pretrained_unet_path: Optional[str], device: str = "cuda", num_views: int = 4,
+                  num_frames: int = 16) -> AnimateDiffMVI2VPipeline:
+    """The sampling pipeline of inference.py:60-245 from the files `config` (configs/inference/inference.yaml, parsed or a
+    path) names: DDIMScheduler(**noise_scheduler_kwargs); transformers' CLIPTokenizer and CLIPTextModel from
+    `<pretrained_model_path>/tokenizer` and `/text_encoder` (local files only); the engine's VAE from `/vae`, UNet
+    (`MVUNetMotionModel.from_pretrained` with the motion adapter, IP-Adapter and `pretrained_unet_path`) and IP-Adapter
+    image tower from `<ip_adapter_path>/models/image_encoder` behind a `CLIPImageProcessor`; FreeInit (butterworth, no fast
+    sampling) when `freeinit_enabled`.  num_views / num_frames wire the UNet's attention processors, as inference.py's
+    --N / --L do."""
+    from transformers import CLIPTextModel, CLIPTokenizer
+
+    from . import pretrained as PT
+    from .clip import CLIPImageProcessor, CLIPVisionModelWithProjection
+    from .vae import AutoencoderKL
+    cfg = read_yaml(config)
+    base, ip = cfg["pretrained_model_path"], cfg.get("ip_adapter_path")
+    scheduler = DDIMScheduler(**(cfg.get("noise_scheduler_kwargs") or {}))
+    tokenizer = CLIPTokenizer.from_pretrained(PT.resolve(base, "tokenizer"), local_files_only=True)
+    text_encoder = CLIPTextModel.from_pretrained(PT.resolve(base, "text_encoder"), local_files_only=True).to(device).eval()
+    vae = AutoencoderKL.from_pretrained(base, subfolder="vae", device=device)
+    model_config = {k: cfg[k] for k in ("mvdream_attn_cfg", "motion_module_attn_cfg", "i2v_cond_time_zero") if k in cfg}
+    unet = MVUNetMotionModel.from_pretrained(base, cfg.get("motion_adapter_path"), ip, pretrained_unet_path, model_config,
+                                             device=device, num_views=num_views, num_frames=num_frames)
+    image_encoder = feature_extractor = None
+    if ip:
+        image_encoder = CLIPVisionModelWithProjection.from_pretrained(PT.resolve(ip, "models/image_encoder"), device=device)
+        feature_extractor = CLIPImageProcessor(device=device)
+    pipe = AnimateDiffMVI2VPipeline(vae=vae, text_encoder=text_encoder, tokenizer=tokenizer, unet=unet, scheduler=scheduler,
+                                    feature_extractor=feature_extractor, image_encoder=image_encoder)
+    if cfg.get("freeinit_enabled"):
+        pipe.enable_free_init(method="butterworth", num_iters=cfg.get("freeinit_num_iters", 3), use_fast_sampling=False)
+    return pipe

@@ -187,6 +187,42 @@ class MVUNetMotionModel(torch.nn.Module):
                 model._loaded.add(k)
         return model
 
+    @classmethod
+    def from_pretrained(cls, pretrained_model_path: str, motion_adapter_path: Optional[str], ip_adapter_path: Optional[str] = None,
+                        pretrained_unet_path: Optional[str] = None, model_config: Optional[dict] = None, device: str = "cuda",
+                        **kwargs):
+        """The released model from its published files, in the order of inference.py:63-223: `<pretrained_model_path>/unet`
+        and the motion adapter through `from_unet2d`, `<ip_adapter_path>/models/ip-adapter_sd15.bin` (or its .safetensors
+        twin) through `_load_ip_adapter_weights`, then the motion-module checkpoint through `weights.load_unet_checkpoint`
+        (0 or 726 keys missing).  Paths are directories or hub ids already in the hub cache (`pretrained.resolve`; nothing
+        is downloaded).  The IP-Adapter's image-embedding width and token count are read off its projection, as diffusers
+        does.  kwargs override the UNetConfig (num_views, num_frames, ...).
+
+        Raises NotImplementedError for a `model_config` (inference.yaml's attention blocks) other than the released
+        wiring, and ValueError listing the first keys of the model that no file provided."""
+        from . import pretrained as PT
+        from .weights import load_unet_checkpoint
+        PT.check_model_config(model_config)
+        unet2d = PT.load_model(pretrained_model_path, "unet")
+        adapter = PT.load_model(motion_adapter_path) if motion_adapter_path else None
+        ip_sd = PT.load_ip_adapter(PT.ip_adapter_file(ip_adapter_path)) if ip_adapter_path else None
+        if ip_sd is not None:
+            proj = ip_sd["image_proj"]["proj.weight"]
+            cross = unet2d.config.get("cross_attention_dim", 768)
+            kwargs.setdefault("ip_image_embed_dim", proj.shape[1])
+            kwargs.setdefault("ip_num_tokens", proj.shape[0] // cross)
+        model = cls.from_unet2d(unet2d, adapter, device=device, **kwargs)
+        if ip_sd is not None:
+            model._load_ip_adapter_weights(ip_sd)
+        if pretrained_unet_path:
+            load_unet_checkpoint(model, pretrained_unet_path)
+        miss = [k for k in key_plan(model.cfg) if k not in model._loaded]
+        if miss:
+            raise ValueError(f"{len(miss)} weights of the model were in none of the files (unet {unet2d.path}, motion adapter "
+                             f"{motion_adapter_path}, IP-Adapter {ip_adapter_path}, checkpoint {pretrained_unet_path}), "
+                             f"e.g. {miss[:5]}")
+        return model
+
     def _load_ip_adapter_weights(self, state_dict):
         """diffusers' loader hook used by animatediff/utils/util.py::load_ip_adapter: {"image_proj": {...}, "ip_adapter": {...}}
         -> encoder_hid_proj.image_projection_layers.0.* and the 16 attn2 processors' to_k_ip / to_v_ip."""

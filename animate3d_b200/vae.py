@@ -263,6 +263,24 @@ class AutoencoderKL(torch.nn.Module):
     def enable_slicing(self):
         pass
 
+    @classmethod
+    def from_pretrained(cls, path: str, subfolder: Optional[str] = "vae", device: str = "cuda"):
+        """diffusers' AutoencoderKL.from_pretrained from local files: `config.json` (geometry and scaling_factor) and
+        `diffusion_pytorch_model.safetensors` (or `.bin`) under `<path>/<subfolder>`; `path` is a directory or a hub id
+        already in the hub cache (`pretrained.resolve`)."""
+        from . import pretrained as PT
+        directory = PT.resolve(path, subfolder)
+        c = PT.read_config(directory)
+        kinds = set(c.get("down_block_types", ["DownEncoderBlock2D"])) | set(c.get("up_block_types", ["UpDecoderBlock2D"]))
+        if kinds != {"DownEncoderBlock2D", "UpDecoderBlock2D"} or c.get("act_fn", "silu") != "silu":
+            raise NotImplementedError(f"{directory}: only the SD VAE (DownEncoderBlock2D / UpDecoderBlock2D, SiLU) is "
+                                      f"implemented, got blocks {sorted(kinds)}, act_fn {c.get('act_fn')!r}")
+        keys = ("in_channels", "out_channels", "latent_channels", "block_out_channels", "layers_per_block", "norm_num_groups",
+                "scaling_factor", "sample_size")
+        vae = cls(**{k: c[k] for k in keys if k in c}, device=device)
+        vae.load_state_dict(PT.load_weights(directory))
+        return vae
+
     # ------------------------------------------------------------------------------------------------ weights
     def load_state_dict(self, sd: Dict[str, torch.Tensor], strict: bool = True, assign: bool = False):
         """diffusers key names; returns (missing_keys, unexpected_keys).  The weights are repacked into the kernels' operand
